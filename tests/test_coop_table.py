@@ -77,7 +77,10 @@ def _walk(gf, lanes, tables, rb):
 
 
 @pytest.mark.parametrize("fixture,degree,order,lanes", [("jgm3_70x70", 21, 21, 8), ("jgm3_70x70", 21, 21, 16), ("jgm3_70x70", 8, 5, 8),
-                                                          ("jgm3_70x70", 70, 70, 32), ("jgm3_70x70", 30, 30, 32), ("luna_jggrx_80x80", 48, 48, 16)])
+                                                          ("jgm3_70x70", 70, 70, 32), ("jgm3_70x70", 30, 30, 32), ("luna_jggrx_80x80", 48, 48, 16),
+                                                          ("jgm3_70x70", 8, 0, 8), ("jgm3_70x70", 8, 1, 8), ("jgm3_70x70", 8, 0, 32),
+                                                          ("jgm3_70x70", 29, 29, 8), ("jgm3_70x70", 30, 30, 16), ("jgm3_70x70", 40, 40, 16),
+                                                          ("jgm3_70x70", 41, 41, 16), ("jgm3_70x70", 47, 47, 16), ("jgm3_70x70", 48, 48, 32)])
 def test_cooperative_table_reproduces_oracle_gravity(oracle, fixture, degree, order, lanes):
     """The schedule is the bin packing with aligned column starts (columns reordered / idle gaps inserted so that lane positions
     start columns on common entries)."""

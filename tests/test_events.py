@@ -202,18 +202,24 @@ def test_gpu_event_locate_matches_host_brent(oracle):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("mode,lanes", [(nb.MODE_STRICT, 1), (nb.MODE_STRICT, 8), (nb.MODE_FAST, 1), (nb.MODE_FAST, 8), (nb.MODE_FAST, 32)])
+@pytest.mark.parametrize("mode,lanes", [(nb.MODE_STRICT, 1), (nb.MODE_STRICT, 8), (nb.MODE_FAST, 1), (nb.MODE_FAST, 8), (nb.MODE_FAST, 32),
+                                        (nb.MODE_FAST, "tx")])
 @pytest.mark.parametrize("kind", ["apsis", "node", "radius"])
 def test_gpu_event_stop_matches_oracle(oracle, mode, lanes, kind):
+    """lanes = "tx": the transposed kernel."""
     frame = nb.EARTH_J2000
     n = 48
     mc, (st, cs, ep) = leo_ensemble(n, seed=17)
     ev = {"apsis": Event.apsis(), "node": Event.node(), "radius": Event.radius(6679.5)}[kind]
     prop = nb.Propagator.default(_dyn(48 if lanes == 32 else 21), mode=mode)
     eng = prop.engine(frame, None)
-    eng.set_lanes(lanes)
+    if lanes == "tx":
+        eng.set_kernel(nb.KERNEL_TRANSPOSED)
+    else:
+        eng.set_lanes(lanes)
     end = 5 * 3600 * S
     out, out_ep, det, status, (g_ep, g_st, g_cnt), g_cross = eng.propagate_batch(st, cs, ep, end, traj_capacity=256, event=(ev.kind, ev.value, 2))
+    assert eng.last_kernel() == (nb.KERNEL_TRANSPOSED if lanes == "tx" else nb.KERNEL_THREAD if lanes == 1 else nb.KERNEL_COOP)
     ref, ref_ep, ref_det, ref_status, (o_ep, o_st, o_cnt), o_cross = _oracle_event(oracle, prop, frame, st, cs, ep, end, 256, ev, 2)
     assert np.array_equal(g_cnt, det["n_steps"] + 1)
     if mode == nb.MODE_STRICT:

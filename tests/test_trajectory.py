@@ -80,17 +80,23 @@ def test_traj_finalize_sorts_back_propagation(oracle):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("mode,lanes", [(nb.MODE_STRICT, 1), (nb.MODE_STRICT, 8), (nb.MODE_FAST, 1), (nb.MODE_FAST, 8), (nb.MODE_FAST, 16)])
+@pytest.mark.parametrize("mode,lanes", [(nb.MODE_STRICT, 1), (nb.MODE_STRICT, 8), (nb.MODE_FAST, 1), (nb.MODE_FAST, 8), (nb.MODE_FAST, 16),
+                                        (nb.MODE_FAST, "tx")])
 def test_gpu_recording_matches_oracle(oracle, mode, lanes):
-    """Every kernel writes the same step-major SoA stream the oracle records: bit-identical in STRICT mode."""
+    """Every kernel writes the same step-major SoA stream the oracle records: bit-identical in STRICT mode.  lanes = "tx": the
+    transposed kernel."""
     frame = nb.EARTH_J2000
     mc, (st, cs, ep) = leo_ensemble(40, seed=42)
     ep = ep + (np.arange(40, dtype=np.int64) % 3) * 900 * S
     prop = nb.Propagator.default(_dyn(21), mode=mode)
     eng = prop.engine(frame, None)
-    eng.set_lanes(lanes)
+    if lanes == "tx":
+        eng.set_kernel(nb.KERNEL_TRANSPOSED)
+    else:
+        eng.set_lanes(lanes)
     end = 2 * 3600 * S
     out, out_ep, det, status, (g_ep, g_st, g_cnt) = eng.propagate_batch(st, cs, ep, end, traj_capacity=128)
+    assert eng.last_kernel() == (nb.KERNEL_TRANSPOSED if lanes == "tx" else nb.KERNEL_THREAD if lanes == 1 else nb.KERNEL_COOP)
     ref, ref_ep, ref_det, ref_status, (o_ep, o_st, o_cnt) = _oracle_traj(oracle, prop, frame, st, cs, ep, end, 128)
     assert (status == 0).all() and np.array_equal(g_cnt, det["n_steps"] + 1)
     if mode == nb.MODE_STRICT:

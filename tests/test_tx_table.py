@@ -76,7 +76,9 @@ def _walk(gf, P, tables, rb):
 
 @pytest.mark.parametrize("fixture,degree,order,P", [("jgm3_70x70", 21, 21, 8), ("jgm3_70x70", 21, 21, 10), ("jgm3_70x70", 8, 5, 8), ("jgm3_70x70", 12, 12, 8),
                                                       ("jgm3_70x70", 40, 40, 8), ("jgm3_70x70", 70, 70, 16), ("luna_jggrx_80x80", 48, 48, 16),
-                                                      ("jgm3_70x70", 33, 20, 16)])
+                                                      ("jgm3_70x70", 33, 20, 16), ("jgm3_70x70", 8, 0, 8), ("jgm3_70x70", 8, 1, 8),
+                                                      ("jgm3_70x70", 8, 0, 16), ("jgm3_70x70", 40, 40, 16), ("jgm3_70x70", 41, 41, 16),
+                                                      ("jgm3_70x70", 41, 41, 8), ("jgm3_70x70", 30, 30, 10), ("jgm3_70x70", 48, 48, 16)])
 def test_transposed_table_reproduces_oracle_gravity(oracle, fixture, degree, order, P):
     moon = fixture.startswith("luna")
     body_frame = nb.IAU_MOON_FRAME if moon else nb.IAU_EARTH_FRAME
