@@ -504,6 +504,8 @@ int32_t nyxb_ziggurat_tables(double* x257, double* f257);                       
 enum nyxb_kernel { NYXB_KERNEL_AUTO = 0, NYXB_KERNEL_THREAD = 1, NYXB_KERNEL_COOP = 2, NYXB_KERNEL_TRANSPOSED = 3 };
 int32_t nyxb_engine_set_kernel(nyxb_engine* eng, int32_t kernel);          /* enum nyxb_kernel; NYXB_RC_UNSUPPORTED if the setup cannot use it */
 int32_t nyxb_engine_last_kernel(const nyxb_engine* eng);                   /* family used by the last propagation launch */
+/* nyxb_propagate_batch_stm sets it to THREAD (one thread per trajectory, STRICT and FAST).  nyxb_od_ekf_batch sets it to COOP
+ * when it ran the warp-cooperative filter (FAST, field of degree >= 8, kernel not forced to THREAD), else to THREAD. */
 /* TRANSPOSED kernel: step attempts per time slice (default 64) and an upper bound on the persistent CTAs (0 = SMs x occupancy).
  * Sets are only parked when there are more sets than CTAs. */
 int32_t nyxb_engine_set_tx_tuning(nyxb_engine* eng, int32_t slice_attempts, int32_t max_ctas);

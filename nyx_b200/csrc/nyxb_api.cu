@@ -847,6 +847,7 @@ extern "C" int32_t nyxb_propagate_batch_stm(nyxb_engine* eng, size_t n, const do
         : nyxb_launch_stm_fast(&eng->S, n, d_state, d_consts, d_ep, end_epoch_ns, d_step, d_stm_in, d_out, d_oep, d_stm, d_det, d_status, st);
     if (err != cudaSuccess) { set_err(std::string("kernel launch: ") + cudaGetErrorString(err)); return NYXB_RC_CUDA; }
     eng->launches += 1;
+    eng->last_kernel = NYXB_KERNEL_THREAD;
     CUDA_TRY(cudaEventRecord(eng->ev1, st));
     CUDA_TRY(cudaMemcpyAsync(out_state_soa, d_out, sizeof(double) * 9 * n, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(out_stm_soa, d_stm, sizeof(double) * 81 * n, cudaMemcpyDeviceToHost, st));
@@ -972,6 +973,7 @@ extern "C" int32_t nyxb_od_ekf_batch(nyxb_engine* eng, const nyxb_od_config* cfg
             : nyxb_launch_od_fast(&eng->S, &od, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st);
     if (err != cudaSuccess) { set_err(std::string("kernel launch: ") + cudaGetErrorString(err)); return NYXB_RC_CUDA; }
     eng->launches += 1;
+    eng->last_kernel = coop ? NYXB_KERNEL_COOP : NYXB_KERNEL_THREAD;
     CUDA_TRY(cudaEventRecord(eng->ev1, st));
     CUDA_TRY(cudaMemcpyAsync(out->state_soa, d_out, sizeof(double) * 9 * n, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(out->epoch_ns, d_oep, sizeof(long long) * n, cudaMemcpyDeviceToHost, st));
