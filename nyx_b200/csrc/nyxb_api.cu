@@ -547,9 +547,7 @@ static int32_t launch_inner(nyxb_engine* e, size_t n, const double* state, const
     } else if (lanes > 1) {
         const DevCoop* cp = get_coop(e, lanes);
         if (!cp) { set_err("cooperative table upload failed"); return NYXB_RC_CUDA; }
-        // one trajectory per lane group: register blocking over two trajectories (T = 2) was measured slower at every ensemble
-        // size and is not dispatched
-        err = nyxb_launch_coop(&e->S, cp, 1, n, state, consts, (const long long*)epoch0, end_epoch, (long long*)step_io,
+        err = nyxb_launch_coop(&e->S, cp, n, state, consts, (const long long*)epoch0, end_epoch, (long long*)step_io,
                                out_state, (long long*)out_epoch, out_details, out_status, &sink, stream);
     } else if (e->mode == NYXB_MODE_STRICT) {
         err = nyxb_launch_thread_strict(&e->S, n, state, consts, (const long long*)epoch0, end_epoch, (long long*)step_io,

@@ -1,6 +1,6 @@
 // nyxb_coop.cu — host side of the lane-cooperative kernel (nyxb_coop_kernel.cuh): column -> lane schedule,
 // record table, dispatch on the lane count.  Kernel summary: G lanes of one warp integrate
-// ONE (or two) trajectories.  The spherical-harmonic double sum (gravity_field.rs:217-249), which is >98 % of
+// one trajectory.  The spherical-harmonic double sum (gravity_field.rs:217-249), which is >98 % of
 // the arithmetic for a 21x21 field, is split across the lanes by COLUMNS of the derived-Legendre
 // triangle: every A[n][m] is produced by its own column recursion (gravity_field.rs:175-181) in a
 // register, and the four partial sums are regrouped so that each A[n][m] is consumed exactly once,
@@ -200,22 +200,21 @@ void nyxb_coop_build_host(int N, int M, const double* c_nm, const double* s_nm, 
 // dispatch: one translation unit per lane count (nyxb_coop_g{8,16,32}.cu) so that they build in parallel
 // ------------------------------------------------------------------------------------------------
 #define NYXB_COOP_DECL(G) \
-    cudaError_t nyxb_launch_coop_g##G(const DevSetup*, const DevCoop*, int, size_t, const double*, const double*, const long long*, \
+    cudaError_t nyxb_launch_coop_g##G(const DevSetup*, const DevCoop*, size_t, const double*, const double*, const long long*, \
                                       long long, long long*, double*, long long*, nyxb_details*, int*, const DevSink*, cudaStream_t);
 NYXB_COOP_DECL(8)
 NYXB_COOP_DECL(16)
 NYXB_COOP_DECL(32)
 
-extern "C" cudaError_t nyxb_launch_coop(const DevSetup* S, const DevCoop* Cp, int T, size_t n, const double* state,
+extern "C" cudaError_t nyxb_launch_coop(const DevSetup* S, const DevCoop* Cp, size_t n, const double* state,
                                         const double* consts, const long long* epoch0, long long end_epoch,
                                         long long* step_io, double* out_state, long long* out_epoch,
                                         nyxb_details* out_details, int* out_status, const DevSink* sink, cudaStream_t stream) {
     if (n == 0) return cudaSuccess;
-    if (T != 1) return cudaErrorInvalidValue;
     switch (Cp->G) {
-    case 8: return nyxb_launch_coop_g8(S, Cp, T, n, state, consts, epoch0, end_epoch, step_io, out_state, out_epoch, out_details, out_status, sink, stream);
-    case 16: return nyxb_launch_coop_g16(S, Cp, T, n, state, consts, epoch0, end_epoch, step_io, out_state, out_epoch, out_details, out_status, sink, stream);
-    case 32: return nyxb_launch_coop_g32(S, Cp, T, n, state, consts, epoch0, end_epoch, step_io, out_state, out_epoch, out_details, out_status, sink, stream);
+    case 8: return nyxb_launch_coop_g8(S, Cp, n, state, consts, epoch0, end_epoch, step_io, out_state, out_epoch, out_details, out_status, sink, stream);
+    case 16: return nyxb_launch_coop_g16(S, Cp, n, state, consts, epoch0, end_epoch, step_io, out_state, out_epoch, out_details, out_status, sink, stream);
+    case 32: return nyxb_launch_coop_g32(S, Cp, n, state, consts, epoch0, end_epoch, step_io, out_state, out_epoch, out_details, out_status, sink, stream);
     default: return cudaErrorInvalidValue;
     }
 }

@@ -52,8 +52,8 @@ extern "C" cudaError_t nyxb_launch_coop_strict(const DevSetup* S, const DevCoopS
 
 void nyxb_coop_build_host(int N, int M, const double* c_nm, const double* s_nm, int G, CoopHost& out);
 
-// T = trajectories integrated together by one lane group (1 or 2: register blocking over the coefficient records)
-extern "C" cudaError_t nyxb_launch_coop(const DevSetup* S, const DevCoop* Cp, int T, size_t n, const double* state,
+// one trajectory per group of Cp->G lanes
+extern "C" cudaError_t nyxb_launch_coop(const DevSetup* S, const DevCoop* Cp, size_t n, const double* state,
                                         const double* consts, const long long* epoch0, long long end_epoch,
                                         long long* step_io, double* out_state, long long* out_epoch,
                                         nyxb_details* out_details, int* out_status, const DevSink* sink, cudaStream_t stream);

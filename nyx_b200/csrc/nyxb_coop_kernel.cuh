@@ -1,6 +1,6 @@
 // nyxb_coop_kernel.cuh — lane-cooperative, register-blocked propagation kernel (FAST mode).
 //
-//   * G lanes of one warp integrate T trajectories together (T = 1 or 2).  The spherical-harmonic
+//   * G lanes of one warp integrate one trajectory together.  The spherical-harmonic
 //     double sum (gravity_field.rs:217-249; >98 % of the arithmetic for a 21x21 field) is split across
 //     the lanes by COLUMNS of the derived-Legendre triangle: every A[n][m] is produced by its own column
 //     recursion (gravity_field.rs:175-181) in a register, and the four partial sums are regrouped so that
@@ -13,11 +13,11 @@
 //     compressed to 40 bytes: the column recursion runs on the un-normalised Q[n][m] = (n-m)! d^m P_n/du^m whose
 //     coefficients (2n+1), (n+m)(n-m) are generated in registers, the normalisation is folded into the stored
 //     coefficients, and the W term reuses the Z term of the entry above (one ratio instead of two coefficients).
-//     The record is fetched ONCE (2 x LDS.128 + LDS.64 from the TMA-staged table) and applied to T trajectories.
+//     The record is fetched ONCE (2 x LDS.128 + LDS.64 from the TMA-staged table).
 //   * RK stage vectors live in shared memory ([stage][6] per trajectory), lane c < 6 owns state component c;
 //     the error norm and the step-size controller are evaluated redundantly by every lane of the group.
-//   * Trajectory t of a group advances by ONE step attempt per outer iteration; a rejected attempt simply
-//     retries in the next iteration while its partner moves on (derive() loop, instance.rs:358-493).
+//   * The trajectory of a group advances by ONE step attempt per outer iteration; a rejected attempt simply
+//     retries in the next iteration while the other groups of the warp move on (derive() loop, instance.rs:358-493).
 //   * HBM is touched only to read the initial state and write the final one.
 //
 // Reference behaviour: instance.rs:87-262, 343-352, 358-493 (propagate/single_step/derive) and
@@ -47,7 +47,6 @@ __host__ __device__ inline size_t coop_meta_bytes(int N, int G, int kmax) {
 __device__ __forceinline__ double shfl_d(unsigned mask, double v, int src, int width) { return __shfl_sync(mask, v, src, width); }
 __device__ __forceinline__ double shfl_xor_d(unsigned mask, double v, int lanemask, int width) { return __shfl_xor_sync(mask, v, lanemask, width); }
 
-__device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ double lds_f64(unsigned addr) {
     double v;
     asm volatile("ld.shared.f64 %0, [%1];" : "=d"(v) : "r"(addr));
@@ -57,29 +56,6 @@ __device__ __forceinline__ int lds_s32(unsigned addr) {
     int v;
     asm volatile("ld.shared.s32 %0, [%1];" : "=r"(v) : "r"(addr));
     return v;
-}
-// ---- TMA 1-D bulk copy global -> shared, completion on an mbarrier (SASS: UBLKCP + SYNCS)
-__device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long* bar, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tma_bulk_g2s(void* dst, const void* src, unsigned bytes, unsigned long long* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "WAIT_LOOP:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra WAIT_DONE;\n"
-        "bra WAIT_LOOP;\n"
-        "WAIT_DONE:\n"
-        "}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
 }
 
 // per-trajectory view of the group's shared memory + constants of motion
@@ -96,50 +72,22 @@ struct TrajCtx {
 // update of the (slow) pole angles and an exact angle addition for the prime-meridian angle W.
 struct RotBase { double sa, ca, sd, cd, sw, cw; };
 
-// third bodies + SRP + drag: a few hundred flops, evaluated redundantly by every lane, kept out of line so that
-// the ephemeris scratch does not inflate the register count of the harmonic sum
-// (scalars, not the TrajCtx, are passed: taking the struct's address would force it into local memory)
-template <bool GEN>
-static __device__ __noinline__ int coop_extra(const DevSetup& S, double dry_mass, double extra_mass, double srp_area, double drag_area,
-                                              long long t_ns, const double y[9], double acc[3]) {
-    double mass = dry_mass + y[8] + extra_mass;
-    const bool has_force = S.has_srp || S.has_drag;
-    if (has_force && !(mass > 0.0)) return NYXB_ERR_MASSLESS;
-    double bpos[NYXB_MAX_BODIES][3];
-    int rc = accel_point_masses(S, t_ns, y, bpos, acc);
-    if (rc) return rc;
-    if (GEN && S.n_xgrav > 0) accel_extra_fields(S, t_ns, y, bpos, acc);
-    if (has_force) accel_post(S, t_ns, y, bpos, mass, srp_area, drag_area, acc);
-    return 0;
-}
-
-// position relative to the body the primary field belongs to (gravity_field.rs:149-154); kept out of line: the Clenshaw scratch must
-// not inflate the register count of the harmonic sum.  An epoch outside the ephemeris is reported by coop_extra (every body).
-static __device__ __noinline__ void coop_field_offset(const DevSetup& S, long long t_ns, double& y0, double& y1, double& y2) {
-    double bp[3];
-    if (body_position(S.bodies[S.grav_body], t_ns, bp)) { y0 -= bp[0]; y1 -= bp[1]; y2 -= bp[2]; }
-}
-
-// Cooperative SpacecraftDynamics::eom for the T stage states held in g[t].ys; lane c < 6 receives dy[c] of each.
-template <int G, int T, bool NC>   // NC ("general fields"): the primary field may belong to another body, further fields may exist
-__device__ __forceinline__ void coop_rhs(const DevSetup& S, const double* __restrict__ recs, int L,
-                                         const double* __restrict__ colseed, unsigned a_cs, unsigned cm_off,
-                                         TrajCtx (&g)[T], const RotBase (&rbase)[T], const double (&dt_s)[T],
-                                         const long long (&t_ns)[T], int lane, unsigned traj_stride_bytes,
-                                         double (&dyc)[T], int (&rc)[T]) {
+// Cooperative SpacecraftDynamics::eom for the stage state held in g.ys; lane c < 6 receives dy[c].  Returns 0 or an nyxb_status error.
+template <int G, bool NC>   // NC ("general fields"): the primary field may belong to another body, further fields may exist
+__device__ __forceinline__ int coop_rhs(const DevSetup& S, const double* __restrict__ recs, int L,
+                                        const double* __restrict__ colseed, unsigned a_cs, unsigned cm_off,
+                                        TrajCtx& g, const RotBase& rb, double dt_s, long long t_ns, int lane, double& dyc) {
     constexpr unsigned FULL = 0xffffffffu;  // the caller keeps the warp converged (see nyxb_k_coop)
     const DevGrav& gv = S.grav;
     const double ra_dot = gv.rot.ra_dot, dec_dot = gv.rot.dec_dot;  // rad/s, precomputed on the host
-    double inv_r[T], rho[T], ub[T], r2[T];
-#pragma unroll
-    for (int t = 0; t < T; ++t) {
+    double inv_r, rho, ub, r2;
+    {
         // ---- inertial -> body-fixed DCM at the stage time (angle addition from the step-epoch base)
         double R[9];
         if (gv.rot.kind == 0) {
             R[0] = 1; R[1] = 0; R[2] = 0; R[3] = 0; R[4] = 1; R[5] = 0; R[6] = 0; R[7] = 0; R[8] = 1;
         } else {
-            const RotBase& rb = rbase[t];
-            const double da = ra_dot * dt_s[t], dd = dec_dot * dt_s[t], dw = gv.rot.wdot * dt_s[t];
+            const double da = ra_dot * dt_s, dd = dec_dot * dt_s, dw = gv.rot.wdot * dt_s;
             const double sa = fma(rb.ca, da, rb.sa), ca = fma(-rb.sa, da, rb.ca);
             const double sd = fma(rb.cd, dd, rb.sd), cd = fma(-rb.sd, dd, rb.cd);
             double sdl, cdl;
@@ -157,24 +105,24 @@ __device__ __forceinline__ void coop_rhs(const DevSetup& S, const double* __rest
             R[3] = fma(cw, b10, -(sw * b00)); R[4] = fma(cw, b11, -(sw * b01)); R[5] = cw * b12;
             R[6] = cd * ca; R[7] = cd * sa; R[8] = sd;
         }
-        double y0 = g[t].ys[0], y1 = g[t].ys[1], y2 = g[t].ys[2];
-        if (NC && S.grav_body >= 0) coop_field_offset(S, t_ns[t], y0, y1, y2);   // field of another body: the state is translated to it first
+        double y0 = g.ys[0], y1 = g.ys[1], y2 = g.ys[2];
+        if (NC && S.grav_body >= 0) field_offset(S, t_ns, y0, y1, y2);   // field of another body: the state is translated to it first
         const double rb0 = fma(R[2], y2, fma(R[1], y1, R[0] * y0));
         const double rb1 = fma(R[5], y2, fma(R[4], y1, R[3] * y0));
         const double rb2 = fma(R[8], y2, fma(R[7], y1, R[6] * y0));
-        inv_r[t] = rsqrt(fma(rb2, rb2, fma(rb1, rb1, rb0 * rb0)));  // one Newton chain instead of sqrt + division
-        rho[t] = gv.r_eq * inv_r[t];
-        ub[t] = (rb2 * inv_r[t]) * rho[t];
-        r2[t] = rho[t] * rho[t];
+        inv_r = rsqrt(fma(rb2, rb2, fma(rb1, rb1, rb0 * rb0)));  // one Newton chain instead of sqrt + division
+        rho = gv.r_eq * inv_r;
+        ub = (rb2 * inv_r) * rho;
+        r2 = rho * rho;
         // park the DCM in the trajectory's scratch (nxt/er are idle during the stages): it is needed again only
         // after the column walk, and keeping it in registers would push the walk's live set past the occupancy target
         if (lane == 0) {
 #pragma unroll
-            for (int q = 0; q < 9; ++q) g[t].nxt[q] = R[q];
+            for (int q = 0; q < 9; ++q) g.nxt[q] = R[q];
         }
         // power tables (cos,sin)(k lambda) cos^k(phi) and rho^k A[k][k]: lane computes k = lane, lane+G, ...
         double zr = 1.0, zi = 0.0, pr = 1.0;
-        double bzr = rb0 * inv_r[t], bzi = rb1 * inv_r[t], bp = rho[t];
+        double bzr = rb0 * inv_r, bzi = rb1 * inv_r, bp = rho;
 #pragma unroll
         for (int bit = 1; bit < G; bit <<= 1) {
             if (lane & bit) {
@@ -190,7 +138,7 @@ __device__ __forceinline__ void coop_rhs(const DevSetup& S, const double* __rest
         }
         const int top = gv.N + 1;
         for (int k = lane; k <= top; k += G) {
-            g[t].rm[k] = zr; g[t].im[k] = zi; g[t].rp[k] = pr * colseed[4 * k];  // rho^k (2k-1)!!: the seed Q[k][k] of column k
+            g.rm[k] = zr; g.im[k] = zi; g.rp[k] = pr * colseed[4 * k];  // rho^k (2k-1)!!: the seed Q[k][k] of column k
             const double nzr = fma(zr, bzr, -(zi * bzi));
             zi = fma(zr, bzi, zi * bzr);
             zr = nzr;
@@ -199,27 +147,21 @@ __device__ __forceinline__ void coop_rhs(const DevSetup& S, const double* __rest
     }
     __syncwarp(FULL);
 
-    // ---- column walk, two entries per iteration.  Per pair: one 80-byte record (5 x LDS.128) and 26 FP64 instructions per
-    // trajectory; the recursion coefficients (2n+1) and (n+m)(n-m) are generated in registers.  The per-column sums
+    // ---- column walk, two entries per iteration.  Per pair: one 80-byte record (5 x LDS.128) and 26 FP64 instructions;
+    // the recursion coefficients (2n+1) and (n+m)(n-m) are generated in registers.  The per-column sums
     // S1..S6 carry no (cos, sin)((m-1) lambda) factor: it is applied once, when the lane switches to its next column
     // (columns have an even number of entries, so the switch is tested once per pair).  Loop invariants are pinned with
     // empty asm: ptxas otherwise rematerialises them inside the loop.
-    unsigned a_rm = smem_u32(g[0].rm), a_seed = smem_u32(colseed);
+    unsigned a_rm = smem_u32(g.rm), a_seed = smem_u32(colseed);
     asm volatile("" : "+r"(a_rm), "+r"(a_cs), "+r"(a_seed));
-#pragma unroll
-    for (int t = 0; t < T; ++t) asm volatile("" : "+d"(r2[t]), "+d"(ub[t]));
+    asm volatile("" : "+d"(r2), "+d"(ub));
     const unsigned pw8 = (unsigned)(gv.N + 3) * 8u;  // rm -> im -> rp stride in bytes
-    double X[T], Y[T], Z[T], W[T], Q1[T], Q2[T], rr[T], ii[T];
-    double S1[T], S2[T], S3[T], S4[T], S5[T], S6[T];
+    double X = 0.0, Y = 0.0, Z = 0.0, W = 0.0, Q1 = 0.0, Q2 = 0.0, rr = 0.0, ii = 0.0;
+    double S1 = 0.0, S2 = 0.0, S3 = 0.0, S4 = 0.0, S5 = 0.0, S6 = 0.0;
     double al = 0.0, be = 0.0;
     int ci = 0;
     int next_start = lds_s32(a_cs);
-    unsigned a_col = a_rm + lds_s32(a_cs + cm_off) * 8;  // &rm[m] of the lane's next column (trajectory 0)
-#pragma unroll
-    for (int t = 0; t < T; ++t) {
-        X[t] = Y[t] = Z[t] = W[t] = Q1[t] = Q2[t] = rr[t] = ii[t] = 0.0;
-        S1[t] = S2[t] = S3[t] = S4[t] = S5[t] = S6[t] = 0.0;
-    }
+    unsigned a_col = a_rm + lds_s32(a_cs + cm_off) * 8;  // &rm[m] of the lane's next column
     const double2* rec = reinterpret_cast<const double2*>(recs) + lane;  // five 16-byte pieces per pair and lane
     // Software pipeline over two register sets (A, B): the records of the NEXT pair are requested before the current
     // pair is consumed, so no LDS latency is exposed; the macro is instantiated twice to avoid register-rotation moves.
@@ -231,46 +173,41 @@ __device__ __forceinline__ void coop_rhs(const DevSetup& S, const double* __rest
             const unsigned a_sd = a_seed + ((a_col - a_rm) >> 3) * 32;                                                  \
             const double pd1 = lds_f64(a_sd + 8), pd2 = lds_f64(a_sd + 16);                                             \
             al = lds_f64(a_sd + 24); be = 0.0;                                                                          \
-            _Pragma("unroll") for (int t = 0; t < T; ++t) {                                                             \
-                const unsigned base = a_col + t * traj_stride_bytes;                                                    \
-                const double q = lds_f64(base + 2 * pw8), rn = lds_f64(base - 8), in_ = lds_f64(base + pw8 - 8);        \
-                /* close the previous column: apply its (cos, sin)((m-1) lambda) */                                     \
-                X[t] = fma(rr[t], S1[t], fma(ii[t], S2[t], X[t]));                                                      \
-                Y[t] = fma(rr[t], S2[t], fma(-ii[t], S1[t], Y[t]));                                                     \
-                Z[t] = fma(rr[t], S3[t], fma(ii[t], S4[t], Z[t]));                                                      \
-                W[t] = fma(rr[t], S5[t], fma(ii[t], S6[t], W[t]));                                                      \
-                Q1[t] = q; rr[t] = rn; ii[t] = in_; Q2[t] = 0.0;                                                        \
-                S1[t] = S2[t] = S3[t] = S4[t] = 0.0;                                                                    \
-                S5[t] = q * pd1; S6[t] = q * pd2; /* W term of the column's first degree (seed record, kappa = 1) */    \
-            }                                                                                                           \
+            const double q = lds_f64(a_col + 2 * pw8), rn = lds_f64(a_col - 8), in_ = lds_f64(a_col + pw8 - 8);         \
+            /* close the previous column: apply its (cos, sin)((m-1) lambda) */                                         \
+            X = fma(rr, S1, fma(ii, S2, X));                                                                            \
+            Y = fma(rr, S2, fma(-ii, S1, Y));                                                                           \
+            Z = fma(rr, S3, fma(ii, S4, Z));                                                                            \
+            W = fma(rr, S5, fma(ii, S6, W));                                                                            \
+            Q1 = q; rr = rn; ii = in_; Q2 = 0.0;                                                                        \
+            S1 = S2 = S3 = S4 = 0.0;                                                                                    \
+            S5 = q * pd1; S6 = q * pd2; /* W term of the column's first degree (seed record, kappa = 1) */              \
             next_start = lds_s32(a_cs + ci * 4);                /* sentinel L+1 after the last column */                \
             a_col = a_rm + lds_s32(a_cs + cm_off + ci * 4) * 8; /* sentinel column 1 */                                 \
         }                                                                                                               \
         rec += 5 * G;                                                                                                   \
         na0 = rec[0]; na1 = rec[G]; nb0 = rec[2 * G]; nb1 = rec[3 * G]; nkk = rec[4 * G]; /* table ends with a null pair */ \
         const double be1 = be + al, al1 = al + 2.0; /* (n+1)^2 - m^2 = n^2 - m^2 + (2n+1) */                             \
-        _Pragma("unroll") for (int t = 0; t < T; ++t) {                                                                 \
-            /* entry a (degree n): Q1 = Q[n], Q2 = Q[n-1] */                                                            \
-            S1[t] = fma(Q1[t], a0.x, S1[t]);                                                                            \
-            S2[t] = fma(Q1[t], a0.y, S2[t]);                                                                            \
-            S3[t] = fma(Q1[t], a1.x, S3[t]);                                                                            \
-            S4[t] = fma(Q1[t], a1.y, S4[t]);                                                                            \
-            const double Qa = fma(al * ub[t], Q1[t], -((be * r2[t]) * Q2[t])); /* Q[n+1] = (2n+1) u Q[n] - (n+m)(n-m) Q[n-1] */ \
-            const double wa = kk.x * Qa;                                                                                \
-            S5[t] = fma(wa, a1.x, S5[t]);                                                                               \
-            S6[t] = fma(wa, a1.y, S6[t]);                                                                               \
-            /* entry b (degree n+1) */                                                                                  \
-            S1[t] = fma(Qa, b0.x, S1[t]);                                                                               \
-            S2[t] = fma(Qa, b0.y, S2[t]);                                                                               \
-            S3[t] = fma(Qa, b1.x, S3[t]);                                                                               \
-            S4[t] = fma(Qa, b1.y, S4[t]);                                                                               \
-            const double Qb = fma(al1 * ub[t], Qa, -((be1 * r2[t]) * Q1[t]));                                           \
-            const double wb = kk.y * Qb;                                                                                \
-            S5[t] = fma(wb, b1.x, S5[t]);                                                                               \
-            S6[t] = fma(wb, b1.y, S6[t]);                                                                               \
-            Q2[t] = Qa;                                                                                                 \
-            Q1[t] = Qb;                                                                                                 \
-        }                                                                                                               \
+        /* entry a (degree n): Q1 = Q[n], Q2 = Q[n-1] */                                                                \
+        S1 = fma(Q1, a0.x, S1);                                                                                         \
+        S2 = fma(Q1, a0.y, S2);                                                                                         \
+        S3 = fma(Q1, a1.x, S3);                                                                                         \
+        S4 = fma(Q1, a1.y, S4);                                                                                         \
+        const double Qa = fma(al * ub, Q1, -((be * r2) * Q2)); /* Q[n+1] = (2n+1) u Q[n] - (n+m)(n-m) Q[n-1] */         \
+        const double wa = kk.x * Qa;                                                                                    \
+        S5 = fma(wa, a1.x, S5);                                                                                         \
+        S6 = fma(wa, a1.y, S6);                                                                                         \
+        /* entry b (degree n+1) */                                                                                      \
+        S1 = fma(Qa, b0.x, S1);                                                                                         \
+        S2 = fma(Qa, b0.y, S2);                                                                                         \
+        S3 = fma(Qa, b1.x, S3);                                                                                         \
+        S4 = fma(Qa, b1.y, S4);                                                                                         \
+        const double Qb = fma(al1 * ub, Qa, -((be1 * r2) * Q1));                                                        \
+        const double wb = kk.y * Qb;                                                                                    \
+        S5 = fma(wb, b1.x, S5);                                                                                         \
+        S6 = fma(wb, b1.y, S6);                                                                                         \
+        Q2 = Qa;                                                                                                        \
+        Q1 = Qb;                                                                                                        \
         be = be1 + al1;                                                                                                 \
         al = al1 + 2.0;                                                                                                 \
         e += 2;                                                                                                         \
@@ -285,80 +222,73 @@ __device__ __forceinline__ void coop_rhs(const DevSetup& S, const double* __rest
         COOP_WALK_PAIR(B0, B1, B2, B3, B4, A0, A1, A2, A3, A4)
     }
 #undef COOP_WALK_PAIR
+    // close the last column
+    X = fma(rr, S1, fma(ii, S2, X));
+    Y = fma(rr, S2, fma(-ii, S1, Y));
+    Z = fma(rr, S3, fma(ii, S4, Z));
+    W = fma(rr, S5, fma(ii, S6, W));
 #pragma unroll
-    for (int t = 0; t < T; ++t) {  // close the last column
-        X[t] = fma(rr[t], S1[t], fma(ii[t], S2[t], X[t]));
-        Y[t] = fma(rr[t], S2[t], fma(-ii[t], S1[t], Y[t]));
-        Z[t] = fma(rr[t], S3[t], fma(ii[t], S4[t], Z[t]));
-        W[t] = fma(rr[t], S5[t], fma(ii[t], S6[t], W[t]));
+    for (int off = G / 2; off >= 1; off >>= 1) {
+        X += shfl_xor_d(FULL, X, off, G);
+        Y += shfl_xor_d(FULL, Y, off, G);
+        Z += shfl_xor_d(FULL, Z, off, G);
+        W += shfl_xor_d(FULL, W, off, G);
     }
+    // ---- reload the stage state and the DCM, assemble the acceleration
+    double y[9];
 #pragma unroll
-    for (int t = 0; t < T; ++t) {
+    for (int e = 0; e < 6; ++e) y[e] = g.ys[e];
+    y[6] = g.cr + g.hz; y[7] = g.cd + g.hz; y[8] = g.pm + g.hz;
+    double R[9];
 #pragma unroll
-        for (int off = G / 2; off >= 1; off >>= 1) {
-            X[t] += shfl_xor_d(FULL, X[t], off, G);
-            Y[t] += shfl_xor_d(FULL, Y[t], off, G);
-            Z[t] += shfl_xor_d(FULL, Z[t], off, G);
-            W[t] += shfl_xor_d(FULL, W[t], off, G);
-        }
-        // ---- reload the stage state and the DCM, assemble the acceleration
-        double y[9];
-#pragma unroll
-        for (int e = 0; e < 6; ++e) y[e] = g[t].ys[e];
-        y[6] = g[t].cr + g[t].hz; y[7] = g[t].cd + g[t].hz; y[8] = g[t].pm + g[t].hz;
-        double R[9];
-#pragma unroll
-        for (int q = 0; q < 9; ++q) R[q] = g[t].nxt[q];
-        double s_, t_, u_;
-        if (NC) {
-            double q0 = y[0], q1 = y[1], q2 = y[2];   // position relative to the field's body
-            if (S.grav_body >= 0) coop_field_offset(S, t_ns[t], q0, q1, q2);
-            s_ = fma(R[2], q2, fma(R[1], q1, R[0] * q0)) * inv_r[t];
-            t_ = fma(R[5], q2, fma(R[4], q1, R[3] * q0)) * inv_r[t];
-            u_ = fma(R[8], q2, fma(R[7], q1, R[6] * q0)) * inv_r[t];
-        } else {
-            s_ = fma(R[2], y[2], fma(R[1], y[1], R[0] * y[0])) * inv_r[t];
-            t_ = fma(R[5], y[2], fma(R[4], y[1], R[3] * y[0])) * inv_r[t];
-            u_ = fma(R[8], y[2], fma(R[7], y[1], R[6] * y[0])) * inv_r[t];
-        }
-        // rr_n A[n][m] = K0 rho (rho^n A),  rr_{n-1} A[n][m] = K0 (rho^n A),  K0 = mu / (r R_eq)
-        const double K0 = (gv.mu * gv.inv_r_eq) * inv_r[t];
-        const double K1 = K0 * rho[t];
-        const double aw = -K0 * W[t];
-        const double ab0 = fma(aw, s_, K1 * X[t]), ab1 = fma(aw, t_, K1 * Y[t]), ab2 = fma(aw, u_, K1 * Z[t]);
-        // two-body (orbital.rs:86-92): from the same 1/r when the field belongs to the centre
-        const double ir_c = (NC && S.grav_body >= 0) ? rsqrt(fma(y[2], y[2], fma(y[1], y[1], y[0] * y[0]))) : inv_r[t];
-        const double fac = -S.mu_central * ir_c * ir_c * ir_c;
-        double acc[3];
-        acc[0] = fma(fac, y[0], fma(R[6], ab2, fma(R[3], ab1, R[0] * ab0)));
-        acc[1] = fma(fac, y[1], fma(R[7], ab2, fma(R[4], ab1, R[1] * ab0)));
-        acc[2] = fma(fac, y[2], fma(R[8], ab2, fma(R[5], ab1, R[2] * ab0)));
-        rc[t] = 0;
-        if (S.n_bodies > 0 || S.has_srp || S.has_drag || (NC && S.n_xgrav > 0)) {
-            // cold path: private copies, so that y/acc of the common path are never address-taken (they stay in registers)
-            double yy[9], aa[3];
-#pragma unroll
-            for (int e = 0; e < 9; ++e) yy[e] = y[e];
-            aa[0] = acc[0]; aa[1] = acc[1]; aa[2] = acc[2];
-            rc[t] = coop_extra<NC>(S, g[t].dry_mass, g[t].extra_mass, g[t].srp_area, g[t].drag_area, t_ns[t], yy, aa);
-            acc[0] = aa[0]; acc[1] = aa[1]; acc[2] = aa[2];
-        }
-        // lane c < 3 keeps the velocity component c, lanes 3..5 the acceleration components (selects, no jump table)
-        const int c3 = lane >= 3 ? lane - 3 : lane;
-        const double vsel = c3 == 0 ? y[3] : (c3 == 1 ? y[4] : y[5]);
-        const double asel = c3 == 0 ? acc[0] : (c3 == 1 ? acc[1] : acc[2]);
-        dyc[t] = lane >= 3 ? asel : vsel;
+    for (int q = 0; q < 9; ++q) R[q] = g.nxt[q];
+    double s_, t_, u_;
+    if (NC) {
+        double q0 = y[0], q1 = y[1], q2 = y[2];   // position relative to the field's body
+        if (S.grav_body >= 0) field_offset(S, t_ns, q0, q1, q2);
+        s_ = fma(R[2], q2, fma(R[1], q1, R[0] * q0)) * inv_r;
+        t_ = fma(R[5], q2, fma(R[4], q1, R[3] * q0)) * inv_r;
+        u_ = fma(R[8], q2, fma(R[7], q1, R[6] * q0)) * inv_r;
+    } else {
+        s_ = fma(R[2], y[2], fma(R[1], y[1], R[0] * y[0])) * inv_r;
+        t_ = fma(R[5], y[2], fma(R[4], y[1], R[3] * y[0])) * inv_r;
+        u_ = fma(R[8], y[2], fma(R[7], y[1], R[6] * y[0])) * inv_r;
     }
+    // rr_n A[n][m] = K0 rho (rho^n A),  rr_{n-1} A[n][m] = K0 (rho^n A),  K0 = mu / (r R_eq)
+    const double K0 = (gv.mu * gv.inv_r_eq) * inv_r;
+    const double K1 = K0 * rho;
+    const double aw = -K0 * W;
+    const double ab0 = fma(aw, s_, K1 * X), ab1 = fma(aw, t_, K1 * Y), ab2 = fma(aw, u_, K1 * Z);
+    // two-body (orbital.rs:86-92): from the same 1/r when the field belongs to the centre
+    const double ir_c = (NC && S.grav_body >= 0) ? rsqrt(fma(y[2], y[2], fma(y[1], y[1], y[0] * y[0]))) : inv_r;
+    const double fac = -S.mu_central * ir_c * ir_c * ir_c;
+    double acc[3];
+    acc[0] = fma(fac, y[0], fma(R[6], ab2, fma(R[3], ab1, R[0] * ab0)));
+    acc[1] = fma(fac, y[1], fma(R[7], ab2, fma(R[4], ab1, R[1] * ab0)));
+    acc[2] = fma(fac, y[2], fma(R[8], ab2, fma(R[5], ab1, R[2] * ab0)));
+    int rc = 0;
+    if (S.n_bodies > 0 || S.has_srp || S.has_drag || (NC && S.n_xgrav > 0)) {
+        // cold path: private copies, so that y/acc of the common path are never address-taken (they stay in registers)
+        double yy[9], aa[3];
+#pragma unroll
+        for (int e = 0; e < 9; ++e) yy[e] = y[e];
+        aa[0] = acc[0]; aa[1] = acc[1]; aa[2] = acc[2];
+        rc = accel_cold<NC>(S, g.dry_mass, g.extra_mass, g.srp_area, g.drag_area, t_ns, yy, aa);
+        acc[0] = aa[0]; acc[1] = aa[1]; acc[2] = aa[2];
+    }
+    // lane c < 3 keeps the velocity component c, lanes 3..5 the acceleration components (selects, no jump table)
+    const int c3 = lane >= 3 ? lane - 3 : lane;
+    const double vsel = c3 == 0 ? y[3] : (c3 == 1 ? y[4] : y[5]);
+    const double asel = c3 == 0 ? acc[0] : (c3 == 1 ? acc[1] : acc[2]);
+    dyc = lane >= 3 ? asel : vsel;
+    return rc;
 }
 
-template <int G, int T, bool SMEM_TABLE, bool NC = false>
+template <int G, bool SMEM_TABLE, bool NC = false>
 #ifndef COOP_MINB1
 #define COOP_MINB1 5
 #endif
-#ifndef COOP_MINB2
-#define COOP_MINB2 3   /* resident CTAs per SM the T = 2 instantiation is compiled for (register cap 65536 / (COOP_CTA * COOP_MINB2)) */
-#endif
-__global__ void __launch_bounds__(COOP_CTA, (T == 1 ? COOP_MINB1 : COOP_MINB2))
+__global__ void __launch_bounds__(COOP_CTA, COOP_MINB1)
 nyxb_k_coop(const __grid_constant__ DevSetup S, const __grid_constant__ DevCoop Cp, size_t n,
             const double* __restrict__ state, const double* __restrict__ consts,
             const long long* __restrict__ epoch0, long long end_epoch, long long* __restrict__ step_io,
@@ -396,312 +326,267 @@ nyxb_k_coop(const __grid_constant__ DevSetup S, const __grid_constant__ DevCoop 
     const unsigned a_cs = smem_u32(sm_cs + lane * (Cp.kmax + 2));
     const unsigned cm_off = (unsigned)(G * (Cp.kmax + 2) * 4);
 
-    // ---- trajectories of this group: pair index strided over the grid so that every SM gets the same share
-    // whole warps are strided over the grid (every SM gets the same number of FULL warps, surplus warps exit)
-    const size_t n_sets = (n + T - 1) / T;
+    // ---- the trajectory of this group: whole warps are strided over the grid (every SM gets the same number of FULL warps,
+    // surplus warps exit)
     const int gpw = 32 / G;
-    const size_t set0 = ((size_t)blockIdx.x + (size_t)gridDim.x * (tid >> 5)) * gpw;  // first set of this WARP
-    if (set0 >= n_sets) return;  // uniform per warp; no block-wide barrier below this point
+    const size_t traj0 = ((size_t)blockIdx.x + (size_t)gridDim.x * (tid >> 5)) * gpw;  // first trajectory of this WARP
+    if (traj0 >= n) return;  // uniform per warp; no block-wide barrier below this point
     // The control flow below is WARP-uniform: every group of the warp runs the same sequence of attempts until all of them
     // are done (a finished or absent group keeps executing on its own scratch without committing anything), so all
     // synchronisation uses the full mask -- sub-warp masks cost a MATCH/REDUX/VOTE sequence per shuffle group.
-    const size_t set_raw = set0 + (tid & 31) / G;
-    const bool group_valid = set_raw < n_sets;
-    const size_t set = group_valid ? set_raw : 0;  // an absent group shadows set 0 and is never committed
+    const size_t traj_raw = traj0 + (tid & 31) / G;
+    const bool valid = traj_raw < n;
+    const size_t traj = valid ? traj_raw : 0;  // an absent group shadows trajectory 0 and is never committed
     const int tstride = coop_traj_stride(N);
-    double* sm = reinterpret_cast<double*>(meta + coop_meta_bytes(N, G, Cp.kmax)) + (size_t)grp * T * tstride;
+    double* sm = reinterpret_cast<double*>(meta + coop_meta_bytes(N, G, Cp.kmax)) + (size_t)grp * tstride;
     const int pw = N + 3;
     const unsigned lw = tid & 31;
     const unsigned gmask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << (lw - lane));  // cold, group-divergent paths only
     constexpr unsigned FULL = 0xffffffffu;
 
-    TrajCtx g[T];
-    size_t traj[T];
-    bool valid[T], done[T], retry[T], last[T], backprop[T];
-    double yc[T], h[T], nx[T], det_error[T];
-    long long epoch[T], step_ns[T], prev_step[T], det_step[T];
-    int n_steps[T], n_rej[T], n_rhs[T];
-    int fixed[T], prev_fixed[T], status[T], rc[T], det_attempts[T];
-    RotBase rbase[T];
+    TrajCtx g;
+    g.kst = sm; g.ys = sm + 96; g.ycur = sm + 102; g.nxt = sm + 108; g.er = sm + 114; g.ev = sm + 120;
+    g.rm = sm + COOP_SM_FIXED; g.im = g.rm + pw; g.rp = g.im + pw;
+    g.hz = 0.0;
+    // every lane of the group reads the same addresses (broadcast within the request)
     const int cidx = lane < 6 ? lane : 0;
-#pragma unroll
-    for (int t = 0; t < T; ++t) {
-        double* s = sm + (size_t)t * tstride;
-        g[t].kst = s; g[t].ys = s + 96; g[t].ycur = s + 102; g[t].nxt = s + 108; g[t].er = s + 114; g[t].ev = s + 120;
-        g[t].rm = s + COOP_SM_FIXED; g[t].im = g[t].rm + pw; g[t].rp = g[t].im + pw;
-        g[t].hz = 0.0;
-        valid[t] = group_valid && (set * T + t) < n;
-        traj[t] = valid[t] ? set * T + t : set * T;  // an absent partner shadows trajectory 0 and is never committed
-        // every lane of the group reads the same addresses (broadcast within the request)
-        yc[t] = state[(size_t)cidx * n + traj[t]];
-        g[t].cr = state[6 * n + traj[t]]; g[t].cd = state[7 * n + traj[t]]; g[t].pm = state[8 * n + traj[t]];
-        g[t].dry_mass = consts[traj[t]]; g[t].extra_mass = consts[n + traj[t]];
-        g[t].srp_area = consts[2 * n + traj[t]]; g[t].drag_area = consts[3 * n + traj[t]];
-        epoch[t] = epoch0[traj[t]];
-        step_ns[t] = step_io ? step_io[traj[t]] : S.init_step_ns;
-        fixed[t] = S.fixed_step;
-        status[t] = 0; rc[t] = 0;
-        det_step[t] = S.init_step_ns; n_steps[t] = 0; n_rej[t] = 0; n_rhs[t] = 0;
-        det_error[t] = 0.0; det_attempts[t] = 1;
-        retry[t] = false; last[t] = false; h[t] = 0.0; nx[t] = 0.0; prev_step[t] = step_ns[t]; prev_fixed[t] = fixed[t];
-        rbase[t].sa = 0; rbase[t].ca = 1; rbase[t].sd = 1; rbase[t].cd = 0; rbase[t].sw = 0; rbase[t].cw = 1;
-        if (lane < 6) g[t].ycur[lane] = yc[t];
-        if (sink.ev_kind && lane == 0) {
-            g[t].ev[0] = event_eval(sink.ev_kind, sink.ev_value, state[traj[t]], state[n + traj[t]], state[2 * n + traj[t]],
-                                    state[3 * n + traj[t]], state[4 * n + traj[t]], state[5 * n + traj[t]]);
-            g[t].ev[1] = 0.0;
-        }
-        if (valid[t] && sink.cap > 0) {  // start state (instance.rs:307, 321)
-            if (lane < 6) sink.state[((size_t)lane * sink.cap) * n + traj[t]] = yc[t];
-            if (lane == 6) sink.epoch[traj[t]] = epoch[t];
-        }
-        // instance.rs:96-115
-        const long long duration = end_epoch - epoch[t];
-        backprop[t] = duration < 0;
-        done[t] = !valid[t] || (duration == 0);
-        if (!done[t] && g[t].pm < 0.0) { rc[t] = NYXB_ERR_FUEL_EXHAUSTED; done[t] = true; }
-        if (!done[t] && duration < 0) step_ns[t] = -step_ns[t];
+    double yc = state[(size_t)cidx * n + traj];
+    g.cr = state[6 * n + traj]; g.cd = state[7 * n + traj]; g.pm = state[8 * n + traj];
+    g.dry_mass = consts[traj]; g.extra_mass = consts[n + traj];
+    g.srp_area = consts[2 * n + traj]; g.drag_area = consts[3 * n + traj];
+    long long epoch = epoch0[traj];
+    long long step_ns = step_io ? step_io[traj] : S.init_step_ns;
+    int fixed = S.fixed_step;
+    int status = 0, rc = 0;
+    long long det_step = S.init_step_ns;
+    int n_steps = 0, n_rej = 0, n_rhs = 0;
+    double det_error = 0.0;
+    int det_attempts = 1;
+    bool retry = false, last = false;
+    double h = 0.0, nx = 0.0;
+    long long prev_step = step_ns;
+    int prev_fixed = fixed;
+    RotBase rbase;
+    rbase.sa = 0; rbase.ca = 1; rbase.sd = 1; rbase.cd = 0; rbase.sw = 0; rbase.cw = 1;
+    if (lane < 6) g.ycur[lane] = yc;
+    if (sink.ev_kind && lane == 0) {
+        g.ev[0] = event_eval(sink.ev_kind, sink.ev_value, state[traj], state[n + traj], state[2 * n + traj],
+                             state[3 * n + traj], state[4 * n + traj], state[5 * n + traj]);
+        g.ev[1] = 0.0;
     }
+    if (valid && sink.cap > 0) {  // start state (instance.rs:307, 321)
+        if (lane < 6) sink.state[((size_t)lane * sink.cap) * n + traj] = yc;
+        if (lane == 6) sink.epoch[traj] = epoch;
+    }
+    // instance.rs:96-115
+    const long long duration = end_epoch - epoch;
+    const bool backprop = duration < 0;
+    bool done = !valid || (duration == 0);
+    if (!done && g.pm < 0.0) { rc = NYXB_ERR_FUEL_EXHAUSTED; done = true; }
+    if (!done && duration < 0) step_ns = -step_ns;
     __syncwarp(FULL);
     const int stages = S.tb.stages;
     const long long stop = end_epoch;
 
     for (;;) {
-        bool all_done = true;
-#pragma unroll
-        for (int t = 0; t < T; ++t) {
-            if (done[t] || retry[t]) { all_done &= done[t]; continue; }
+        if (!done && !retry) {
             // ---- instance.rs:149-196: pick this step (regular, or the final fixed step to the stop time)
-            last[t] = false;
-            prev_step[t] = step_ns[t];
-            prev_fixed[t] = fixed[t];
-            if ((!backprop[t] && epoch[t] + step_ns[t] > stop) || (backprop[t] && epoch[t] + step_ns[t] <= stop)) {
-                if (stop == epoch[t]) { done[t] = true; continue; }
-                step_ns[t] = stop - epoch[t];
-                fixed[t] = 1;
-                last[t] = true;
-            }
-            all_done = false;
-            det_attempts[t] = 1;
-            h[t] = dur_to_seconds(step_ns[t]);
-        }
-        if (__all_sync(FULL, all_done)) break;
-        // ---- orientation angles at the step epochs: lanes 0..2 evaluate one sin/cos pair each
-        if (S.grav.rot.kind != 0) {
-#pragma unroll
-            for (int t = 0; t < T; ++t) {
-                const double t_s = dur_to_seconds(epoch[t]);
-                const double d = t_s / 86400.0;
-                const double Tc = d / 36525.0;
-                double ang;
-                if (lane == 0) ang = (S.grav.rot.ra0 + S.grav.rot.ra1 * Tc) * NYXB_DEG2RAD;
-                else if (lane == 1) ang = (S.grav.rot.dec0 + S.grav.rot.dec1 * Tc) * NYXB_DEG2RAD;
-                else ang = fmod(S.grav.rot.w0 + S.grav.rot.w1 * d, 360.0) * NYXB_DEG2RAD;
-                double sv, cv;
-                det_sincos(ang, sv, cv);
-                rbase[t].sa = shfl_d(FULL, sv, 0, G); rbase[t].ca = shfl_d(FULL, cv, 0, G);
-                rbase[t].sd = shfl_d(FULL, sv, 1, G); rbase[t].cd = shfl_d(FULL, cv, 1, G);
-                rbase[t].sw = shfl_d(FULL, sv, 2, G); rbase[t].cw = shfl_d(FULL, cv, 2, G);
-            }
-        }
-        // ---- derive(): one attempt for every trajectory of the group (instance.rs:358-493)
-        for (int i = 0; i < stages; ++i) {
-            double dt_s[T], dyc[T];
-            long long t_ns[T];
-            int rcs[T];
-#pragma unroll
-            for (int t = 0; t < T; ++t) {
-                // stage state y + h * sum_j a_ij k_j (instance.rs:376-394); stage 0 is y itself
-                if (lane < 6) {
-                    double ysv = yc[t];
-                    if (i > 0) {
-                        const double* arow = &S.tb.a[(i - 1) * NYXB_MAX_STAGES];
-                        double w0 = 0.0, w1 = 0.0;  // two chains: the sum is latency-bound otherwise
-                        int j = 0;
-                        for (; j + 1 < i; j += 2) {
-                            w0 = fma(arow[j], g[t].kst[j * 6 + lane], w0);
-                            w1 = fma(arow[j + 1], g[t].kst[(j + 1) * 6 + lane], w1);
-                        }
-                        if (j < i) w0 = fma(arow[j], g[t].kst[j * 6 + lane], w0);
-                        ysv = fma(h[t], w0 + w1, yc[t]);
-                    }
-                    g[t].ys[lane] = ysv;
+            last = false;
+            prev_step = step_ns;
+            prev_fixed = fixed;
+            if (ctl_past_stop(epoch, step_ns, stop, backprop)) {
+                if (stop == epoch) {
+                    done = true;
+                } else {
+                    step_ns = stop - epoch;
+                    fixed = 1;
+                    last = true;
                 }
-                g[t].hz = (i > 0) ? h[t] * 0.0 : 0.0;
-                const long long off_ns = (i > 0) ? dur_from_seconds(S.tb.c[i - 1] * h[t]) : 0;  // stage epoch is ns-truncated
-                dt_s[t] = (double)off_ns * 1e-9;
-                t_ns[t] = epoch[t] + off_ns;
             }
+            if (!done) {
+                det_attempts = 1;
+                h = dur_to_seconds(step_ns);
+            }
+        }
+        if (__all_sync(FULL, done)) break;
+        // ---- orientation angles at the step epoch: lanes 0..2 evaluate one sin/cos pair each
+        if (S.grav.rot.kind != 0) {
+            const double t_s = dur_to_seconds(epoch);
+            const double d = t_s / 86400.0;
+            const double Tc = d / 36525.0;
+            double ang;
+            if (lane == 0) ang = (S.grav.rot.ra0 + S.grav.rot.ra1 * Tc) * NYXB_DEG2RAD;
+            else if (lane == 1) ang = (S.grav.rot.dec0 + S.grav.rot.dec1 * Tc) * NYXB_DEG2RAD;
+            else ang = fmod(S.grav.rot.w0 + S.grav.rot.w1 * d, 360.0) * NYXB_DEG2RAD;
+            double sv, cv;
+            det_sincos(ang, sv, cv);
+            rbase.sa = shfl_d(FULL, sv, 0, G); rbase.ca = shfl_d(FULL, cv, 0, G);
+            rbase.sd = shfl_d(FULL, sv, 1, G); rbase.cd = shfl_d(FULL, cv, 1, G);
+            rbase.sw = shfl_d(FULL, sv, 2, G); rbase.cw = shfl_d(FULL, cv, 2, G);
+        }
+        // ---- derive(): one attempt (instance.rs:358-493)
+        for (int i = 0; i < stages; ++i) {
+            // stage state y + h * sum_j a_ij k_j (instance.rs:376-394); stage 0 is y itself
+            if (lane < 6) {
+                double ysv = yc;
+                if (i > 0) {
+                    const double* arow = &S.tb.a[(i - 1) * NYXB_MAX_STAGES];
+                    double w0 = 0.0, w1 = 0.0;  // two chains: the sum is latency-bound otherwise
+                    int j = 0;
+                    for (; j + 1 < i; j += 2) {
+                        w0 = fma(arow[j], g.kst[j * 6 + lane], w0);
+                        w1 = fma(arow[j + 1], g.kst[(j + 1) * 6 + lane], w1);
+                    }
+                    if (j < i) w0 = fma(arow[j], g.kst[j * 6 + lane], w0);
+                    ysv = fma(h, w0 + w1, yc);
+                }
+                g.ys[lane] = ysv;
+            }
+            g.hz = (i > 0) ? h * 0.0 : 0.0;
+            const long long off_ns = (i > 0) ? dur_from_seconds(S.tb.c[i - 1] * h) : 0;  // stage epoch is ns-truncated
+            const double dt_s = (double)off_ns * 1e-9;
+            const long long t_ns = epoch + off_ns;
             __syncwarp(FULL);
-            coop_rhs<G, T, NC>(S, recs, Cp.L, sm_seed, a_cs, cm_off, g, rbase, dt_s, t_ns, lane,
-                           (unsigned)(tstride * 8), dyc, rcs);
-#pragma unroll
-            for (int t = 0; t < T; ++t) {
-                if (done[t]) continue;
-                ++n_rhs[t];
-                if (rcs[t]) { rc[t] = rcs[t]; done[t] = true; continue; }
-                if (lane < 6) g[t].kst[i * 6 + lane] = dyc[t];
+            double dyc;
+            const int rcs = coop_rhs<G, NC>(S, recs, Cp.L, sm_seed, a_cs, cm_off, g, rbase, dt_s, t_ns, lane, dyc);
+            if (!done) {
+                ++n_rhs;
+                if (rcs) { rc = rcs; done = true; }
+                else if (lane < 6) g.kst[i * 6 + lane] = dyc;
             }
             // every lane read the stage state (ys) and the parked DCM (nxt) at the end of coop_rhs: order those reads before the
             // next stage's writes (compute-sanitizer racecheck found a write-after-read on ys without it)
             __syncwarp(FULL);
         }
-#pragma unroll
-        for (int t = 0; t < T; ++t) {
+        {
             double er = 0.0;
-            nx[t] = yc[t];
+            nx = yc;
             if (lane < 6) {
                 for (int i = 0; i < stages; ++i) {
-                    const double ki = g[t].kst[i * 6 + lane];
-                    if (!fixed[t]) er = fma(h[t] * S.tb.e[i], ki, er);
-                    nx[t] = fma(h[t] * S.tb.b[i], ki, nx[t]);
+                    const double ki = g.kst[i * 6 + lane];
+                    if (!fixed) er = fma(h * S.tb.e[i], ki, er);
+                    nx = fma(h * S.tb.b[i], ki, nx);
                 }
-                g[t].nxt[lane] = nx[t];
-                g[t].er[lane] = er;
+                g.nxt[lane] = nx;
+                g.er[lane] = er;
             }
         }
         __syncwarp(FULL);
-#pragma unroll
-        for (int t = 0; t < T; ++t) {
-            if (done[t]) continue;
+        if (!done) {
             long long dt_ns = 0;
-            bool accept;
-            if (fixed[t]) {
-                det_step[t] = step_ns[t]; dt_ns = step_ns[t]; accept = true;
+            bool accept = true;
+            if (fixed) {
+                det_step = step_ns; dt_ns = step_ns;
             } else {
                 double e9[9], c9[9], y9[9];
 #pragma unroll
-                for (int e = 0; e < 6; ++e) { e9[e] = g[t].er[e]; c9[e] = g[t].nxt[e]; y9[e] = g[t].ycur[e]; }
+                for (int e = 0; e < 6; ++e) { e9[e] = g.er[e]; c9[e] = g.nxt[e]; y9[e] = g.ycur[e]; }
                 e9[6] = e9[7] = e9[8] = 0.0;
-                y9[6] = g[t].cr; y9[7] = g[t].cd; y9[8] = g[t].pm;
-                c9[6] = g[t].cr + g[t].hz; c9[7] = g[t].cd + g[t].hz; c9[8] = g[t].pm + g[t].hz;
-                det_error[t] = error_estimate(S.error_ctrl, e9, c9, y9);
-                accept = det_error[t] <= S.tolerance || h[t] <= S.min_step_s || det_attempts[t] >= S.attempts;
+                y9[6] = g.cr; y9[7] = g.cd; y9[8] = g.pm;
+                c9[6] = g.cr + g.hz; c9[7] = g.cd + g.hz; c9[8] = g.pm + g.hz;
+                det_error = error_estimate(S.error_ctrl, e9, c9, y9);
+                accept = ctl_accept(S, det_error, h, det_attempts);
                 if (accept) {
                     bool bad = false;
 #pragma unroll
                     for (int e = 0; e < 9; ++e) bad |= (c9[e] != c9[e]);
-                    if (bad) { rc[t] = NYXB_ERR_PROP_MATH; done[t] = true; continue; }
-                    if (det_attempts[t] >= S.attempts) status[t] |= NYXB_WARN_MAX_ATTEMPTS;
-                    det_step[t] = dur_from_seconds(h[t]);
-                    double hn = h[t];
-                    if (det_error[t] < S.tolerance) {
-                        const double proposed = 0.9 * h[t] * pow_inv_int(S.tolerance / det_error[t], S.tb.order);
-                        if (fabs(proposed) > fabs(S.max_step_s)) {
-                            const double sg = (proposed != proposed) ? proposed : (signbit(proposed) ? -1.0 : 1.0);
-                            hn = S.max_step_s * sg;
-                        } else {
-                            hn = proposed;
-                        }
+                    if (bad) {
+                        rc = NYXB_ERR_PROP_MATH; done = true; accept = false;
+                    } else {
+                        step_ns = ctl_accepted<pow_inv_int>(S, det_error, h, det_attempts, status, det_step);
+                        dt_ns = det_step;
                     }
-                    step_ns[t] = dur_from_seconds(hn);
-                    const long long ab = step_ns[t] < 0 ? -step_ns[t] : step_ns[t];
-                    if (ab < S.min_step_ns) step_ns[t] = (step_ns[t] < 0) ? -S.min_step_ns : S.min_step_ns;
-                    dt_ns = det_step[t];
                 } else {
-                    det_attempts[t] += 1;
-                    n_rej[t] += 1;
-                    const double proposed = 0.9 * h[t] * pow_inv_int(S.tolerance / det_error[t], S.tb.order - 1);
-                    h[t] = (proposed < S.min_step_s) ? S.min_step_s : proposed;
-                    retry[t] = true;
+                    det_attempts += 1;
+                    n_rej += 1;
+                    h = ctl_retry<pow_inv_int>(S, det_error, h);
+                    retry = true;
                 }
             }
-            if (!accept) continue;
-            // ---- single_step(): instance.rs:343-352
-            retry[t] = false;
-            epoch[t] += dt_ns;
-            yc[t] = nx[t];  // committed below, after every lane has finished reading ycur/nxt
-            g[t].cr = g[t].cr < 0.0 ? 0.0 : (g[t].cr > 2.0 ? 2.0 : g[t].cr);  // cosmic/spacecraft.rs:494
-            n_steps[t] += 1;
-            if (n_steps[t] < sink.cap) {  // the channel send of instance.rs:186-193 / 255-259 (56 B per accepted step)
-                const size_t s = (size_t)n_steps[t];
-                if (lane < 6) sink.state[((size_t)lane * sink.cap + s) * n + traj[t]] = nx[t];
-                if (lane == 6) sink.epoch[s * n + traj[t]] = epoch[t];
-            }
-            if (g[t].pm < 0.0) { rc[t] = NYXB_ERR_FUEL_EXHAUSTED; done[t] = true; }
-            if (sink.ev_kind && !last[t]) {  // stop condition on non-final steps (instance.rs:243-252, event.rs:120-150); nxt = new state
-                const double yn = event_eval(sink.ev_kind, sink.ev_value, g[t].nxt[0], g[t].nxt[1], g[t].nxt[2], g[t].nxt[3], g[t].nxt[4], g[t].nxt[5]);
-                const double cnt = g[t].ev[1] + ((g[t].ev[0] * yn < 0.0) ? 1.0 : 0.0);
-                __syncwarp(gmask);
-                if (lane == 0) { g[t].ev[0] = yn; g[t].ev[1] = cnt; }
-                if (cnt >= (double)sink.ev_trigger) done[t] = true;
-            }
-            if (last[t]) {
-                step_ns[t] = prev_step[t];
-                fixed[t] = prev_fixed[t];
-                if (backprop[t]) step_ns[t] = -step_ns[t];
-                done[t] = true;
+            if (accept) {
+                // ---- single_step(): instance.rs:343-352
+                retry = false;
+                epoch += dt_ns;
+                yc = nx;  // committed below, after every lane has finished reading ycur/nxt
+                g.cr = g.cr < 0.0 ? 0.0 : (g.cr > 2.0 ? 2.0 : g.cr);  // cosmic/spacecraft.rs:494
+                n_steps += 1;
+                if (n_steps < sink.cap) {  // the channel send of instance.rs:186-193 / 255-259 (56 B per accepted step)
+                    const size_t s = (size_t)n_steps;
+                    if (lane < 6) sink.state[((size_t)lane * sink.cap + s) * n + traj] = nx;
+                    if (lane == 6) sink.epoch[s * n + traj] = epoch;
+                }
+                if (g.pm < 0.0) { rc = NYXB_ERR_FUEL_EXHAUSTED; done = true; }
+                if (sink.ev_kind && !last) {  // stop condition on non-final steps (instance.rs:243-252, event.rs:120-150); nxt = new state
+                    const double yn = event_eval(sink.ev_kind, sink.ev_value, g.nxt[0], g.nxt[1], g.nxt[2], g.nxt[3], g.nxt[4], g.nxt[5]);
+                    const double cnt = g.ev[1] + ((g.ev[0] * yn < 0.0) ? 1.0 : 0.0);
+                    __syncwarp(gmask);
+                    if (lane == 0) { g.ev[0] = yn; g.ev[1] = cnt; }
+                    if (cnt >= (double)sink.ev_trigger) done = true;
+                }
+                if (last) {
+                    step_ns = prev_step;
+                    fixed = prev_fixed;
+                    if (backprop) step_ns = -step_ns;
+                    done = true;
+                }
             }
         }
         __syncwarp(FULL);  // all lanes are done reading ycur/nxt/er
-#pragma unroll
-        for (int t = 0; t < T; ++t)
-            if (lane < 6) g[t].ycur[lane] = yc[t];
+        if (lane < 6) g.ycur[lane] = yc;
     }
     __syncwarp(FULL);
-#pragma unroll
-    for (int t = 0; t < T; ++t) {
-        if (!valid[t]) continue;
-        if (lane < 6) out_state[(size_t)lane * n + traj[t]] = yc[t];
-        if (lane == 6) {
-            out_state[6 * n + traj[t]] = g[t].cr; out_state[7 * n + traj[t]] = g[t].cd; out_state[8 * n + traj[t]] = g[t].pm;
-            out_epoch[traj[t]] = epoch[t];
-            if (step_io) step_io[traj[t]] = step_ns[t];
-            if (sink.ev_kind) {
-                const int cnt = (int)g[t].ev[1];
-                sink.ev_crossings[traj[t]] = cnt;
-                if (rc[t] == 0 && cnt < sink.ev_trigger) rc[t] = NYXB_ERR_EVENT_NOT_FOUND;  // event.rs:177-182
-            }
-            out_status[traj[t]] = (status[t] & NYXB_WARN_MAX_ATTEMPTS) | rc[t];
-            if (sink.cap > 0) sink.count[traj[t]] = (n_steps[t] + 1 < sink.cap) ? n_steps[t] + 1 : sink.cap;
-        }
-        if (lane == 7 && out_details) {
-            nyxb_details d;
-            d.step_ns = det_step[t]; d.error = det_error[t]; d.attempts = det_attempts[t]; d._pad = 0;
-            d.n_steps = n_steps[t]; d.n_rejected = n_rej[t]; d.n_rhs = n_rhs[t];
-            out_details[traj[t]] = d;
-        }
+    if (!valid) return;
+    if (lane < 6) out_state[(size_t)lane * n + traj] = yc;
+    if (lane == 6) {
+        out_state[6 * n + traj] = g.cr; out_state[7 * n + traj] = g.cd; out_state[8 * n + traj] = g.pm;
+        out_epoch[traj] = epoch;
+        if (step_io) step_io[traj] = step_ns;
+        out_status[traj] = ctl_finish(sink, traj, status, rc, (int)g.ev[1], n_steps);
+    }
+    if (lane == 7 && out_details) {
+        nyxb_details d;
+        d.step_ns = det_step; d.error = det_error; d.attempts = det_attempts; d._pad = 0;
+        d.n_steps = n_steps; d.n_rejected = n_rej; d.n_rhs = n_rhs;
+        out_details[traj] = d;
     }
 }
 
-template <int G, int T, bool TAB, bool NC>
-static cudaError_t launch_gt(const DevSetup* S, const DevCoop* Cp, size_t n, size_t smem, const double* state,
-                             const double* consts, const long long* epoch0, long long end_epoch, long long* step_io,
-                             double* out_state, long long* out_epoch, nyxb_details* out_details, int* out_status,
-                             const DevSink* sink, cudaStream_t stream) {
-    cudaError_t e = cudaFuncSetAttribute(nyxb_k_coop<G, T, TAB, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+template <int G, bool TAB, bool NC>
+static cudaError_t launch_g(const DevSetup* S, const DevCoop* Cp, size_t n, size_t smem, const double* state,
+                            const double* consts, const long long* epoch0, long long end_epoch, long long* step_io,
+                            double* out_state, long long* out_epoch, nyxb_details* out_details, int* out_status,
+                            const DevSink* sink, cudaStream_t stream) {
+    cudaError_t e = cudaFuncSetAttribute(nyxb_k_coop<G, TAB, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     int dev = 0, sms = 0, occ = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, nyxb_k_coop<G, T, TAB, NC>, COOP_CTA, smem);
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, nyxb_k_coop<G, TAB, NC>, COOP_CTA, smem);
     if (e != cudaSuccess) return e;
     if (occ < 1) occ = 1;
     const size_t groups = COOP_CTA / G;
-    const size_t n_sets = (n + T - 1) / T;
     // one resident wave spread evenly over the SMs when the ensemble fits; otherwise plain tiling
-    size_t grid = (n_sets + groups - 1) / groups;
+    size_t grid = (n + groups - 1) / groups;
     const size_t wave = (size_t)sms * occ;
     if (grid <= wave) grid = ((grid + sms - 1) / sms) * sms;  // one resident wave, same CTA count on every SM
-    nyxb_k_coop<G, T, TAB, NC><<<(unsigned)grid, COOP_CTA, smem, stream>>>(*S, *Cp, n, state, consts, epoch0, end_epoch, step_io,
-                                                                       out_state, out_epoch, out_details, out_status, *sink);
+    nyxb_k_coop<G, TAB, NC><<<(unsigned)grid, COOP_CTA, smem, stream>>>(*S, *Cp, n, state, consts, epoch0, end_epoch, step_io,
+                                                                        out_state, out_epoch, out_details, out_status, *sink);
     return cudaGetLastError();
 }
 
 template <int G>
-cudaError_t nyxb_launch_coop_g(const DevSetup* S, const DevCoop* Cp, int T, size_t n, const double* state, const double* consts,
+cudaError_t nyxb_launch_coop_g(const DevSetup* S, const DevCoop* Cp, size_t n, const double* state, const double* consts,
                                const long long* epoch0, long long end_epoch, long long* step_io, double* out_state,
                                long long* out_epoch, nyxb_details* out_details, int* out_status, const DevSink* sink,
                                cudaStream_t stream) {
     const size_t groups = COOP_CTA / G;
-    const size_t grp_bytes = groups * (size_t)T * coop_traj_stride(S->grav.N) * sizeof(double) + coop_meta_bytes(S->grav.N, G, Cp->kmax);
+    const size_t grp_bytes = groups * coop_traj_stride(S->grav.N) * sizeof(double) + coop_meta_bytes(S->grav.N, G, Cp->kmax);
     const size_t with_table = grp_bytes + coop_rec_bytes(Cp->L, G);
     // stage the record table in shared memory when at least two CTAs still fit per SM (227 KB usable)
     const bool tab = with_table * 2 <= 227 * 1024;
     const size_t smem = tab ? with_table : grp_bytes;
     if (smem > 227 * 1024) return cudaErrorInvalidConfiguration;
-#define NYXB_COOP_GO(TT, TAB) ((S->grav_body >= 0 || S->n_xgrav > 0) ? launch_gt<G, TT, TAB, true>(S, Cp, n, smem, state, consts, epoch0, end_epoch, step_io, out_state, out_epoch, out_details, out_status, sink, stream) : launch_gt<G, TT, TAB, false>(S, Cp, n, smem, state, consts, epoch0, end_epoch, step_io, out_state, out_epoch, out_details, out_status, sink, stream))
-    if (T != 1) return cudaErrorInvalidValue;   // T = 2 (register blocking over two trajectories) lost at every size and is not instantiated
-    return tab ? NYXB_COOP_GO(1, true) : NYXB_COOP_GO(1, false);
+#define NYXB_COOP_GO(TAB) ((S->grav_body >= 0 || S->n_xgrav > 0) ? launch_g<G, TAB, true>(S, Cp, n, smem, state, consts, epoch0, end_epoch, step_io, out_state, out_epoch, out_details, out_status, sink, stream) : launch_g<G, TAB, false>(S, Cp, n, smem, state, consts, epoch0, end_epoch, step_io, out_state, out_epoch, out_details, out_status, sink, stream))
+    return tab ? NYXB_COOP_GO(true) : NYXB_COOP_GO(false);
 #undef NYXB_COOP_GO
 }

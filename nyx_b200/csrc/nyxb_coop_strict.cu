@@ -291,7 +291,7 @@ nyxb_k_coop_strict(const __grid_constant__ DevSetup S, const __grid_constant__ D
         bool last = false;
         const long long prev_step = step_ns;
         const int prev_fixed = fixed;
-        if ((!backprop && epoch + step_ns > stop) || (backprop && epoch + step_ns <= stop)) {
+        if (ctl_past_stop(epoch, step_ns, stop, backprop)) {
             if (stop == epoch) break;
             step_ns = stop - epoch;
             fixed = 1;
@@ -345,32 +345,18 @@ nyxb_k_coop_strict(const __grid_constant__ DevSetup S, const __grid_constant__ D
             y9[6] = g.cr; y9[7] = g.cd; y9[8] = g.pm;
             c9[6] = g.cr + g.hz; c9[7] = g.cd + g.hz; c9[8] = g.pm + g.hz;
             det_error = error_estimate(S.error_ctrl, e9, c9, y9);
-            if (det_error <= S.tolerance || h <= S.min_step_s || det_attempts >= S.attempts) {
+            if (ctl_accept(S, det_error, h, det_attempts)) {
                 bool bad = false;
 #pragma unroll
                 for (int e = 0; e < 9; ++e) bad |= (c9[e] != c9[e]);
                 if (bad) { rc = NYXB_ERR_PROP_MATH; break; }
-                if (det_attempts >= S.attempts) status |= NYXB_WARN_MAX_ATTEMPTS;
-                det_step = dur_from_seconds(h);
-                if (det_error < S.tolerance) {
-                    const double proposed = 0.9 * h * pow_inv_int(S.tolerance / det_error, S.tb.order);
-                    if (fabs(proposed) > fabs(S.max_step_s)) {
-                        const double sg = (proposed != proposed) ? proposed : (signbit(proposed) ? -1.0 : 1.0);
-                        h = S.max_step_s * sg;
-                    } else {
-                        h = proposed;
-                    }
-                }
-                step_ns = dur_from_seconds(h);
-                const long long ab = step_ns < 0 ? -step_ns : step_ns;
-                if (ab < S.min_step_ns) step_ns = (step_ns < 0) ? -S.min_step_ns : S.min_step_ns;
+                step_ns = ctl_accepted<pow_inv_int>(S, det_error, h, det_attempts, status, det_step);
                 dt_ns = det_step;
                 break;
             }
             det_attempts += 1;
             n_rej += 1;
-            const double proposed = 0.9 * h * pow_inv_int(S.tolerance / det_error, S.tb.order - 1);
-            h = (proposed < S.min_step_s) ? S.min_step_s : proposed;
+            h = ctl_retry<pow_inv_int>(S, det_error, h);
             __syncwarp(gmask);
         }
         if (rc) break;
@@ -403,12 +389,7 @@ nyxb_k_coop_strict(const __grid_constant__ DevSetup S, const __grid_constant__ D
         out_state[6 * n + traj] = g.cr; out_state[7 * n + traj] = g.cd; out_state[8 * n + traj] = g.pm;
         out_epoch[traj] = epoch;
         if (step_io) step_io[traj] = step_ns;
-        if (sink.ev_kind) {
-            sink.ev_crossings[traj] = ev_count;
-            if (rc == 0 && ev_count < sink.ev_trigger) rc = NYXB_ERR_EVENT_NOT_FOUND;  // event.rs:177-182
-        }
-        out_status[traj] = (status & NYXB_WARN_MAX_ATTEMPTS) | rc;
-        if (sink.cap > 0) sink.count[traj] = (n_steps + 1 < sink.cap) ? n_steps + 1 : sink.cap;
+        out_status[traj] = ctl_finish(sink, traj, status, rc, ev_count, n_steps);
     }
     if (lane == 7 && out_details) {
         nyxb_details d;

@@ -1,7 +1,8 @@
 // nyxb_device.cuh — device-side data model and right-hand side (force models) of the
 // H100 batched propagator.  Shared by the per-thread kernel (nyxb_kernels.cu, built twice:
-// STRICT = no FMA contraction / reference operation order, FAST = FMA allowed) and by the
-// lane-cooperative kernel (nyxb_coop.cu).
+// STRICT = no FMA contraction / reference operation order, FAST = FMA allowed), the cooperative and
+// transposed kernels (nyxb_coop_kernel.cuh, nyxb_coop_strict.cu, nyxb_tx.cu) and the STM / filter kernels
+// (nyxb_od*.cu).  Every one of them calls the step-size controller defined at the end of this file.
 //
 // Reference behaviour implemented here (paths relative to /root/reference/nyx-core/src):
 //   SpacecraftDynamics::eom   dynamics/spacecraft.rs:191-310
@@ -721,6 +722,30 @@ __device__ inline int eom_full(const DevSetup& S, long long epoch_ns, double del
     return 0;
 }
 
+// Cold part of the right-hand side in the cooperative and transposed kernels, whose harmonic sum is evaluated apart: third bodies,
+// further fields (GEN), SRP and drag added onto acc.  Out of line so that the ephemeris scratch does not inflate the register count
+// of the harmonic sum (scalars, not a context struct, are passed: taking a struct's address would force it into local memory).
+template <bool GEN>
+static __device__ __noinline__ int accel_cold(const DevSetup& S, double dry_mass, double extra_mass, double srp_area, double drag_area,
+                                              long long t_ns, const double y[9], double acc[3]) {
+    const double mass = dry_mass + y[8] + extra_mass;
+    const bool has_force = S.has_srp || S.has_drag;
+    if (has_force && !(mass > 0.0)) return NYXB_ERR_MASSLESS;
+    double bpos[NYXB_MAX_BODIES][3];
+    const int rc = accel_point_masses(S, t_ns, y, bpos, acc);
+    if (rc) return rc;
+    if (GEN && S.n_xgrav > 0) accel_extra_fields(S, t_ns, y, bpos, acc);
+    if (has_force) accel_post(S, t_ns, y, bpos, mass, srp_area, drag_area, acc);
+    return 0;
+}
+
+// position relative to the body the primary field belongs to (gravity_field.rs:149-154); out of line: the Clenshaw scratch must not
+// inflate the register count of the harmonic sum.  An epoch outside the ephemeris is reported by accel_cold, which evaluates every body.
+static __device__ __noinline__ void field_offset(const DevSetup& S, long long t_ns, double& y0, double& y1, double& y2) {
+    double bp[3];
+    if (body_position(S.bodies[S.grav_body], t_ns, bp)) { y0 -= bp[0]; y1 -= bp[1]; y2 -= bp[2]; }
+}
+
 // ---- ErrorControl::estimate (error_ctrl.rs:79-230); err/cand/cur are 9-vectors whose
 // entries 6..8 carry zero error (their derivatives are zero without guidance).
 __device__ __forceinline__ double rss_step3(const double* e, const double* cand, const double* cur) {
@@ -783,4 +808,81 @@ __device__ inline double error_estimate(int ctrl, const double err[9], const dou
         return (mag > 0.1) ? e / mag : e;
     }
     }
+}
+
+// ---- step-size controller of every kernel family (instance.rs:149-196, 416-490).  Each kernel keeps the controller state in its own
+// storage and checks the candidate for NaN itself; ROOT is x^(1/n): pow_inv_int, or the transposed kernel's tx_pow_inv_int.
+// The clamps are NaN-sensitive as written: (p < min) ? min : p is not fmax.
+
+// the final step of a run: the regular step would pass the stop epoch (forward) or reach it (backward)
+__device__ __forceinline__ bool ctl_past_stop(long long epoch, long long step_ns, long long stop, bool backprop) {
+    return backprop ? epoch + step_ns <= stop : epoch + step_ns > stop;
+}
+
+// an attempt of h seconds with error estimate err is accepted
+__device__ __forceinline__ bool ctl_accept(const DevSetup& S, double err, double h, int attempts) {
+    return err <= S.tolerance || h <= S.min_step_s || attempts >= S.attempts;
+}
+
+// after an accepted attempt: the max-attempts warning, the step taken (det_step, ns) and, returned, the step of the next attempt (ns)
+template <double (*ROOT)(double, int)>
+__device__ __forceinline__ long long ctl_accepted(const DevSetup& S, double err, double h, int attempts, int& status, long long& det_step) {
+    if (attempts >= S.attempts) status |= NYXB_WARN_MAX_ATTEMPTS;
+    det_step = dur_from_seconds(h);
+    if (err < S.tolerance) {
+        const double proposed = 0.9 * h * ROOT(S.tolerance / err, S.tb.order);
+        if (fabs(proposed) > fabs(S.max_step_s)) {
+            const double sg = (proposed != proposed) ? proposed : (signbit(proposed) ? -1.0 : 1.0);
+            h = S.max_step_s * sg;
+        } else {
+            h = proposed;
+        }
+    }
+    long long step_ns = dur_from_seconds(h);
+    const long long ab = step_ns < 0 ? -step_ns : step_ns;
+    if (ab < S.min_step_ns) step_ns = (step_ns < 0) ? -S.min_step_ns : S.min_step_ns;
+    return step_ns;
+}
+
+// the step (seconds, unquantised) of the retry after a rejected attempt
+template <double (*ROOT)(double, int)>
+__device__ __forceinline__ double ctl_retry(const DevSetup& S, double err, double h) {
+    const double proposed = 0.9 * h * ROOT(S.tolerance / err, S.tb.order - 1);
+    return (proposed < S.min_step_s) ? S.min_step_s : proposed;
+}
+
+// end of a run of trajectory i: event crossings and event-not-found (event.rs:177-182), the recorded count; returns the status word
+__device__ __forceinline__ int ctl_finish(const DevSink& sink, size_t i, int status, int rc, int crossings, long long n_steps) {
+    if (sink.ev_kind) {
+        sink.ev_crossings[i] = crossings;
+        if (rc == 0 && crossings < sink.ev_trigger) rc = NYXB_ERR_EVENT_NOT_FOUND;
+    }
+    if (sink.cap > 0) sink.count[i] = (n_steps + 1 < sink.cap) ? n_steps + 1 : sink.cap;
+    return (status & NYXB_WARN_MAX_ATTEMPTS) | rc;
+}
+
+// ---- shared-memory addressing and the TMA 1-D bulk copy global -> shared with completion on an mbarrier (SASS: UBLKCP + SYNCS),
+// used by the cooperative and transposed kernels to stage their coefficient tables
+__device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+}
+__device__ __forceinline__ void mbar_expect_tx(unsigned long long* bar, unsigned bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void tma_bulk_g2s(void* dst, const void* src, unsigned bytes, unsigned long long* bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned parity) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "WAIT_LOOP:\n"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
+        "@p bra WAIT_DONE;\n"
+        "bra WAIT_LOOP;\n"
+        "WAIT_DONE:\n"
+        "}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
 }

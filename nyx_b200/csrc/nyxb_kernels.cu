@@ -93,31 +93,17 @@ __device__ static int derive(const DevSetup& S, Inst& in, long long& dt_ns, doub
             return 0;
         }
         in.det_error = error_estimate(S.error_ctrl, err_est, next, in.y);
-        if (in.det_error <= S.tolerance || h <= S.min_step_s || in.det_attempts >= S.attempts) {
+        if (ctl_accept(S, in.det_error, h, in.det_attempts)) {
 #pragma unroll
             for (int e = 0; e < 9; ++e)
                 if (next[e] != next[e]) return NYXB_ERR_PROP_MATH;
-            if (in.det_attempts >= S.attempts) in.status |= NYXB_WARN_MAX_ATTEMPTS;
-            in.det_step_ns = dur_from_seconds(h);
-            if (in.det_error < S.tolerance) {
-                double proposed = 0.9 * h * pow_inv_int(S.tolerance / in.det_error, S.tb.order);
-                if (fabs(proposed) > fabs(S.max_step_s)) {
-                    double sg = (proposed != proposed) ? proposed : (signbit(proposed) ? -1.0 : 1.0);
-                    h = S.max_step_s * sg;
-                } else {
-                    h = proposed;
-                }
-            }
-            in.step_ns = dur_from_seconds(h);
-            long long ab = in.step_ns < 0 ? -in.step_ns : in.step_ns;
-            if (ab < S.min_step_ns) in.step_ns = (in.step_ns < 0) ? -S.min_step_ns : S.min_step_ns;
+            in.step_ns = ctl_accepted<pow_inv_int>(S, in.det_error, h, in.det_attempts, in.status, in.det_step_ns);
             dt_ns = in.det_step_ns;
             return 0;
         }
         in.det_attempts += 1;
         in.n_rejected += 1;
-        double proposed = 0.9 * h * pow_inv_int(S.tolerance / in.det_error, S.tb.order - 1);
-        h = (proposed < S.min_step_s) ? S.min_step_s : proposed;
+        h = ctl_retry<pow_inv_int>(S, in.det_error, h);
     }
 }
 
@@ -155,7 +141,7 @@ __device__ static int propagate(const DevSetup& S, Inst& in, long long duration_
     if (backprop) in.step_ns = -in.step_ns;
     for (;;) {
         long long epoch = in.epoch_ns;
-        if ((!backprop && epoch + in.step_ns > stop) || (backprop && epoch + in.step_ns <= stop)) {
+        if (ctl_past_stop(epoch, in.step_ns, stop, backprop)) {
             if (stop == epoch) return 0;
             long long prev_step = in.step_ns;
             int prev_fixed = in.fixed;
@@ -204,12 +190,7 @@ NYXB_KTHREAD(const __grid_constant__ DevSetup S, size_t n,
     record_state(in, 0);  // start state (instance.rs:307, 321)
     in.ev_count = 0;
     in.ev_prev = sink.ev_kind ? event_eval(sink.ev_kind, sink.ev_value, in.y[0], in.y[1], in.y[2], in.y[3], in.y[4], in.y[5]) : 0.0;
-    int rc = propagate<GRAV>(S, in, end_epoch - in.epoch_ns);
-    if (sink.ev_kind) {
-        sink.ev_crossings[i] = in.ev_count;
-        if (rc == 0 && in.ev_count < sink.ev_trigger) rc = NYXB_ERR_EVENT_NOT_FOUND;  // event.rs:177-182
-    }
-    if (sink.cap > 0) sink.count[i] = (in.n_steps + 1 < sink.cap) ? in.n_steps + 1 : sink.cap;
+    const int rc = propagate<GRAV>(S, in, end_epoch - in.epoch_ns);
 #pragma unroll
     for (int e = 0; e < 9; ++e) out_state[(size_t)e * n + i] = in.y[e];
     out_epoch[i] = in.epoch_ns;
@@ -220,7 +201,7 @@ NYXB_KTHREAD(const __grid_constant__ DevSetup S, size_t n,
         d.n_steps = in.n_steps; d.n_rejected = in.n_rejected; d.n_rhs = in.n_rhs;
         out_details[i] = d;
     }
-    out_status[i] = (in.status & NYXB_WARN_MAX_ATTEMPTS) | rc;
+    out_status[i] = ctl_finish(sink, i, in.status, rc, in.ev_count, in.n_steps);
 }
 
 extern "C" cudaError_t NYXB_LAUNCH_THREAD(const DevSetup* S, size_t n, const double* state, const double* consts,

@@ -281,30 +281,16 @@ __device__ static int derive_coop(const Ctx& cx, InstC& in, long long& dt_ns, do
             return 0;
         }
         in.det_error = error_estimate(S.error_ctrl, err_est, next, in.y);
-        if (in.det_error <= S.tolerance || h <= S.min_step_s || in.det_attempts >= S.attempts) {
+        if (ctl_accept(S, in.det_error, h, in.det_attempts)) {
             for (int e = 0; e < 9; ++e) bad = bad || (next[e] != next[e]);
             if (__any_sync(FULL, bad)) return NYXB_ERR_PROP_MATH;
-            if (in.det_attempts >= S.attempts) in.status |= NYXB_WARN_MAX_ATTEMPTS;
-            in.det_step_ns = dur_from_seconds(h);
-            if (in.det_error < S.tolerance) {
-                double proposed = 0.9 * h * pow_inv_int(S.tolerance / in.det_error, S.tb.order);
-                if (fabs(proposed) > fabs(S.max_step_s)) {
-                    double sg = (proposed != proposed) ? proposed : (signbit(proposed) ? -1.0 : 1.0);
-                    h = S.max_step_s * sg;
-                } else {
-                    h = proposed;
-                }
-            }
-            in.step_ns = dur_from_seconds(h);
-            long long ab = in.step_ns < 0 ? -in.step_ns : in.step_ns;
-            if (ab < S.min_step_ns) in.step_ns = (in.step_ns < 0) ? -S.min_step_ns : S.min_step_ns;
+            in.step_ns = ctl_accepted<pow_inv_int>(S, in.det_error, h, in.det_attempts, in.status, in.det_step_ns);
             dt_ns = in.det_step_ns;
             return 0;
         }
         in.det_attempts += 1;
         in.n_rejected += 1;
-        double proposed = 0.9 * h * pow_inv_int(S.tolerance / in.det_error, S.tb.order - 1);
-        h = (proposed < S.min_step_s) ? S.min_step_s : proposed;
+        h = ctl_retry<pow_inv_int>(S, in.det_error, h);
     }
 }
 
@@ -331,7 +317,7 @@ __device__ static int propagate_coop(const Ctx& cx, InstC& in, long long duratio
     if (backprop) in.step_ns = -in.step_ns;
     for (;;) {
         long long epoch = in.epoch_ns;
-        if ((!backprop && epoch + in.step_ns > stop) || (backprop && epoch + in.step_ns <= stop)) {
+        if (ctl_past_stop(epoch, in.step_ns, stop, backprop)) {
             if (stop == epoch) return 0;
             long long prev_step = in.step_ns;
             int prev_fixed = in.fixed;

@@ -36,18 +36,9 @@
 #define TX_MINB 2   /* resident CTAs per SM the kernel is compiled for (register cap 65536 / (256 * TX_MINB)) */
 #endif
 
-#ifndef NYXB_TX_TT
-#define NYXB_TX_TT 1
-#endif
-
 namespace {
-// TT = 1 (the build): a set is 32 trajectories, a walker lane carries one.  TT = 2 (-DNYXB_TX_TT=2, not built, not dispatched): a set
-// is 64 trajectories, a walker lane carries trajectories l and l + 32 through the same record loads (half the shared-memory
-// wavefronts per FP64 instruction) and every helper role is played by two warps — but then only ONE set context fits a CTA's
-// registers, and the serial stretch between two attempts is no longer covered by a second set.
-constexpr int TT = NYXB_TX_TT;
-constexpr int NL = 32 * TT;    // trajectories per set: stride of every per-trajectory shared-memory array
-constexpr int HW = 3 * TT;     // helper warps per set context
+constexpr int NL = 32;   // trajectories per set, one per lane: stride of every per-trajectory shared-memory array
+constexpr int HW = 3;    // helper warps per set context
 constexpr unsigned FULL = 0xffffffffu;
 
 // ---- per-trajectory controller state kept in shared memory ([field][lane])
@@ -117,30 +108,6 @@ __device__ __forceinline__ TxSm tx_views(unsigned char* smem, const TxLayout& L,
 __device__ __forceinline__ void nb_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 __device__ __forceinline__ void nb_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
-__device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void tx_mbar_init(unsigned long long* bar, unsigned count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void tx_mbar_expect(unsigned long long* bar, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tx_bulk_g2s(void* dst, const void* src, unsigned bytes, unsigned long long* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tx_mbar_wait(unsigned long long* bar, unsigned parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "TX_WAIT_LOOP:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra TX_WAIT_DONE;\n"
-        "bra TX_WAIT_LOOP;\n"
-        "TX_WAIT_DONE:\n"
-        "}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-
 __device__ __forceinline__ void tx_mbar_arrive(unsigned long long* bar) {   // release.cta: the thread's earlier shared stores are published
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
@@ -171,27 +138,6 @@ enum { TR_POLL = 1, TR_WALK = 2, TR_WALK_END = 3, TR_DONE_WAIT = 4, TR_DONE_SEEN
 #define TX_TRACE(code, ctx, stg) do { } while (0)
 #endif
 
-// third bodies + SRP + drag for one trajectory (cold path of the harmonics-dominated ensembles this kernel serves)
-__device__ __noinline__ int tx_extra(const DevSetup& S, double dry_mass, double extra_mass, double srp_area, double drag_area,
-                                     long long t_ns, const double y[9], double acc[3]) {
-    const double mass = dry_mass + y[8] + extra_mass;
-    const bool has_force = S.has_srp || S.has_drag;
-    if (has_force && !(mass > 0.0)) return NYXB_ERR_MASSLESS;
-    double bpos[NYXB_MAX_BODIES][3];
-    const int rc = accel_point_masses(S, t_ns, y, bpos, acc);
-    if (rc) return rc;
-    if (S.n_xgrav > 0) accel_extra_fields(S, t_ns, y, bpos, acc);
-    if (has_force) accel_post(S, t_ns, y, bpos, mass, srp_area, drag_area, acc);
-    return 0;
-}
-
-// position relative to the body the primary field belongs to (gravity_field.rs:149-154); an epoch outside the ephemeris is reported
-// by tx_extra, which evaluates every body
-__device__ __noinline__ void tx_field_offset(const DevSetup& S, long long t_ns, double& y0, double& y1, double& y2) {
-    double bp[3];
-    if (body_position(S.bodies[S.grav_body], t_ns, bp)) { y0 -= bp[0]; y1 -= bp[1]; y2 -= bp[2]; }
-}
-
 // ---- one column of the walk.  (a01, a23, kk) hold the column's first record (prefetched); A / K point at it; on return they hold
 // the first record of the next column.
 // Entry n of column m (record p1..p4, kappa; Q = Q[n], Qn = Q[n+1]):
@@ -202,7 +148,7 @@ __device__ __noinline__ void tx_field_offset(const DevSetup& S, long long t_ns, 
 // warps per scheduler keep the FP64 pipe fed.  12 FP64 instructions per entry.  The loop is unrolled by hand over two register
 // sets for the prefetched record so that no register-to-register moves are left in it (the compiler's own rotation cost 14
 // IMAD.MOV per two entries and made the loop issue-bound).
-// per-trajectory registers of a walker lane (TT of them)
+// registers of a walker lane (its trajectory)
 struct TxLaneState {
     double ub, r2, dc, dg;                  // u rho, rho^2 and their doubles
     double zar, zai, pa, zbr, zbi, pb;      // current powers of the two exponent sequences
@@ -211,32 +157,28 @@ struct TxLaneState {
     double cQ, cc1, cg, cS5, cS6;           // set-up of the column about to be walked
 };
 #define NYXB_TX_ENTRY(P01, P23, PK)                             \
-    _Pragma("unroll") for (int u = 0; u < TT; ++u) {            \
-        const double Qn = fma(c1[u], Q[u], -m2[u]);             \
-        c1[u] += t[u].dc; d[u] += g[u]; g[u] += t[u].dg;        \
-        m2[u] = d[u] * Q[u];                                    \
-        S1[u] = fma(Q[u], (P01).x, S1[u]);                      \
-        S2[u] = fma(Q[u], (P01).y, S2[u]);                      \
-        S3[u] = fma(Q[u], (P23).x, S3[u]);                      \
-        S4[u] = fma(Q[u], (P23).y, S4[u]);                      \
+    {                                                           \
+        const double Qn = fma(c1, Q, -m2);                      \
+        c1 += t.dc; d += g; g += t.dg;                          \
+        m2 = d * Q;                                             \
+        S1 = fma(Q, (P01).x, S1);                               \
+        S2 = fma(Q, (P01).y, S2);                               \
+        S3 = fma(Q, (P23).x, S3);                               \
+        S4 = fma(Q, (P23).y, S4);                               \
         const double wv = (PK) * Qn;                            \
-        S5[u] = fma(wv, (P23).x, S5[u]);                        \
-        S6[u] = fma(wv, (P23).y, S6[u]);                        \
-        Q[u] = Qn;                                              \
+        S5 = fma(wv, (P23).x, S5);                              \
+        S6 = fma(wv, (P23).y, S6);                              \
+        Q = Qn;                                                 \
     }
-// t[u].(cQ, cc1, cg, cS5, cS6) arrive set up for this column — Q = rho^m x seed, c1 = (2m+1) u rho, g = (2m+1) rho^2, S5 / S6 the
+// t.(cQ, cc1, cg, cS5, cS6) arrive set up for this column — Q = rho^m x seed, c1 = (2m+1) u rho, g = (2m+1) rho^2, S5 / S6 the
 // column's seed W term — because the caller sets the NEXT column up right behind the close of this one, in the same basic block, so
-// the two short dependent chains overlap.  Every record load serves the TT trajectories of the lane.
+// the two short dependent chains overlap.
 template <bool SEQ_B>
 __device__ __forceinline__ void tx_column(const double2*& A, const double*& K, double2& a01, double2& a23, double& kk, int len,
-                                          TxLaneState (&t)[TT]) {
-    double Q[TT], c1[TT], g[TT], m2[TT], d[TT], S1[TT], S2[TT], S3[TT], S4[TT], S5[TT], S6[TT];
-#pragma unroll
-    for (int u = 0; u < TT; ++u) {
-        Q[u] = t[u].cQ; c1[u] = t[u].cc1; g[u] = t[u].cg; S5[u] = t[u].cS5; S6[u] = t[u].cS6;
-        m2[u] = 0.0; d[u] = 0.0;   // entry n = m: (n+m)(n-m) = 0
-        S1[u] = 0.0; S2[u] = 0.0; S3[u] = 0.0; S4[u] = 0.0;
-    }
+                                          TxLaneState& t) {
+    double Q = t.cQ, c1 = t.cc1, g = t.cg, S5 = t.cS5, S6 = t.cS6;
+    double m2 = 0.0, d = 0.0;   // entry n = m: (n+m)(n-m) = 0
+    double S1 = 0.0, S2 = 0.0, S3 = 0.0, S4 = 0.0;
     double2 b01, b23;
     double bk;
 #pragma unroll 2
@@ -248,14 +190,11 @@ __device__ __forceinline__ void tx_column(const double2*& A, const double*& K, d
         A += 4; K += 2;
     }
     // close the column: apply its (cos, sin)((m-1) lambda) cos^(m-1)(phi)
-#pragma unroll
-    for (int u = 0; u < TT; ++u) {
-        const double rr = SEQ_B ? t[u].zbr : t[u].zar, ii = SEQ_B ? t[u].zbi : t[u].zai;
-        t[u].X = fma(rr, S1[u], fma(ii, S2[u], t[u].X));
-        t[u].Y = fma(rr, S2[u], fma(-ii, S1[u], t[u].Y));
-        t[u].Z = fma(rr, S3[u], fma(ii, S4[u], t[u].Z));
-        t[u].W = fma(rr, S5[u], fma(ii, S6[u], t[u].W));
-    }
+    const double rr = SEQ_B ? t.zbr : t.zar, ii = SEQ_B ? t.zbi : t.zai;
+    t.X = fma(rr, S1, fma(ii, S2, t.X));
+    t.Y = fma(rr, S2, fma(-ii, S1, t.Y));
+    t.Z = fma(rr, S3, fma(ii, S4, t.Z));
+    t.W = fma(rr, S5, fma(ii, S6, t.W));
 }
 
 // ---- instance.rs:149-196: choose the step of the next attempt (regular, or the final fixed step to the stop time)
@@ -268,7 +207,7 @@ __device__ __forceinline__ void tx_pick_step(const TxSm& sm, int lane, long long
         fl &= ~(F_LAST | F_PREVFIXED);
         if (fl & F_FIXED) fl |= F_PREVFIXED;
         sm.i64[TXI_PREV_STEP * NL + lane] = step_ns;
-        if ((!back && epoch + step_ns > stop) || (back && epoch + step_ns <= stop)) {
+        if (ctl_past_stop(epoch, step_ns, stop, back)) {
             if (stop == epoch) {
                 fl |= F_DONE;
             } else {
@@ -350,8 +289,8 @@ __device__ __noinline__ void tx_controller(const DevSetup& S, const DevSink& sin
         c9[6] = cr + hz; c9[7] = cd + hz; c9[8] = pm + hz;
         const double err = error_estimate(S.error_ctrl, e9, c9, y9);
         sm.f64[TXF_ERR * NL + lane] = err;
-        int att = sm.i32[TXW_ATT * NL + lane];
-        accept = err <= S.tolerance || h <= S.min_step_s || att >= S.attempts;
+        const int att = sm.i32[TXW_ATT * NL + lane];
+        accept = ctl_accept(S, err, h, att);
         if (accept) {
             bool bad = false;
 #pragma unroll
@@ -361,28 +300,14 @@ __device__ __noinline__ void tx_controller(const DevSetup& S, const DevSink& sin
                 sm.i32[TXW_FLAGS * NL + lane] = fl | F_DONE;
                 return;
             }
-            if (att >= S.attempts) sm.i32[TXW_STATUS * NL + lane] |= NYXB_WARN_MAX_ATTEMPTS;
-            const long long det_step = dur_from_seconds(h);
+            long long det_step;
+            step_ns = ctl_accepted<tx_pow_inv_int>(S, err, h, att, sm.i32[TXW_STATUS * NL + lane], det_step);
             sm.i64[TXI_DET_STEP * NL + lane] = det_step;
-            double hn = h;
-            if (err < S.tolerance) {
-                const double proposed = 0.9 * h * tx_pow_inv_int(S.tolerance / err, S.tb.order);
-                if (fabs(proposed) > fabs(S.max_step_s)) {
-                    const double sg = (proposed != proposed) ? proposed : (signbit(proposed) ? -1.0 : 1.0);
-                    hn = S.max_step_s * sg;
-                } else {
-                    hn = proposed;
-                }
-            }
-            step_ns = dur_from_seconds(hn);
-            const long long ab = step_ns < 0 ? -step_ns : step_ns;
-            if (ab < S.min_step_ns) step_ns = (step_ns < 0) ? -S.min_step_ns : S.min_step_ns;
             dt_ns = det_step;
         } else {
             sm.i32[TXW_ATT * NL + lane] = att + 1;
             sm.i64[TXI_NREJ * NL + lane] += 1;
-            const double proposed = 0.9 * h * tx_pow_inv_int(S.tolerance / err, S.tb.order - 1);
-            sm.f64[TXF_H * NL + lane] = (proposed < S.min_step_s) ? S.min_step_s : proposed;
+            sm.f64[TXF_H * NL + lane] = ctl_retry<tx_pow_inv_int>(S, err, h);
             sm.i32[TXW_FLAGS * NL + lane] = fl | F_RETRY;
             return;
         }
@@ -510,15 +435,8 @@ __device__ __noinline__ void tx_park_ctl(const DevSink& sink, const DevTxQueue& 
     d.n_rejected = sm.i64[TXI_NREJ * NL + lane];
     d.n_rhs = sm.i64[TXI_NRHS * NL + lane];
     q.details[tr] = d;
-    int rc_out = rc;
-    if (sink.ev_kind) {
-        const int cnt = sm.i32[TXW_EVCNT * NL + lane];
-        sink.ev_crossings[tr] = cnt;
-        if (rc == 0 && cnt < sink.ev_trigger) rc_out = NYXB_ERR_EVENT_NOT_FOUND;   // event.rs:177-182 (final once the run is done)
-    }
-    out_status[tr] = (st & NYXB_WARN_MAX_ATTEMPTS) | rc_out;
+    out_status[tr] = ctl_finish(sink, tr, st, rc, sm.i32[TXW_EVCNT * NL + lane], d.n_steps);   // final once the run is done
     if (step_io) step_io[tr] = step_ns;
-    if (sink.cap > 0) sink.count[tr] = (d.n_steps + 1 < sink.cap) ? d.n_steps + 1 : sink.cap;
 }
 
 // ---- prologue of stage q for the 32 trajectories of a set, run by the lead helper: body-fixed position, 1/r, the recursion
@@ -546,7 +464,7 @@ __device__ __forceinline__ void tx_prologue(const DevSetup& S, const TxSm& sm, i
     double ir_c = 0.0;   // 1/|r| about the integration centre (two-body term)
     if (S.grav_body >= 0) {   // field of another body: the state is translated to it first (gravity_field.rs:149-154)
         ir_c = rsqrt(fma(y2, y2, fma(y1, y1, y0 * y0)));
-        tx_field_offset(S, t_ns, y0, y1, y2);
+        field_offset(S, t_ns, y0, y1, y2);
     }
     const double rb0 = fma(rn[2 * NL], y2, fma(rn[1 * NL], y1, rn[0] * y0));
     const double rb1 = fma(rn[5 * NL], y2, fma(rn[4 * NL], y1, rn[3 * NL] * y0));
@@ -709,7 +627,7 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
     // context has a stage ready, so the serial stretch between two step attempts of one set (error norm, controller, commit,
     // first prologue) is covered by the other set's stages instead of stalling the walkers.
     __shared__ __align__(8) unsigned long long ready_bar[NCTX][2];
-    __shared__ int s_set[NCTX], s_fresh[NCTX], s_exit[NCTX], s_done_half[NCTX][TT], s_slice_end[NCTX];
+    __shared__ int s_set[NCTX], s_fresh[NCTX], s_exit[NCTX], s_done[NCTX], s_slice_end[NCTX];
     __shared__ __align__(8) unsigned long long kick_bar;   // context 0 arrives half-way through its first attempt: context 1 starts then
     const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
 #ifdef NYXB_TX_TRACE
@@ -717,7 +635,6 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
 #endif
     constexpr int NPOW = 6;   // P = 16: z^(2^k), k < NPOW: bits of the exponents below 2P, and the common ratio z^(2P)
     static_assert(P == 8 || P == 10 || P == 16, "walker positions");
-    static_assert(TT == 1 || NCTX == 1, "sets of 64 trajectories: one set context per CTA");
     constexpr int NT_RW = (P + HW) * 32;
     constexpr int NT_HB = HW * 32;   // threads on the helpers' own barrier   // threads on a READY / DONE barrier: the walkers + the three helpers of the context
     // named barriers of context c: HB (helpers among themselves), READY[parity], DONE[parity]
@@ -732,22 +649,22 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
 
     // ---- CTA-shared tables (records, column seeds, schedule): ONE TMA bulk copy
     if (tid == 0) {
-        tx_mbar_init(&tma_bar, 1);
+        mbar_init(&tma_bar, 1);
 #pragma unroll
-        tx_mbar_init(&kick_bar, 1);
+        mbar_init(&kick_bar, 1);
 #pragma unroll
         for (int c = 0; c < NCTX; ++c) {
             s_exit[c] = 0;
-            tx_mbar_init(&ready_bar[c][0], NT_HB);
-            tx_mbar_init(&ready_bar[c][1], NT_HB);
+            mbar_init(&ready_bar[c][0], NT_HB);
+            mbar_init(&ready_bar[c][1], NT_HB);
         }
     }
     __syncthreads();
     if (tid == 0) {
-        tx_mbar_expect(&tma_bar, blob_bytes);
-        tx_bulk_g2s(smem + L.blob, Tx.recA, blob_bytes, &tma_bar);
+        mbar_expect_tx(&tma_bar, blob_bytes);
+        tma_bulk_g2s(smem + L.blob, Tx.recA, blob_bytes, &tma_bar);
     }
-    tx_mbar_wait(&tma_bar, 0);
+    mbar_wait(&tma_bar, 0);
     __syncthreads();   // the last CTA-wide barrier: from here on walkers and helpers meet on named barriers only
 
     if (w < P) {
@@ -794,32 +711,29 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
                 const TxSm sm = tx_views(smem, L, c, N);
                 // z^e = (cos, sin)(e lambda) cos^e(phi) and rho^(e+1) for the two interleaved exponent sequences of this position:
                 // e = pos + 2P j (za, pa) and e = 2P-1-pos + 2P j (zb, pb)
-                TxLaneState t[TT];
-#pragma unroll
-                for (int u = 0; u < TT; ++u) {
-                    const double* wk = sm.wk + par * TxWk<P>::COUNT * NL + u * 32 + lane;
-                    t[u].ub = wk[WK_UB * NL]; t[u].r2 = wk[WK_R2 * NL];
-                    t[u].dc = t[u].ub + t[u].ub; t[u].dg = t[u].r2 + t[u].r2;
-                    if constexpr (TxWk<P>::ALL) {   // published: z^pos, z^(2P-1-pos), z^(2P), rho^(pos+1), rho^(2P-pos), rho^(2P)
-                        constexpr int E = TxWk<P>::E;
-                        t[u].zar = wk[(TxWk<P>::ZR + pos) * NL]; t[u].zai = wk[(TxWk<P>::ZI + pos) * NL];
-                        t[u].pa = wk[(TxWk<P>::RH + pos + 1) * NL];
-                        t[u].zbr = wk[(TxWk<P>::ZR + E - 1 - pos) * NL]; t[u].zbi = wk[(TxWk<P>::ZI + E - 1 - pos) * NL];
-                        t[u].pb = wk[(TxWk<P>::RH + E - pos) * NL];
-                        t[u].qr = wk[(TxWk<P>::ZR + E) * NL]; t[u].qi = wk[(TxWk<P>::ZI + E) * NL]; t[u].qp = wk[(TxWk<P>::RH + E) * NL];
-                    } else {
-                        switch (pos) {   // one specialised copy per position: the choices below are compile-time there
-#define NYXB_TX_CASE(WW) case WW: tx_start_powers<WW, NPOW - 1>(wk, t[u].zar, t[u].zai, t[u].pa, t[u].zbr, t[u].zbi, t[u].pb); break;
-                            NYXB_TX_CASE(0) NYXB_TX_CASE(1) NYXB_TX_CASE(2) NYXB_TX_CASE(3) NYXB_TX_CASE(4) NYXB_TX_CASE(5) NYXB_TX_CASE(6) NYXB_TX_CASE(7)
-                            NYXB_TX_CASE(8) NYXB_TX_CASE(9) NYXB_TX_CASE(10) NYXB_TX_CASE(11) NYXB_TX_CASE(12) NYXB_TX_CASE(13) NYXB_TX_CASE(14)
-                            default: tx_start_powers<15, NPOW - 1>(wk, t[u].zar, t[u].zai, t[u].pa, t[u].zbr, t[u].zbi, t[u].pb); break;
+                TxLaneState t;
+                const double* wk = sm.wk + par * TxWk<P>::COUNT * NL + lane;
+                t.ub = wk[WK_UB * NL]; t.r2 = wk[WK_R2 * NL];
+                t.dc = t.ub + t.ub; t.dg = t.r2 + t.r2;
+                if constexpr (TxWk<P>::ALL) {   // published: z^pos, z^(2P-1-pos), z^(2P), rho^(pos+1), rho^(2P-pos), rho^(2P)
+                    constexpr int E = TxWk<P>::E;
+                    t.zar = wk[(TxWk<P>::ZR + pos) * NL]; t.zai = wk[(TxWk<P>::ZI + pos) * NL];
+                    t.pa = wk[(TxWk<P>::RH + pos + 1) * NL];
+                    t.zbr = wk[(TxWk<P>::ZR + E - 1 - pos) * NL]; t.zbi = wk[(TxWk<P>::ZI + E - 1 - pos) * NL];
+                    t.pb = wk[(TxWk<P>::RH + E - pos) * NL];
+                    t.qr = wk[(TxWk<P>::ZR + E) * NL]; t.qi = wk[(TxWk<P>::ZI + E) * NL]; t.qp = wk[(TxWk<P>::RH + E) * NL];
+                } else {
+                    switch (pos) {   // one specialised copy per position: the choices below are compile-time there
+#define NYXB_TX_CASE(WW) case WW: tx_start_powers<WW, NPOW - 1>(wk, t.zar, t.zai, t.pa, t.zbr, t.zbi, t.pb); break;
+                        NYXB_TX_CASE(0) NYXB_TX_CASE(1) NYXB_TX_CASE(2) NYXB_TX_CASE(3) NYXB_TX_CASE(4) NYXB_TX_CASE(5) NYXB_TX_CASE(6) NYXB_TX_CASE(7)
+                        NYXB_TX_CASE(8) NYXB_TX_CASE(9) NYXB_TX_CASE(10) NYXB_TX_CASE(11) NYXB_TX_CASE(12) NYXB_TX_CASE(13) NYXB_TX_CASE(14)
+                        default: tx_start_powers<15, NPOW - 1>(wk, t.zar, t.zai, t.pa, t.zbr, t.zbi, t.pb); break;
 #undef NYXB_TX_CASE
-                        }
-                        t[u].qr = wk[(WK_POW + 3 * (NPOW - 1)) * NL]; t[u].qi = wk[(WK_POW + 3 * (NPOW - 1) + 1) * NL];   // z^(2P)
-                        t[u].qp = wk[(WK_POW + 3 * (NPOW - 1) + 2) * NL];                                             // rho^(2P)
                     }
-                    t[u].X = 0.0; t[u].Y = 0.0; t[u].Z = 0.0; t[u].W = 0.0;
+                    t.qr = wk[(WK_POW + 3 * (NPOW - 1)) * NL]; t.qi = wk[(WK_POW + 3 * (NPOW - 1) + 1) * NL];   // z^(2P)
+                    t.qp = wk[(WK_POW + 3 * (NPOW - 1) + 2) * NL];                                             // rho^(2P)
                 }
+                t.X = 0.0; t.Y = 0.0; t.Z = 0.0; t.W = 0.0;
                 const double2* A = recA + 2 * rec_off;
                 const double* K = recK + rec_off;
                 double2 a01 = A[0], a23 = A[1];
@@ -829,11 +743,8 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
                 int len = my[3];
                 {
                     const double4 sd = *reinterpret_cast<const double4*>(colseed + 4 * my[2]);
-#pragma unroll
-                    for (int u = 0; u < TT; ++u) {
-                        t[u].cQ = t[u].pa * sd.x; t[u].cc1 = sd.w * t[u].ub; t[u].cg = sd.w * t[u].r2;
-                        t[u].cS5 = t[u].cQ * sd.y; t[u].cS6 = t[u].cQ * sd.z;
-                    }
+                    t.cQ = t.pa * sd.x; t.cc1 = sd.w * t.ub; t.cg = sd.w * t.r2;
+                    t.cS5 = t.cQ * sd.y; t.cS6 = t.cQ * sd.z;
                 }
                 // two columns per trip: the first belongs to sequence a, the second to sequence b (no exchange of the two register
                 // sets); the set-up of the next column needs only the OTHER sequence's rho power, which is already there, and the
@@ -843,13 +754,10 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
                         const int len_n = my[5 + 2 * k];   // the schedule rows end with a null column (all-zero seeds)
                         const double4 sd_n = *reinterpret_cast<const double4*>(colseed + 4 * my[4 + 2 * k]);
                         tx_column<false>(A, K, a01, a23, kk, len, t);
-#pragma unroll
-                        for (int u = 0; u < TT; ++u) {
-                            t[u].cQ = t[u].pb * sd_n.x; t[u].cc1 = sd_n.w * t[u].ub; t[u].cg = sd_n.w * t[u].r2;
-                            t[u].cS5 = t[u].cQ * sd_n.y; t[u].cS6 = t[u].cQ * sd_n.z;
-                            const double nr = fma(t[u].zar, t[u].qr, -(t[u].zai * t[u].qi));
-                            t[u].zai = fma(t[u].zar, t[u].qi, t[u].zai * t[u].qr); t[u].zar = nr; t[u].pa *= t[u].qp;
-                        }
+                        t.cQ = t.pb * sd_n.x; t.cc1 = sd_n.w * t.ub; t.cg = sd_n.w * t.r2;
+                        t.cS5 = t.cQ * sd_n.y; t.cS6 = t.cQ * sd_n.z;
+                        const double nr = fma(t.zar, t.qr, -(t.zai * t.qi));
+                        t.zai = fma(t.zar, t.qi, t.zai * t.qr); t.zar = nr; t.pa *= t.qp;
                         len = len_n;
                     }
                     if (k + 1 >= ncol) break;
@@ -857,21 +765,15 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
                         const int len_n = my[7 + 2 * k];
                         const double4 sd_n = *reinterpret_cast<const double4*>(colseed + 4 * my[6 + 2 * k]);
                         tx_column<true>(A, K, a01, a23, kk, len, t);
-#pragma unroll
-                        for (int u = 0; u < TT; ++u) {
-                            t[u].cQ = t[u].pa * sd_n.x; t[u].cc1 = sd_n.w * t[u].ub; t[u].cg = sd_n.w * t[u].r2;
-                            t[u].cS5 = t[u].cQ * sd_n.y; t[u].cS6 = t[u].cQ * sd_n.z;
-                            const double nr = fma(t[u].zbr, t[u].qr, -(t[u].zbi * t[u].qi));
-                            t[u].zbi = fma(t[u].zbr, t[u].qi, t[u].zbi * t[u].qr); t[u].zbr = nr; t[u].pb *= t[u].qp;
-                        }
+                        t.cQ = t.pa * sd_n.x; t.cc1 = sd_n.w * t.ub; t.cg = sd_n.w * t.r2;
+                        t.cS5 = t.cQ * sd_n.y; t.cS6 = t.cQ * sd_n.z;
+                        const double nr = fma(t.zbr, t.qr, -(t.zbi * t.qi));
+                        t.zbi = fma(t.zbr, t.qi, t.zbi * t.qr); t.zbr = nr; t.pb *= t.qp;
                         len = len_n;
                     }
                 }
-#pragma unroll
-                for (int u = 0; u < TT; ++u) {
-                    double* pt = sm.part + ((par * P + pos) * 4) * NL + u * 32 + lane;
-                    pt[0] = t[u].X; pt[NL] = t[u].Y; pt[2 * NL] = t[u].Z; pt[3 * NL] = t[u].W;
-                }
+                double* pt = sm.part + ((par * P + pos) * 4) * NL + lane;
+                pt[0] = t.X; pt[NL] = t.Y; pt[2 * NL] = t.Z; pt[3 * NL] = t.W;
                 nb_arrive(1 + c * BAR_PER_CTX + 3 + par, NT_RW);   // DONE[par]: the partial sums of this position are in shared memory
                 TX_TRACE(TR_WALK_END, c, st);
             }
@@ -880,21 +782,13 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
     }
 
     // =================================================================================================== HELPER
-    // set context; helper role j: owns state components j (position) and j + 3 (velocity); TT = 2: half of the set this warp serves
-    const int c = (w - P) / HW, j = ((w - P) % HW) % 3, half = ((w - P) % HW) / 3;
-    const int tl = half * 32 + lane;   // trajectory of this thread inside the set
+    // set context; helper role j: owns state components j (position) and j + 3 (velocity) of trajectory `lane` of the set
+    const int c = (w - P) / HW, j = (w - P) % HW;
     const TxSm sm = tx_views(smem, L, c, N);
     const int BAR_HB = 1 + c * BAR_PER_CTX, BAR_DONE = BAR_HB + 3;
     const DevGrav& gv = S.grav;
     const bool has_extra = S.n_bodies > 0 || S.has_srp || S.has_drag || S.n_xgrav > 0;
-    const bool lead = (j == 0);   // helper 0 also runs the DCM, the controller (of its half of the set) and, half 0, the set queue
-    const bool lead0 = lead && half == 0;
-    // every trajectory of the set is done (read between the helpers' barriers that follow the votes of the leads)
-    auto set_done = [&]() {
-        bool d = s_done_half[c][0] != 0;
-        if (TT == 2) d = d && s_done_half[c][TT - 1] != 0;
-        return d;
-    };
+    const bool lead = (j == 0);   // helper 0 also runs the DCM, the controller and the set queue
     const double* ta = S.tb.a;    // a_{q,m} (stage q >= 1, m < q) = ta[(q - 1) * NYXB_MAX_STAGES + m]
 
     // The two sets of a CTA must not reach the serial stretch between two attempts (error norm, controller, commit, first
@@ -903,13 +797,13 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
     // every such stretch).  Context 1 therefore starts when context 0 is half-way through its first attempt.
     bool kick_pending = (NCTX > 1 && c == 0);
     if (NCTX > 1 && c == 1) {
-        if (lead0 && lane == 0) tx_mbar_wait(&kick_bar, 0);
+        if (lead && lane == 0) mbar_wait(&kick_bar, 0);
         nb_sync(BAR_HB, NT_HB);
     }
 
     for (;;) {
         // ---------------------------------------------------------------- acquire a set: a fresh one, else a parked one
-        if (lead0 && lane == 0) {
+        if (lead && lane == 0) {
             int set = -1, fresh = 0;
             if (atomicAdd(q.ctl + TXQ_FRESH, 0) < q.n_sets) {
                 const int f = atomicAdd(q.ctl + TXQ_FRESH, 1);
@@ -931,14 +825,14 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
             s_exit[c] = set < 0;   // nothing fresh, nothing parked: every unfinished set is in progress in another context
         }
         nb_sync(BAR_HB, NT_HB);
-        if (s_exit[c] && kick_pending && lead0 && lane == 0) tx_mbar_arrive(&kick_bar);
+        if (s_exit[c] && kick_pending && lead && lane == 0) tx_mbar_arrive(&kick_bar);
         if (s_exit[c]) {
             tx_mbar_arrive(&ready_bar[c][0]);   // releases the walkers (they expect stage 0), which read s_exit and drop this context
             return;
         }
         const int set = s_set[c];
         const int round = s_fresh[c] ? 0 : 1;   // 0: initial state from the inputs; otherwise from the parking area
-        const size_t traj_raw = (size_t)set * NL + tl;
+        const size_t traj_raw = (size_t)set * NL + lane;
         const bool valid = traj_raw < n;
         const size_t tr = valid ? traj_raw : (size_t)set * NL;   // an absent lane shadows the set's first trajectory, never committed
 
@@ -947,68 +841,68 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
         for (int hh = 0; hh < 2; ++hh) {
             const int cc = j + 3 * hh;
             const double yc = (round == 0) ? state[(size_t)cc * n + tr] : __ldcg(out_state + (size_t)cc * n + tr);
-            sm.ycur[cc * NL + tl] = yc;
+            sm.ycur[cc * NL + lane] = yc;
             if (round == 0 && valid && sink.cap > 0) sink.state[((size_t)cc * sink.cap) * n + tr] = yc;
         }
         if (lead) {
-            tx_load_ctl(S, sink, q, sm, tl, n, tr, valid, round, state, consts, epoch0, end_epoch, step_io, out_state, out_epoch);
-            tx_pick_step(sm, tl, end_epoch);
-            const bool done = sm.i32[TXW_FLAGS * NL + tl] & F_DONE;
+            tx_load_ctl(S, sink, q, sm, lane, n, tr, valid, round, state, consts, epoch0, end_epoch, step_io, out_state, out_epoch);
+            tx_pick_step(sm, lane, end_epoch);
+            const bool done = sm.i32[TXW_FLAGS * NL + lane] & F_DONE;
             const bool all = __all_sync(FULL, done);
-            if (lane == 0) { s_done_half[c][half] = all; if (half == 0) s_slice_end[c] = 0; }
-            if (gv.rot.kind != 0) tx_rot_store(sm.rot, tl, tx_rot_base(gv.rot, sm.i64[TXI_EPOCH * NL + tl]));
+            if (lane == 0) { s_done[c] = all; s_slice_end[c] = 0; }
+            if (gv.rot.kind != 0) tx_rot_store(sm.rot, lane, tx_rot_base(gv.rot, sm.i64[TXI_EPOCH * NL + lane]));
         }
         nb_sync(BAR_HB, NT_HB);
 
         // ---------------------------------------------------------------- step attempts of this slice
-        for (int it = 0; !set_done(); ++it) {
+        for (int it = 0; !s_done[c]; ++it) {
             TX_TRACE(TR_TOP, c, 0);
-            const double h = sm.f64[TXF_H * NL + tl];
-            const long long epoch = sm.i64[TXI_EPOCH * NL + tl];
-            const double r_own = sm.ycur[j * NL + tl], v_own = sm.ycur[(3 + j) * NL + tl];
+            const double h = sm.f64[TXF_H * NL + lane];
+            const long long epoch = sm.i64[TXI_EPOCH * NL + lane];
+            const double r_own = sm.ycur[j * NL + lane], v_own = sm.ycur[(3 + j) * NL + lane];
             // orientation angles at the step epoch (the lead evaluates every DCM of the attempt).  They are NOT evaluated here, on the
             // serial path between two attempts: helper 1 evaluates them for the epoch this attempt leads to while the walkers are
             // busy, and commits them to sm.rot when the controller accepts the step (a rejected step keeps its epoch).
             TxRotBase rb_;
             rb_.sa = 0.0; rb_.ca = 1.0; rb_.sd = 1.0; rb_.cd = 0.0; rb_.sw = 0.0; rb_.cw = 1.0;
             TxRotBase rb_next = rb_;
-            const bool fixed = sm.i32[TXW_FLAGS * NL + tl] & F_FIXED;
+            const bool fixed = sm.i32[TXW_FLAGS * NL + lane] & F_FIXED;
             // candidate state and error estimate (instance.rs:402-414), accumulated stage by stage in the reference's order
             double nx_r = r_own, nx_v = v_own, er_r = 0.0, er_v = 0.0;
             int rc_acc = 0;
             double Rn[9];
             // ---- prime the pipeline: stage 0 (the state itself) and stage 1 (needs only V_0 = v): instance.rs:369-394
-            sm.kst[(0 * 6 + j) * NL + tl] = v_own;                 // k_0[j] = V_0
-            sm.ysp[(0 * 3 + j) * NL + tl] = r_own;                 // P_0
+            sm.kst[(0 * 6 + j) * NL + lane] = v_own;                 // k_0[j] = V_0
+            sm.ysp[(0 * 3 + j) * NL + lane] = r_own;                 // P_0
             const long long off1 = (stages > 1) ? dur_from_seconds(S.tb.c[0] * h) : 0;
-            if (stages > 1) sm.ysp[(1 * 3 + j) * NL + tl] = fma(h, ta[0] * v_own, r_own);   // P_1 = r + h a_10 V_0
+            if (stages > 1) sm.ysp[(1 * 3 + j) * NL + lane] = fma(h, ta[0] * v_own, r_own);   // P_1 = r + h a_10 V_0
             nb_sync(BAR_HB, NT_HB);
             TX_TRACE(TR_PRIMED, c, 0);
             if (lead) {
                 if (gv.rot.kind != 0) {
-                    rb_.sa = sm.rot[tl]; rb_.ca = sm.rot[NL + tl]; rb_.sd = sm.rot[2 * NL + tl]; rb_.cd = sm.rot[3 * NL + tl];
-                    rb_.sw = sm.rot[4 * NL + tl]; rb_.cw = sm.rot[5 * NL + tl];
+                    rb_.sa = sm.rot[lane]; rb_.ca = sm.rot[NL + lane]; rb_.sd = sm.rot[2 * NL + lane]; rb_.cd = sm.rot[3 * NL + lane];
+                    rb_.sw = sm.rot[4 * NL + lane]; rb_.cw = sm.rot[5 * NL + lane];
                 }
                 tx_dcm(gv.rot, rb_, 0, Rn);
 #pragma unroll
-                for (int k = 0; k < 9; ++k) sm.rn[k * NL + tl] = Rn[k];
+                for (int k = 0; k < 9; ++k) sm.rn[k * NL + lane] = Rn[k];
             } else if (j == 1 && stages > 1) {   // the DCM of stage 1 in parallel with the lead's (both sat on the serial path between attempts)
                 TxRotBase rb1 = rb_;
                 if (gv.rot.kind != 0) {
-                    rb1.sa = sm.rot[tl]; rb1.ca = sm.rot[NL + tl]; rb1.sd = sm.rot[2 * NL + tl]; rb1.cd = sm.rot[3 * NL + tl];
-                    rb1.sw = sm.rot[4 * NL + tl]; rb1.cw = sm.rot[5 * NL + tl];
+                    rb1.sa = sm.rot[lane]; rb1.ca = sm.rot[NL + lane]; rb1.sd = sm.rot[2 * NL + lane]; rb1.cd = sm.rot[3 * NL + lane];
+                    rb1.sw = sm.rot[4 * NL + lane]; rb1.cw = sm.rot[5 * NL + lane];
                 }
                 tx_dcm(gv.rot, rb1, off1, Rn);
 #pragma unroll
-                for (int k = 0; k < 9; ++k) sm.rn[(9 + k) * NL + tl] = Rn[k];
+                for (int k = 0; k < 9; ++k) sm.rn[(9 + k) * NL + lane] = Rn[k];
             }
             nb_sync(BAR_HB, NT_HB);
             TX_TRACE(TR_DCM01, c, 0);
-            tx_prologue<P>(S, sm, tl, 0, j, sm.ysp, epoch);
+            tx_prologue<P>(S, sm, lane, 0, j, sm.ysp, epoch);
             tx_mbar_arrive(&ready_bar[c][0]);
             TX_TRACE(TR_READY, c, 0);
             if (stages > 1) {
-                tx_prologue<P>(S, sm, tl, 1, j, sm.ysp + 3 * NL, epoch + off1);
+                tx_prologue<P>(S, sm, lane, 1, j, sm.ysp + 3 * NL, epoch + off1);
                 tx_mbar_arrive(&ready_bar[c][1]);
                 TX_TRACE(TR_READY, c, 1);
             }
@@ -1020,15 +914,15 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
                 double preV = 0.0, preP = 0.0;
                 long long off2 = 0;
                 {
-                    const double vi = sm.kst[(i * 6 + j) * NL + tl];   // V_i
+                    const double vi = sm.kst[(i * 6 + j) * NL + lane];   // V_i
                     if (!fixed) er_r = fma(h * S.tb.e[i], vi, er_r);
                     nx_r = fma(h * S.tb.b[i], vi, nx_r);
                 }
                 if (j == 1 && i == 0 && gv.rot.kind != 0)
-                    rb_next = tx_rot_base(gv.rot, epoch + (fixed ? sm.i64[TXI_STEP * NL + tl] : dur_from_seconds(h)));
+                    rb_next = tx_rot_base(gv.rot, epoch + (fixed ? sm.i64[TXI_STEP * NL + lane] : dur_from_seconds(h)));
                 if (i + 1 < stages) {   // V_{i+1} = v + h sum_{l<=i} a_{i+1,l} A_l: all terms but the last
                     const double* arow = ta + i * NYXB_MAX_STAGES;
-                    const double* kc = sm.kst + (3 + j) * NL + tl;
+                    const double* kc = sm.kst + (3 + j) * NL + lane;
                     double w0 = 0.0, w1 = 0.0;
                     int l = 0;
                     for (; l + 1 < i; l += 2) { w0 = fma(arow[l], kc[l * 6 * NL], w0); w1 = fma(arow[l + 1], kc[(l + 1) * 6 * NL], w1); }
@@ -1037,7 +931,7 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
                 }
                 if (i + 2 < stages) {   // P_{i+2} = r + h sum_{m<=i+1} a_{i+2,m} V_m: all terms but the last (V_i is known)
                     const double* arow = ta + (i + 1) * NYXB_MAX_STAGES;
-                    const double* kc = sm.kst + j * NL + tl;
+                    const double* kc = sm.kst + j * NL + lane;
                     double w0 = 0.0, w1 = 0.0;
                     int m = 0;
                     for (; m + 1 <= i; m += 2) { w0 = fma(arow[m], kc[m * 6 * NL], w0); w1 = fma(arow[m + 1], kc[(m + 1) * 6 * NL], w1); }
@@ -1048,12 +942,12 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
                     if (lead) {   // DCM of stage i+2 (its parity buffer was last read in the prologue of stage i, two barriers ago)
                         tx_dcm(gv.rot, rb_, off2, Rn);
 #pragma unroll
-                        for (int k = 0; k < 9; ++k) sm.rn[(par * 9 + k) * NL + tl] = Rn[k];
+                        for (int k = 0; k < 9; ++k) sm.rn[(par * 9 + k) * NL + lane] = Rn[k];
                     }
                 }
                 TX_TRACE(TR_DCM_DONE, c, i);
                 if (kick_pending && i == stages / 2) {
-                    if (lead0 && lane == 0) tx_mbar_arrive(&kick_bar);
+                    if (lead && lane == 0) tx_mbar_arrive(&kick_bar);
                     kick_pending = false;
                 }
                 TX_TRACE(TR_DONE_WAIT, c, i);
@@ -1066,14 +960,14 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
                     double ax[4] = {0.0, 0.0, 0.0, 0.0}, ay[4] = {0.0, 0.0, 0.0, 0.0}, az[4] = {0.0, 0.0, 0.0, 0.0}, aw4[4] = {0.0, 0.0, 0.0, 0.0};
 #pragma unroll
                     for (int p = 0; p < P; ++p) {
-                        const double* pt = sm.part + ((par * P + p) * 4) * NL + tl;
+                        const double* pt = sm.part + ((par * P + p) * 4) * NL + lane;
                         ax[p & 3] += pt[0]; ay[p & 3] += pt[NL]; az[p & 3] += pt[2 * NL]; aw4[p & 3] += pt[3 * NL];
                     }
                     X = (ax[0] + ax[1]) + (ax[2] + ax[3]); Y = (ay[0] + ay[1]) + (ay[2] + ay[3]);
                     Z = (az[0] + az[1]) + (az[2] + az[3]); Wt = (aw4[0] + aw4[1]) + (aw4[2] + aw4[3]);
                 }
                 TX_TRACE(TR_REDUCED, c, i);
-                const double* as = sm.as + par * AS_COUNT * NL + tl;
+                const double* as = sm.as + par * AS_COUNT * NL + lane;
                 const double K0 = as[AS_K0 * NL], K1 = as[AS_K1 * NL];
                 const double aw = -K0 * Wt;
                 const double ab0 = fma(aw, as[AS_S * NL], K1 * X), ab1 = fma(aw, as[AS_T * NL], K1 * Y), ab2 = fma(aw, as[AS_U * NL], K1 * Z);
@@ -1084,58 +978,58 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
                     const double hz = (i > 0) ? h * 0.0 : 0.0;
                     yy[0] = as[AS_P0 * NL]; yy[1] = as[AS_P1 * NL]; yy[2] = as[AS_P2 * NL];
 #pragma unroll
-                    for (int e = 0; e < 3; ++e) yy[3 + e] = sm.kst[(i * 6 + e) * NL + tl];   // V_i
-                    yy[6] = sm.f64[TXF_CR * NL + tl] + hz; yy[7] = sm.f64[TXF_CD * NL + tl] + hz; yy[8] = sm.f64[TXF_PM * NL + tl] + hz;
+                    for (int e = 0; e < 3; ++e) yy[3 + e] = sm.kst[(i * 6 + e) * NL + lane];   // V_i
+                    yy[6] = sm.f64[TXF_CR * NL + lane] + hz; yy[7] = sm.f64[TXF_CD * NL + lane] + hz; yy[8] = sm.f64[TXF_PM * NL + lane] + hz;
                     const long long offi = (i > 0) ? dur_from_seconds(S.tb.c[i - 1] * h) : 0;
-                    const int rcx = tx_extra(S, sm.f64[TXF_DRY * NL + tl], sm.f64[TXF_EXTRA * NL + tl], sm.f64[TXF_SRPA * NL + tl],
-                                             sm.f64[TXF_DRAGA * NL + tl], epoch + offi, yy, aa);
+                    const int rcx = accel_cold<true>(S, sm.f64[TXF_DRY * NL + lane], sm.f64[TXF_EXTRA * NL + lane], sm.f64[TXF_SRPA * NL + lane],
+                                                     sm.f64[TXF_DRAGA * NL + lane], epoch + offi, yy, aa);
                     acc += (j == 0) ? aa[0] : (j == 1 ? aa[1] : aa[2]);
                     if (rcx && !rc_acc) rc_acc = rcx | ((i + 1) << 8);
                 }
-                sm.kst[(i * 6 + 3 + j) * NL + tl] = acc;     // k_i[3+j] = A_i
+                sm.kst[(i * 6 + 3 + j) * NL + lane] = acc;     // k_i[3+j] = A_i
                 if (!fixed) er_v = fma(h * S.tb.e[i], acc, er_v);
                 nx_v = fma(h * S.tb.b[i], acc, nx_v);
                 if (i + 1 < stages) {
                     const double vn = fma(h, fma(ta[i * NYXB_MAX_STAGES + i], acc, preV), v_own);   // V_{i+1}
-                    sm.kst[((i + 1) * 6 + j) * NL + tl] = vn;                                    // k_{i+1}[j]
+                    sm.kst[((i + 1) * 6 + j) * NL + lane] = vn;                                    // k_{i+1}[j]
                     if (i + 2 < stages)
-                        sm.ysp[(par * 3 + j) * NL + tl] = fma(h, fma(ta[(i + 1) * NYXB_MAX_STAGES + i + 1], vn, preP), r_own);   // P_{i+2}
+                        sm.ysp[(par * 3 + j) * NL + lane] = fma(h, fma(ta[(i + 1) * NYXB_MAX_STAGES + i + 1], vn, preP), r_own);   // P_{i+2}
                     TX_TRACE(TR_ACC_DONE, c, i);
                     nb_sync(BAR_HB, NT_HB);   // V_{i+1} and the position components of stage i+2 of all three helpers are in shared memory
                     TX_TRACE(TR_HB_PASSED, c, i);
                     if (i + 2 < stages) {
-                        tx_prologue<P>(S, sm, tl, par, j, sm.ysp + par * 3 * NL, epoch + off2);
+                        tx_prologue<P>(S, sm, lane, par, j, sm.ysp + par * 3 * NL, epoch + off2);
                         tx_mbar_arrive(&ready_bar[c][par]);   // walker inputs of stage i+2 are published
                         TX_TRACE(TR_READY, c, i + 2);
                     }
                 }
             }
             TX_TRACE(TR_STAGES_END, c, 0);
-            sm.nxt[j * NL + tl] = nx_r; sm.nxt[(3 + j) * NL + tl] = nx_v;
-            sm.er[j * NL + tl] = er_r; sm.er[(3 + j) * NL + tl] = er_v;
-            if (lead) sm.i32[TXW_RCST * NL + tl] = rc_acc;
+            sm.nxt[j * NL + lane] = nx_r; sm.nxt[(3 + j) * NL + lane] = nx_v;
+            sm.er[j * NL + lane] = er_r; sm.er[(3 + j) * NL + lane] = er_v;
+            if (lead) sm.i32[TXW_RCST * NL + lane] = rc_acc;
             nb_sync(BAR_HB, NT_HB);
             TX_TRACE(TR_CTRL_IN, c, 0);
             if (lead) {
-                tx_controller(S, sink, sm, tl, n, tr, stages);
+                tx_controller(S, sink, sm, lane, n, tr, stages);
                 TX_TRACE(TR_CTRL_OUT, c, 0);
                 const bool slice_end = q.slice > 0 && it + 1 >= q.slice;
-                if (!slice_end) tx_pick_step(sm, tl, end_epoch);
+                if (!slice_end) tx_pick_step(sm, lane, end_epoch);
                 TX_TRACE(TR_PICKED, c, 0);
-                const bool done = sm.i32[TXW_FLAGS * NL + tl] & F_DONE;
+                const bool done = sm.i32[TXW_FLAGS * NL + lane] & F_DONE;
                 const bool all = __all_sync(FULL, done);
-                if (lane == 0) { s_done_half[c][half] = all; if (half == 0) s_slice_end[c] = slice_end; }
+                if (lane == 0) { s_done[c] = all; s_slice_end[c] = slice_end; }
             }
             nb_sync(BAR_HB, NT_HB);
             TX_TRACE(TR_CTRL_END, c, 0);
-            if (sm.i32[TXW_ACC * NL + tl]) {
-                if (j == 1 && gv.rot.kind != 0) tx_rot_store(sm.rot, tl, rb_next);   // read by the lead after the next HB barrier
-                const long long ns = sm.i64[TXI_NSTEPS * NL + tl];
+            if (sm.i32[TXW_ACC * NL + lane]) {
+                if (j == 1 && gv.rot.kind != 0) tx_rot_store(sm.rot, lane, rb_next);   // read by the lead after the next HB barrier
+                const long long ns = sm.i64[TXI_NSTEPS * NL + lane];
 #pragma unroll
                 for (int hh = 0; hh < 2; ++hh) {
                     const int cc = j + 3 * hh;
-                    const double nx = sm.nxt[cc * NL + tl];
-                    sm.ycur[cc * NL + tl] = nx;
+                    const double nx = sm.nxt[cc * NL + lane];
+                    sm.ycur[cc * NL + lane] = nx;
                     // the channel send of instance.rs:186-193 / 255-259: lanes are consecutive trajectories, one 256-byte store per warp
                     if (valid && ns < sink.cap) sink.state[((size_t)cc * sink.cap + (size_t)ns) * n + tr] = nx;
                 }
@@ -1145,18 +1039,18 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
         }
 
         if (kick_pending) {
-            if (lead0 && lane == 0) tx_mbar_arrive(&kick_bar);
+            if (lead && lane == 0) tx_mbar_arrive(&kick_bar);
             kick_pending = false;
         }
         // ---------------------------------------------------------------- park the set (== final outputs when it is done)
         if (valid) {
-            out_state[(size_t)j * n + tr] = sm.ycur[j * NL + tl];
-            out_state[(size_t)(j + 3) * n + tr] = sm.ycur[(j + 3) * NL + tl];
+            out_state[(size_t)j * n + tr] = sm.ycur[j * NL + lane];
+            out_state[(size_t)(j + 3) * n + tr] = sm.ycur[(j + 3) * NL + lane];
         }
-        if (lead) tx_park_ctl(sink, q, sm, tl, n, tr, step_io, out_state, out_epoch, out_status);
+        if (lead) tx_park_ctl(sink, q, sm, lane, n, tr, step_io, out_state, out_epoch, out_status);
         __threadfence();
         nb_sync(BAR_HB, NT_HB);
-        if (lead0 && lane == 0 && !set_done()) {   // park: the set becomes resumable by any context
+        if (lead && lane == 0 && !s_done[c]) {   // park: the set becomes resumable by any context
             while (atomicCAS(q.ctl + TXQ_LOCK, 0, 1) != 0) __nanosleep(64);
             __threadfence();
             volatile int* vc = q.ctl;
@@ -1199,7 +1093,6 @@ TxBlob tx_blob(int N, int P, int n_rec, int kmax) {
 // ------------------------------------------------------------------------------------------------
 // host: zigzag column -> position schedule and record table
 // ------------------------------------------------------------------------------------------------
-#if NYXB_TX_TT == 1
 void nyxb_tx_build_host(int N, int M, const double* c_nm, const double* s_nm, int P, TxHost& out) {
     const double sqrt2 = std::sqrt(2.0);
     auto C = [&](int n, int m) { return (n <= N && m <= M && m <= n) ? c_nm[(size_t)n * (N + 1) + m] : 0.0; };
@@ -1282,12 +1175,10 @@ void nyxb_tx_build_host(int N, int M, const double* c_nm, const double* s_nm, in
     }
 }
 
-#endif   // NYXB_TX_TT == 1 (host-only table builder)
-
 // set contexts per CTA: two sets in flight while both fit beside the table (P = 8: degrees up to ~40), one otherwise
 static int tx_contexts(const DevSetup* S, const DevTx* Tx, size_t* smem_bytes) {
     const TxBlob b = tx_blob(S->grav.N, Tx->P, Tx->n_rec, Tx->kmax);
-    for (int nctx = (TT == 1 && Tx->P <= 10 ? 2 : 1); nctx >= 1; --nctx) {
+    for (int nctx = (Tx->P <= 10 ? 2 : 1); nctx >= 1; --nctx) {
         const size_t smem = tx_layout(b.bytes, Tx->P, S->grav.N, nctx).total;
         if (smem <= 227 * 1024) { if (smem_bytes) *smem_bytes = smem; return nctx; }
     }
@@ -1295,20 +1186,13 @@ static int tx_contexts(const DevSetup* S, const DevTx* Tx, size_t* smem_bytes) {
 }
 
 // set contexts one SM holds for this setup (one persistent CTA per SM; 0: the tables do not fit) and its dynamic shared memory
-#if NYXB_TX_TT == 1
-#define NYXB_TX_OCCUPANCY nyxb_tx_occupancy
-#define NYXB_TX_LAUNCH nyxb_launch_tx
-#else   // sets of 64 trajectories (8 walker positions only)
-#define NYXB_TX_OCCUPANCY nyxb_tx2_occupancy
-#define NYXB_TX_LAUNCH nyxb_launch_tx2
-#endif
-extern "C" int NYXB_TX_OCCUPANCY(const DevSetup* S, const DevTx* Tx, size_t* smem_bytes) {
-    if (TT == 1 ? (Tx->P != 8 && Tx->P != 10 && Tx->P != 16) : Tx->P != 8) return 0;
+extern "C" int nyxb_tx_occupancy(const DevSetup* S, const DevTx* Tx, size_t* smem_bytes) {
+    if (Tx->P != 8 && Tx->P != 10 && Tx->P != 16) return 0;
     return tx_contexts(S, Tx, smem_bytes);
 }
 
 // `grid` CTAs, each with nyxb_tx_occupancy() set contexts
-extern "C" cudaError_t NYXB_TX_LAUNCH(const DevSetup* S, const DevTx* Tx, const DevTxQueue* q, size_t n, const double* state,
+extern "C" cudaError_t nyxb_launch_tx(const DevSetup* S, const DevTx* Tx, const DevTxQueue* q, size_t n, const double* state,
                                       const double* consts, const long long* epoch0, long long end_epoch, long long* step_io,
                                       double* out_state, long long* out_epoch, int* out_status, const DevSink* sink,
                                       int grid, cudaStream_t stream) {
@@ -1318,18 +1202,13 @@ extern "C" cudaError_t NYXB_TX_LAUNCH(const DevSetup* S, const DevTx* Tx, const 
     const int nctx = tx_contexts(S, Tx, &smem);
     if (nctx < 1 || grid < 1) return cudaErrorInvalidConfiguration;
 #define NYXB_TX_GO(PP, CC) tx_launch_p<PP, CC>(S, Tx, q, n, state, consts, epoch0, end_epoch, step_io, out_state, out_epoch, out_status, sink, grid, smem, b.bytes, b.off_recK, b.off_seed, b.off_sched, stream)
-#if NYXB_TX_TT == 1
     if (Tx->P == 8) return nctx == 2 ? NYXB_TX_GO(8, 2) : NYXB_TX_GO(8, 1);
     if (Tx->P == 10) return nctx == 2 ? NYXB_TX_GO(10, 2) : NYXB_TX_GO(10, 1);
     if (Tx->P == 16) return NYXB_TX_GO(16, 1);
-#else
-    if (Tx->P == 8) return NYXB_TX_GO(8, 1);
-#endif
     return cudaErrorInvalidValue;
 #undef NYXB_TX_GO
 }
 
-#if NYXB_TX_TT == 1
 // host-side view of the blob (nyxb_api.cu uploads it as one allocation; the kernel copies it with one TMA bulk copy)
 size_t nyxb_tx_pack_blob(const TxHost* h, int N, unsigned char* dst) {
     const TxBlob b = tx_blob(N, h->P, h->n_rec, h->kmax);
@@ -1342,4 +1221,3 @@ size_t nyxb_tx_pack_blob(const TxHost* h, int N, unsigned char* dst) {
     }
     return b.bytes;
 }
-#endif   // NYXB_TX_TT == 1
