@@ -1,0 +1,430 @@
+// nyxb_od_arc.cuh — the PropInstance over state + STM and the filter loop (KalmanODProcess::process_arc), written once for the
+// per-thread (nyxb_od.cu) and the warp-cooperative (nyxb_od_coop.cu) kernels.
+//
+// Both kernels instantiate these templates with a backend B, a plain struct that says who computes what and where the arrays live:
+//   B::stride, first()   an 81-entry loop runs over entries first(), first() + stride, ...: 0 and 1 for one thread per filter, the lane
+//                        and 32 for one warp per filter;
+//   sync()               makes the entries written by every lane visible to all of them (nothing, or __syncwarp());
+//   lead()               the lane that writes the scalar records;
+//   any(v)               v on any lane (the NaN check of the candidate);
+//   S                    the DevSetup;
+//   phi                  the STM, column-major like the ABI;
+//   B::Step(b)           one propagation's scratch: candidate STM nphi, stage derivatives k[i][6], stage A-matrix parts Ai[i][12];
+//   B::Filt(b)           one filter's storage: covariance P and state deviation xdev, and the update scratch Pb, T, F (9x9,
+//                        row-major), PHt and K (9x2);
+//   rhs(in, dt, ys, st, i) one right-hand side at in.epoch + dt into stage slot i: st.k[i] = (v, a), st.Ai[i][0..8] = d(a)/d(r)
+//                        row-major, st.Ai[i][9..11] = d(a)/d(Cr).
+// The scratch types let the per-thread backend keep its temporaries in scoped locals; the warp backend points them into its slab.
+// Every scalar below (OdInst, h, the window, the gain inputs) is computed by every lane alike, so all lanes take the same branches.
+#pragma once
+#include "nyxb_od_device.cuh"
+
+// PropInstance scalars of one trajectory or filter (instance.rs:87-262)
+struct OdInst {
+    double y[9];
+    long long epoch_ns, step_ns;
+    int fixed, status;
+    long long det_step_ns;
+    double det_error;
+    int det_attempts;
+    long long n_steps, n_rejected, n_rhs;
+    double dry_mass, extra_mass, srp_area;
+};
+
+__device__ __forceinline__ void od_load(const DevSetup& S, OdInst& in, size_t i, size_t n, const double* state, const double* consts,
+                                        const long long* epoch0, const long long* step_io) {
+#pragma unroll
+    for (int e = 0; e < 9; ++e) in.y[e] = state[(size_t)e * n + i];
+    in.dry_mass = consts[i]; in.extra_mass = consts[n + i]; in.srp_area = consts[2 * n + i];
+    in.epoch_ns = epoch0[i];
+    in.step_ns = step_io ? step_io[i] : S.init_step_ns;
+    in.fixed = S.fixed_step;
+    in.status = 0;
+    in.det_step_ns = S.init_step_ns; in.det_error = 0.0; in.det_attempts = 1;
+    in.n_steps = 0; in.n_rejected = 0; in.n_rhs = 0;
+}
+
+template <class B>
+__device__ __forceinline__ void od_store(const B& b, const OdInst& in, int rc, size_t i, size_t n, double* out_state, long long* out_epoch,
+                                         nyxb_details* out_details, int* out_status) {
+    for (int r = b.first(); r < 9; r += B::stride) out_state[(size_t)r * n + i] = in.y[r];
+    if (!b.lead()) return;
+    out_epoch[i] = in.epoch_ns;
+    if (out_details) {
+        nyxb_details d;
+        d.step_ns = in.det_step_ns; d.error = in.det_error; d.attempts = in.det_attempts; d._pad = 0;
+        d.n_steps = in.n_steps; d.n_rejected = in.n_rejected; d.n_rhs = in.n_rhs;
+        out_details[i] = d;
+    }
+    out_status[i] = (in.status & NYXB_WARN_MAX_ATTEMPTS) | rc;
+}
+
+template <class B>
+__device__ __forceinline__ void od_reset_stm(B& b) {
+    for (int e = b.first(); e < 81; e += B::stride) b.phi[e] = ((e / 9) == (e % 9)) ? 1.0 : 0.0;
+    b.sync();
+}
+
+// ------------------------------------------------------------------------- PropInstance over state + STM
+// instance.rs:358-493 on the 90-vector; stage STM derivative = ctx.stm * A_i (spacecraft.rs:213) with ctx = step start.  The candidate
+// STM goes to st.nphi.  Components 6-8 get h * 0 added (instance.rs:394): NaN-propagating, and -0 becomes +0.
+template <class B>
+__device__ __forceinline__ int od_derive(B& b, typename B::Step& st, OdInst& in, long long& dt_ns, double next[9]) {
+    const DevSetup& S = b.S;
+    const int stages = S.tb.stages;
+    in.det_attempts = 1;
+    double h = dur_to_seconds(in.step_ns);
+    for (;;) {
+        int rc = b.rhs(in, 0.0, in.y, st, 0);
+        if (rc) return rc;
+        for (int i = 0; i < stages - 1; ++i) {
+            double wi[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+            const double* arow = &S.tb.a[i * NYXB_MAX_STAGES];
+            for (int j = 0; j <= i; ++j) {
+                double a_ij = arow[j];
+#if !NYXB_STRICT
+                if (a_ij == 0.0) continue;
+#endif
+#pragma unroll
+                for (int e = 0; e < 6; ++e) wi[e] += a_ij * st.k[j][e];
+            }
+            double ys[9];
+#pragma unroll
+            for (int e = 0; e < 6; ++e) ys[e] = in.y[e] + h * wi[e];
+            const double hz = h * 0.0;
+            ys[6] = in.y[6] + hz; ys[7] = in.y[7] + hz; ys[8] = in.y[8] + hz;
+            rc = b.rhs(in, S.tb.c[i] * h, ys, st, i + 1);
+            if (rc) return rc;
+        }
+        double err_est[9] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+#pragma unroll
+        for (int e = 0; e < 9; ++e) next[e] = in.y[e];
+        { const double hz = h * 0.0; next[6] += hz; next[7] += hz; next[8] += hz; }
+        for (int i = 0; i < stages; ++i) {
+            if (!in.fixed) {
+                double cf = h * S.tb.e[i];
+#pragma unroll
+                for (int e = 0; e < 6; ++e) err_est[e] += cf * st.k[i][e];
+            }
+            double cb = h * S.tb.b[i];
+#pragma unroll
+            for (int e = 0; e < 6; ++e) next[e] += cb * st.k[i][e];
+        }
+        // candidate STM: entry (r, c) = phi(r, c) + sum_i (h b_i) (phi A_i)(r, c), where (phi A_i)(r, c) is
+        // c < 3: sum_q phi(r, 3+q) G(q, c); 3 <= c < 6: phi(r, c-3); c == 6: sum_q phi(r, 3+q) gcr(q); c > 6: 0
+        bool bad = false;
+        for (int e = b.first(); e < 81; e += B::stride) {
+            const int c = e / 9, r = e - 9 * c;
+            double v = b.phi[e];
+            if (c < 7) {
+                const double p3 = b.phi[27 + r], p4 = b.phi[36 + r], p5 = b.phi[45 + r], pc = (c >= 3 && c < 6) ? b.phi[(c - 3) * 9 + r] : 0.0;
+                for (int i = 0; i < stages; ++i) {
+                    const double cb = h * S.tb.b[i];
+                    const double* Gi = st.Ai[i];
+                    double d;
+                    if (c < 3) d = (p3 * Gi[c] + p4 * Gi[3 + c]) + p5 * Gi[6 + c];
+                    else if (c < 6) d = pc;
+                    else d = (p3 * Gi[9] + p4 * Gi[10]) + p5 * Gi[11];
+                    v += cb * d;
+                }
+            }
+            st.nphi[e] = v;
+            bad = bad || (v != v);
+        }
+        b.sync();
+        if (in.fixed) {
+            in.det_step_ns = in.step_ns;
+            dt_ns = in.step_ns;
+            return 0;
+        }
+        in.det_error = error_estimate(S.error_ctrl, err_est, next, in.y);
+        if (ctl_accept(S, in.det_error, h, in.det_attempts)) {
+            for (int e = 0; e < 9; ++e) bad = bad || (next[e] != next[e]);
+            if (b.any(bad)) return NYXB_ERR_PROP_MATH;
+            in.step_ns = ctl_accepted<pow_inv_int>(S, in.det_error, h, in.det_attempts, in.status, in.det_step_ns);
+            dt_ns = in.det_step_ns;
+            return 0;
+        }
+        in.det_attempts += 1;
+        in.n_rejected += 1;
+        h = ctl_retry<pow_inv_int>(S, in.det_error, h);
+    }
+}
+
+template <class B>
+__device__ __forceinline__ int od_single_step(B& b, typename B::Step& st, OdInst& in) {
+    long long dt;
+    double next[9];
+    int rc = od_derive(b, st, in, dt, next);
+    if (rc) return rc;
+    in.epoch_ns += dt;
+#pragma unroll
+    for (int e = 0; e < 9; ++e) in.y[e] = next[e];
+    for (int e = b.first(); e < 81; e += B::stride) b.phi[e] = st.nphi[e];
+    b.sync();
+    in.y[6] = in.y[6] < 0.0 ? 0.0 : (in.y[6] > 2.0 ? 2.0 : in.y[6]);
+    in.n_steps += 1;
+    return (in.y[8] < 0.0) ? NYXB_ERR_FUEL_EXHAUSTED : 0;
+}
+
+template <class B>
+__device__ int od_propagate(B& b, OdInst& in, long long duration_ns) {
+    if (duration_ns == 0) return 0;
+    long long stop = in.epoch_ns + duration_ns;
+    if (in.y[8] < 0.0) return NYXB_ERR_FUEL_EXHAUSTED;
+    bool backprop = duration_ns < 0;
+    if (backprop) in.step_ns = -in.step_ns;
+    typename B::Step st(b);
+    for (;;) {
+        long long epoch = in.epoch_ns;
+        if (ctl_past_stop(epoch, in.step_ns, stop, backprop)) {
+            if (stop == epoch) return 0;
+            long long prev_step = in.step_ns;
+            int prev_fixed = in.fixed;
+            in.step_ns = stop - epoch;
+            in.fixed = 1;
+            int rc = od_single_step(b, st, in);
+            if (rc) return rc;
+            in.step_ns = prev_step;
+            in.fixed = prev_fixed;
+            if (backprop) in.step_ns = -in.step_ns;
+            return 0;
+        }
+        int rc = od_single_step(b, st, in);
+        if (rc) return rc;
+    }
+}
+
+// ------------------------------------------------------------------------- time update, measurement update (filtering.rs:59-316)
+// f.Pb = Phi P Phi^T (+ SNC: ProcessNoise::propagate, snc.rs:211-286); filtering.rs:61-78 / 132-150
+template <class B>
+__device__ __forceinline__ void od_covar_bar(const DevOd& od, const OdInst& in, long long prev_epoch, B& b, typename B::Filt& f) {
+    for (int e = b.first(); e < 81; e += B::stride) {   // T = Phi P
+        const int r = e / 9, c = e - 9 * r;
+        double s = 0.0;
+#pragma unroll
+        for (int k = 0; k < 9; ++k) s += b.phi[k * 9 + r] * f.P[k * 9 + c];
+        f.T[e] = s;
+    }
+    b.sync();
+    for (int e = b.first(); e < 81; e += B::stride) {   // Pb = T Phi^T
+        const int r = e / 9, c = e - 9 * r;
+        double s = 0.0;
+#pragma unroll
+        for (int k = 0; k < 9; ++k) s += f.T[r * 9 + k] * b.phi[k * 9 + c];
+        f.Pb[e] = s;
+    }
+    b.sync();
+    if (!od.snc_enabled) return;
+    const long long delta = in.epoch_ns - prev_epoch;
+    if (delta > od.snc_disable_ns) return;
+    double s[3] = { od.snc_diag[0], od.snc_diag[1], od.snc_diag[2] };
+    if (od.snc_frame == 1) {  // RIC: rotate, keep the diagonal (snc.rs:226-247)
+        const double* y = in.y;
+        double rn = norm3(y[0], y[1], y[2]);
+        double rh[3] = { y[0] / rn, y[1] / rn, y[2] / rn };
+        double hx = y[1] * y[5] - y[2] * y[4], hy = y[2] * y[3] - y[0] * y[5], hz = y[0] * y[4] - y[1] * y[3];
+        double hn = norm3(hx, hy, hz);
+        double ch[3] = { hx / hn, hy / hn, hz / hn };
+        double ih[3] = { ch[1] * rh[2] - ch[2] * rh[1], ch[2] * rh[0] - ch[0] * rh[2], ch[0] * rh[1] - ch[1] * rh[0] };
+        double d[3];
+#pragma unroll
+        for (int i = 0; i < 3; ++i) d[i] = ((rh[i] * s[0]) * rh[i] + (ih[i] * s[1]) * ih[i]) + (ch[i] * s[2]) * ch[i];
+        s[0] = d[0]; s[1] = d[1]; s[2] = d[2];
+    }
+    double dt = dur_to_seconds(delta);
+    double g1 = (dt * dt) / 2.0, g2 = dt;
+    for (int i = b.first(); i < 3; i += B::stride) {
+        f.Pb[i * 9 + i] += (g1 * s[i]) * g1;
+        f.Pb[i * 9 + 3 + i] += (g1 * s[i]) * g2;
+        f.Pb[(3 + i) * 9 + i] += (g2 * s[i]) * g1;
+        f.Pb[(3 + i) * 9 + 3 + i] += (g2 * s[i]) * g2;
+    }
+    b.sync();
+}
+
+// KalmanFilter::time_update, filtering.rs:59-102
+template <class B>
+__device__ __forceinline__ void od_time_update(const DevOd& od, const OdInst& in, long long& prev_epoch, B& b, typename B::Filt& f) {
+    od_covar_bar(od, in, prev_epoch, b, f);
+    const bool tracking = od.variant == NYXB_KF_DEVIATION_TRACKING;
+    for (int r = b.first(); r < 9; r += B::stride) {   // new deviation into T, free once Pb is formed
+        double s = 0.0;
+        if (tracking)
+            for (int k = 0; k < 9; ++k) s += b.phi[k * 9 + r] * f.xdev[k];
+        f.T[r] = s;
+    }
+    b.sync();
+    for (int r = b.first(); r < 9; r += B::stride) f.xdev[r] = f.T[r];
+    for (int e = b.first(); e < 81; e += B::stride) f.P[e] = f.Pb[e];
+    b.sync();
+    prev_epoch = in.epoch_ns;
+}
+
+// ------------------------------------------------------------------------- KalmanODProcess::process_arc (od/process/mod.rs:128-497)
+// Loads filter i, runs the whole arc and stores the final covariance, deviation, state, details and status.
+template <class B>
+__device__ void od_process_arc(const DevOd& od, B& b, size_t i, size_t n, const double* state, const double* consts, const long long* epoch0,
+                               double* out_state, long long* out_epoch, nyxb_details* out_details, int* out_status) {
+    const DevSetup& S = b.S;
+    OdInst in;
+    od_load(S, in, i, n, state, consts, epoch0, nullptr);
+    if (!in.fixed) in.step_ns = od.max_step_ns;              // :170-172
+    typename B::Filt f(b);
+    for (int e = b.first(); e < 81; e += B::stride) {
+        const int r = e / 9, c = e - 9 * r;
+        f.P[e] = od.covar0[(size_t)(c * 9 + r) * n + i];
+    }
+    for (int r = b.first(); r < 9; r += B::stride) f.xdev[r] = 0.0;
+    od_reset_stm(b);                                         // prop.with(nominal.with_stm()) :167
+    long long prev_epoch = in.epoch_ns;
+    long long epoch = in.epoch_ns;
+    int rc = 0;
+    const bool ekf = od.variant == NYXB_KF_REFERENCE_UPDATE;
+    const int M = od.msr_size;
+    for (long long k = 0; k < od.n_msr && rc == 0; ++k) {
+        const long long t_k = od.msr_epoch[k];
+        const double o[2] = { od.obs[((size_t)k * 2 + 0) * n + i], od.obs[((size_t)k * 2 + 1) * n + i] };
+        int flags = 0;
+        if (o[0] != o[0] && o[1] != o[1]) {
+            if (od.flags && b.lead()) od.flags[(size_t)k * n + i] = NYXB_MSRF_ABSENT;
+            continue;
+        }
+        for (;;) {
+            long long delta_t = t_k - epoch;
+            long long next_step = delta_t;                                      // :218
+            if (in.step_ns < next_step) next_step = in.step_ns;
+            if (od.max_step_ns < next_step) next_step = od.max_step_ns;
+            rc = od_propagate(b, in, next_step);                                // :232-234
+            if (rc) break;
+            epoch = in.epoch_ns;
+            long long gap = in.epoch_ns - t_k;
+            if (gap < 0) gap = -gap;
+            if (!(gap < od.eps_ns)) {                                           // :250
+                od_time_update(od, in, prev_epoch, b, f);                       // :417-421
+                od_reset_stm(b);
+                continue;
+            }
+            in.epoch_ns = t_k;                                                  // :254
+            const int trk = od.msr_tracker[k];
+            if (trk < 0 || trk >= od.n_stations) break;                         // unknown tracker :400-410
+            const DevStation& gs = od.stations[trk];
+            const int windows = gs.n_types / M;
+            for (int wno = 0; wno <= windows; ++wno) {                          // :270-398
+                OdWindow w;
+                const int wrc = od_window_setup(S, gs, M, wno, o, t_k, in.y, w);
+                if (wrc == OD_WIN_EMPTY) break;
+                if (wrc == OD_WIN_UNAVAILABLE) continue;
+                if (wrc == OD_WIN_EPHEMERIS) { rc = NYXB_ERR_EPHEMERIS; break; }
+                if (wrc == OD_WIN_NOT_VISIBLE) { flags |= NYXB_MSRF_NOT_VISIBLE; continue; }
+                const double (&H)[2][9] = w.H;
+                const double* Rk = w.Rk;
+                // ---- measurement_update (filtering.rs:107-316)
+                od_covar_bar(od, in, prev_epoch, b, f);
+                for (int e = b.first(); e < 18; e += B::stride) {               // PHt[r][q], r = e / 2, q = e % 2
+                    const int r = e >> 1, q = e & 1;
+                    double s = 0.0;
+                    if (q < M)
+                        for (int c = 0; c < 9; ++c) s += f.Pb[r * 9 + c] * H[q][c];
+                    f.PHt[e] = s;
+                }
+                b.sync();
+                double Sk[2][2] = { {0.0, 0.0}, {0.0, 0.0} }, pre[2] = { 0.0, 0.0 };
+                for (int a = 0; a < M; ++a)
+                    for (int bb = 0; bb < M; ++bb) {
+                        double s = 0.0;
+                        for (int c = 0; c < 9; ++c) s += H[a][c] * f.PHt[c * 2 + bb];
+                        Sk[a][bb] = s + ((a == bb) ? Rk[a] : 0.0);
+                    }
+                for (int q = 0; q < M; ++q) pre[q] = w.real_obs[q] - w.comp[q];
+                double ratio;
+                if (!od_ratio(M, Sk, Rk, pre, ratio)) { rc = NYXB_ERR_PROP_MATH; break; }   // SingularNoiseRk
+                const int rslot = (M == 1) ? wno : 0;
+                if (b.lead()) {
+                    if (od.ratio) od.ratio[((size_t)k * 2 + rslot) * n + i] = ratio;
+                    if (od.prefit) for (int q = 0; q < w.ncur; ++q) od.prefit[((size_t)k * 2 + wno * M + q) * n + i] = pre[q];
+                }
+                flags |= NYXB_MSRF_PROCESSED;
+                if (od.reject >= 0.0 && ratio > od.reject) {                    // :169-184
+                    od_time_update(od, in, prev_epoch, b, f);
+                    flags |= NYXB_MSRF_REJECTED;
+                } else {
+                    // gain K = PHt S^-1 (Cholesky solve; plain inverse when S is not positive definite)
+                    double Si[2][2];
+                    if (!od_sinv(M, Sk, Si)) { rc = NYXB_ERR_PROP_MATH; break; }   // SingularKalmanGain
+                    for (int e = b.first(); e < 18; e += B::stride) {           // K[r][q]
+                        const int r = e >> 1, q = e & 1;
+                        double s = 0.0;
+                        if (q < M)
+                            for (int bb = 0; bb < M; ++bb) s += f.PHt[r * 2 + bb] * Si[bb][q];
+                        f.K[e] = s;
+                    }
+                    b.sync();
+                    // xhat and postfit in every lane, so that the state replacement stays in registers
+                    double xhat[9], post[2] = { 0.0, 0.0 };
+                    if (ekf) {
+                        for (int r = 0; r < 9; ++r) { double s = 0.0; for (int q = 0; q < M; ++q) s += f.K[r * 2 + q] * pre[q]; xhat[r] = s; }
+                        for (int q = 0; q < M; ++q) { double s = 0.0; for (int c = 0; c < 9; ++c) s += H[q][c] * xhat[c]; post[q] = pre[q] - s; }
+                    } else {
+                        double xbar[9];
+                        for (int r = 0; r < 9; ++r) { double s = 0.0; for (int c = 0; c < 9; ++c) s += b.phi[c * 9 + r] * f.xdev[c]; xbar[r] = s; }
+                        for (int q = 0; q < M; ++q) { double s = 0.0; for (int c = 0; c < 9; ++c) s += H[q][c] * xbar[c]; post[q] = pre[q] - s; }
+                        for (int r = 0; r < 9; ++r) { double s = 0.0; for (int q = 0; q < M; ++q) s += f.K[r * 2 + q] * post[q]; xhat[r] = xbar[r] + s; }
+                    }
+                    // Joseph update: (I - K H) Pbar (I - K H)^T + K R K^T, then symmetrise (filtering.rs:290-300)
+                    for (int e = b.first(); e < 81; e += B::stride) {           // F = I - K H
+                        const int r = e / 9, c = e - 9 * r;
+                        double s = 0.0;
+                        for (int q = 0; q < M; ++q) s += f.K[r * 2 + q] * H[q][c];
+                        f.F[e] = ((r == c) ? 1.0 : 0.0) - s;
+                    }
+                    b.sync();
+                    for (int e = b.first(); e < 81; e += B::stride) {           // T = F Pb
+                        const int r = e / 9, c = e - 9 * r;
+                        double s = 0.0;
+#pragma unroll
+                        for (int kk = 0; kk < 9; ++kk) s += f.F[r * 9 + kk] * f.Pb[kk * 9 + c];
+                        f.T[e] = s;
+                    }
+                    b.sync();
+                    for (int e = b.first(); e < 81; e += B::stride) {           // Pb <- T F^T + K R K^T (Pb is dead after T)
+                        const int r = e / 9, c = e - 9 * r;
+                        double s = 0.0;
+#pragma unroll
+                        for (int kk = 0; kk < 9; ++kk) s += f.T[r * 9 + kk] * f.F[c * 9 + kk];
+                        double s2 = 0.0;
+                        for (int q = 0; q < M; ++q) s2 += (f.K[r * 2 + q] * Rk[q]) * f.K[c * 2 + q];
+                        f.Pb[e] = s + s2;
+                    }
+                    b.sync();
+                    for (int e = b.first(); e < 81; e += B::stride) {
+                        const int r = e / 9, c = e - 9 * r;
+                        f.P[e] = 0.5 * (f.Pb[e] + f.Pb[c * 9 + r]);
+                    }
+                    for (int r = b.first(); r < 9; r += B::stride) f.xdev[r] = xhat[r];
+                    b.sync();
+                    prev_epoch = in.epoch_ns;
+                    if (od.postfit && b.lead()) for (int q = 0; q < w.ncur; ++q) od.postfit[((size_t)k * 2 + wno * M + q) * n + i] = post[q];
+                    if (ekf) {                                                  // :364-369 `Spacecraft + OVector<9>`
+                        for (int r = 0; r < 9; ++r) in.y[r] = in.y[r] + xhat[r];
+                        in.y[6] = in.y[6] < 0.0 ? 0.0 : (in.y[6] > 2.0 ? 2.0 : in.y[6]);
+                    }
+                }
+                od_reset_stm(b);                                                // reset_stm :371
+            }
+            for (int r = b.first(); r < 9; r += B::stride) {
+                if (od.est_state) od.est_state[((size_t)k * 9 + r) * n + i] = in.y[r];
+                if (od.est_cov) od.est_cov[((size_t)k * 9 + r) * n + i] = f.P[r * 9 + r];
+            }
+            break;
+        }
+        if (od.flags && b.lead()) od.flags[(size_t)k * n + i] = flags;
+    }
+    b.sync();
+    for (int e = b.first(); e < 81; e += B::stride) {
+        const int r = e / 9, c = e - 9 * r;
+        od.covar[(size_t)(c * 9 + r) * n + i] = f.P[e];
+    }
+    if (od.state_dev) for (int r = b.first(); r < 9; r += B::stride) od.state_dev[(size_t)r * n + i] = f.xdev[r];
+    od_store(b, in, rc, i, n, out_state, out_epoch, out_details, out_status);
+}

@@ -53,7 +53,7 @@ VARIANTS = {
 
 # Short SNC disable time: the filter time-updates after every integration step, so the time since the previous update is 45.5 s or 14.5 s
 # on a processed interval and 60 s after a measurement that was not visible (no update at its epoch).  A 50 s disable time therefore
-# takes both branches of the SNC code (nyxb_od.cu add_snc, nyxb_od_coop.cu w_covar_bar, snc.rs:188-196, 264-266).
+# takes both branches of the SNC code (nyxb_od_arc.cuh od_covar_bar, snc.rs:188-196, 264-266).
 
 # Field shapes: (config, degree, order).  Columns per lane of the warp-cooperative kernel: 1 up to degree 31, 2 for 32..63, 3 from 64.
 SHAPES = [("field", 8, 0), ("field", 8, 1), ("field", 8, 8), ("field", 21, 4), ("field", 31, 31), ("field", 32, 32),
