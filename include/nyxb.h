@@ -510,7 +510,10 @@ int32_t nyxb_engine_last_kernel(const nyxb_engine* eng);                   /* fa
  * Sets are only parked when there are more sets than CTAs. */
 int32_t nyxb_engine_set_tx_tuning(nyxb_engine* eng, int32_t slice_attempts, int32_t max_ctas);
 int32_t nyxb_engine_set_tx_positions(nyxb_engine* eng, int32_t positions);   /* walker warps per set: 0 = by degree, 8, 10, 16 */
-int32_t nyxb_engine_set_lanes(nyxb_engine* eng, int32_t lanes_per_trajectory); /* 0 = auto */
+/* 0 = auto, 1, 8, 16, 32.  STRICT mode keeps each trajectory's Legendre triangle in shared memory, which limits the forced lane
+ * counts by degree: 8 lanes up to degree 50, 16 up to 75, 32 up to 96.  Above that the call returns NYXB_RC_UNSUPPORTED and the
+ * setting is unchanged.  The automatic choice always fits. */
+int32_t nyxb_engine_set_lanes(nyxb_engine* eng, int32_t lanes_per_trajectory);
 int32_t nyxb_engine_get_lanes(const nyxb_engine* eng);
 int64_t nyxb_engine_launch_count(const nyxb_engine* eng); /* kernels launched so far */
 double nyxb_engine_last_kernel_ms(const nyxb_engine* eng); /* CUDA-event time of the last launch (host API only) */
@@ -522,7 +525,8 @@ double nyxb_measure_fp64_tflops(int32_t device, int32_t iters);
 /* Host-only inspection of the cooperative kernel's coefficient table (no device needed): the column -> lane
  * schedule and the packed records for `lanes` in {8,16,32}.  Two-call pattern: with recs == NULL only the sizes are
  * returned.  Layouts: recs [(L+2)/2 pairs][5 pieces][lanes][2], col_start / col_m [lanes][kmax], colseed [N+2][4]
- * (see nyx_b200/csrc/nyxb_coop.h).  Used by the CPU tests to check the table algebra against a direct evaluation. */
+ * (see nyx_b200/csrc/nyxb_coop.h); col_m = N + 2 marks a stop column (zero seed, no records) that ends a column's recursion
+ * before a long idle gap of its lane.  Used by the CPU tests to check the table algebra against a direct evaluation. */
 int32_t nyxb_coop_table_dump(const nyxb_gravity_field* field, int32_t lanes, int32_t* out_L, int32_t* out_kmax,
                              double* recs, int32_t* col_start, int32_t* col_m, double* colseed);
 

@@ -1153,6 +1153,11 @@ extern "C" int32_t nyxb_engine_set_lanes(nyxb_engine* eng, int32_t lanes) {
         set_err("cooperative lanes need a gravity field");
         return NYXB_RC_UNSUPPORTED;
     }
+    if (lanes > 1 && eng->mode == NYXB_MODE_STRICT && nyxb_coop_strict_smem(eng->S.grav.N, lanes) > NYXB_COOP_STRICT_SMEM_MAX) {
+        set_err("STRICT cooperative kernel: the shared-memory slabs of a degree-" + std::to_string(eng->S.grav.N) + " field at " +
+                std::to_string(lanes) + " lanes per trajectory exceed the 227 KB of a block (8 lanes: degree <= 50, 16 lanes: <= 75)");
+        return NYXB_RC_UNSUPPORTED;
+    }
     eng->lanes = lanes;
     return NYXB_RC_OK;
 }

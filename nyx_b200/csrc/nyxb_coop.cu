@@ -134,6 +134,27 @@ void nyxb_coop_build_host(int N, int M, const double* c_nm, const double* s_nm, 
         }
         align_boundaries(cap, col_len, cols, starts, load);
     }
+    // Through an idle gap of its lane (null records) a column's recursion keeps running past its last degree, and
+    // |Q[n][m]| <= rho^n (n+m)! / (2^m m!) grows without bound: near the surface it overflows once n reaches ~160 (95x95 on 32 lanes
+    // idles for 62 entries), and inf x 0 = NaN would enter the sums.  Where that bound passes 1e300 before the lane's next column
+    // (or the end of the walk), a stop column m = N + 2 starts at the end of the column: its seed is zero, so Q stays 0.
+    const int L = *std::max_element(load.begin(), load.end());
+    for (int lane = 0; lane < G; ++lane) {
+        std::vector<std::pair<int, int>> sc;
+        for (size_t k = 0; k < cols[lane].size(); ++k) sc.push_back({starts[lane][k], cols[lane][k]});
+        std::sort(sc.begin(), sc.end());
+        std::vector<std::pair<int, int>> with_stops;
+        for (size_t k = 0; k < sc.size(); ++k) {
+            with_stops.push_back(sc[k]);
+            const int m = sc[k].second, end = sc[k].first + col_len(m), next = k + 1 < sc.size() ? sc[k + 1].first : L;
+            const int n_top = m + (next - sc[k].first) + 2;   // highest degree the recursion reaches before the next switch
+            if (next > end && std::lgamma(n_top + m + 1.0) - m * std::log(2.0) - std::lgamma(m + 1.0) > 300.0 * std::log(10.0))
+                with_stops.push_back({end, N + 2});
+        }
+        cols[lane].clear();
+        starts[lane].clear();
+        for (auto& p : with_stops) { starts[lane].push_back(p.first); cols[lane].push_back(p.second); }
+    }
     out.G = G;
     out.L = *std::max_element(load.begin(), load.end());
     out.kmax = 1;
@@ -172,6 +193,7 @@ void nyxb_coop_build_host(int N, int M, const double* c_nm, const double* s_nm, 
             int e = starts[lane][k];
             out.col_start[(size_t)lane * out.kmax + k] = e;
             out.col_m[(size_t)lane * out.kmax + k] = m;
+            if (m == N + 2) continue;   // stop column: no records
             auto kappa = [&](int n) -> double {  // W term of degree n = kappa * (Z term of degree n-1), n > m
                 return (double)(((long double)vr11(n - 1, m - 1) * scale(n, m)) / ((long double)vr01(n - 1, m - 1) * scale(n - 1, m)));
             };

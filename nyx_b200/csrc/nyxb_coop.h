@@ -45,6 +45,10 @@ struct CoopStrictHost {
     std::vector<int> cols, rows;
 };
 void nyxb_coop_strict_build_host(int N, int M, int G, CoopStrictHost& out);
+// dynamic shared memory of one CTA of the STRICT cooperative kernel at degree N and G lanes per trajectory, and its limit (the
+// opt-in maximum per block on sm_90): the per-trajectory triangle grows as N^2 / 2, so 8 lanes fit up to degree 50, 16 up to 75
+size_t nyxb_coop_strict_smem(int N, int G);
+#define NYXB_COOP_STRICT_SMEM_MAX (227 * 1024)
 extern "C" cudaError_t nyxb_launch_coop_strict(const DevSetup* S, const DevCoopStrict* Cs, size_t n, const double* state,
                                                const double* consts, const long long* epoch0, long long end_epoch,
                                                long long* step_io, double* out_state, long long* out_epoch,

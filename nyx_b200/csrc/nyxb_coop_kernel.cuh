@@ -37,10 +37,11 @@ __host__ __device__ inline int coop_traj_stride(int N) {
     int s = COOP_SM_FIXED + 3 * (N + 3);
     return s + ((8 - (s & 15)) & 15);
 }
-// bytes of the CTA-shared table region: records [(L+2)/2 pairs][5 x 16 B][G], then colseed[N+2][4], col_start/col_m [G][kmax+2]
+// bytes of the CTA-shared table region: records [(L+2)/2 pairs][5 x 16 B][G], then colseed[N+3][4] (row N+2 zero: the seed of
+// the stop column, see nyxb_coop_build_host), col_start/col_m [G][kmax+2]
 __host__ __device__ inline size_t coop_rec_bytes(int L, int G) { return (size_t)(L + 2) * G * NYXB_COOP_REC_BYTES; }
 __host__ __device__ inline size_t coop_meta_bytes(int N, int G, int kmax) {
-    size_t b = (size_t)(N + 2) * 32 + (size_t)2 * G * (kmax + 2) * 4;
+    size_t b = (size_t)(N + 3) * 32 + (size_t)2 * G * (kmax + 2) * 4;
     return (b + 15) & ~(size_t)15;
 }
 
@@ -136,7 +137,7 @@ __device__ __forceinline__ int coop_rhs(const DevSetup& S, const double* __restr
             bzr = nb;
             bp *= bp;
         }
-        const int top = gv.N + 1;
+        const int top = gv.N + 2;   // N + 2: the stop column's (zero) seed
         for (int k = lane; k <= top; k += G) {
             g.rm[k] = zr; g.im[k] = zi; g.rp[k] = pr * colseed[4 * k];  // rho^k (2k-1)!!: the seed Q[k][k] of column k
             const double nzr = fma(zr, bzr, -(zi * bzi));
@@ -304,7 +305,7 @@ nyxb_k_coop(const __grid_constant__ DevSetup S, const __grid_constant__ DevCoop 
     const size_t rec_bytes = SMEM_TABLE ? coop_rec_bytes(Cp.L, G) : 0;
     unsigned char* meta = smem_raw + rec_bytes;
     double* sm_seed = reinterpret_cast<double*>(meta);
-    int* sm_cs = reinterpret_cast<int*>(meta + (size_t)(N + 2) * 32);
+    int* sm_cs = reinterpret_cast<int*>(meta + (size_t)(N + 3) * 32);
     int* sm_cm = sm_cs + G * (Cp.kmax + 2);
     if (SMEM_TABLE) {
         if (tid == 0) mbar_init(&tma_bar, 1);
@@ -314,7 +315,7 @@ nyxb_k_coop(const __grid_constant__ DevSetup S, const __grid_constant__ DevCoop 
             tma_bulk_g2s(smem_raw, Cp.recs, (unsigned)rec_bytes, &tma_bar);
         }
     }
-    for (int k = tid; k < (N + 2) * 4; k += COOP_CTA) sm_seed[k] = __ldg(Cp.colseed + k);
+    for (int k = tid; k < (N + 3) * 4; k += COOP_CTA) sm_seed[k] = k < (N + 2) * 4 ? __ldg(Cp.colseed + k) : 0.0;
     for (int k = tid; k < G * (Cp.kmax + 2); k += COOP_CTA) {
         const int l = k / (Cp.kmax + 2), q = k % (Cp.kmax + 2);
         sm_cs[k] = (q < Cp.kmax) ? __ldg(Cp.col_start + l * Cp.kmax + q) : Cp.L + 1;

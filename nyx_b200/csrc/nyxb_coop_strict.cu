@@ -33,6 +33,8 @@ __host__ __device__ inline int scoop_traj_stride(int N) {
     return s + ((8 - (s & 15)) & 15);
 }
 
+size_t nyxb_coop_strict_smem(int N, int G) { return (size_t)(SCOOP_CTA / G) * (size_t)scoop_traj_stride(N) * sizeof(double); }
+
 void nyxb_coop_strict_build_host(int N, int M, int G, CoopStrictHost& out) {
     auto lpt = [&](const std::vector<std::pair<int, int>>& items /* (id, weight), any order */, std::vector<std::vector<int>>& lists) {
         std::vector<std::pair<int, int>> it = items;
@@ -405,8 +407,8 @@ static cudaError_t launch_strict_g(const DevSetup* S, const DevCoopStrict* Cs, s
                                    long long* out_epoch, nyxb_details* out_details, int* out_status, const DevSink* sink,
                                    cudaStream_t stream) {
     const size_t groups = SCOOP_CTA / G;
-    const size_t smem = groups * (size_t)scoop_traj_stride(S->grav.N) * sizeof(double);
-    if (smem > 227 * 1024) return cudaErrorInvalidConfiguration;
+    const size_t smem = nyxb_coop_strict_smem(S->grav.N, G);
+    if (smem > NYXB_COOP_STRICT_SMEM_MAX) return cudaErrorInvalidConfiguration;   // nyxb_engine_set_lanes refuses these first
     cudaError_t e = cudaFuncSetAttribute(nyxb_k_coop_strict<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     int dev = 0, sms = 0, occ = 0;

@@ -17,7 +17,7 @@
 // another order than the per-thread one (tolerance parity, tests/test_gpu_stm_od.py).
 #include "nyxb_od_arc.cuh"
 
-#define ODC_KMAX 4           // columns per lane (>= ceil((N+1)/32) + 1)
+#define ODC_KMAX 4           // columns per lane (>= the host's deal of the N+1 columns over 32 lanes: 4 at N = 96)
 #define ODC_WPB 4            // warps (filters) per block
 #define FULL 0xffffffffu
 

@@ -20,8 +20,10 @@ stations; BASELINE configs[4] in small).
 
 Field shapes where the code paths switch.  The warp-cooperative filter deals the columns m = 0..min(M, N) of the Legendre triangle
 to 32 lanes (nyxb_api.cu, nyxb_od_ekf_batch) and builds its z^j / rho^j power table in ceil((N + 1) / 32) passes: one column per
-lane and one pass up to N = 31, two for N = 32..63, three for N = 64..95 (coop_columns_per_lane below restates the deal).  Degree 96
-would take four columns per lane (ODC_KMAX); no fixture goes that high, so that case is not run."""
+lane and one pass up to N = 31, two for N = 32..63, three for N = 64..95 and four at N = 96 (coop_columns_per_lane below restates
+the deal).  Only the full 96x96 field gives a lane four columns (ODC_KMAX); 96x95 has 96 columns, three per lane, with four passes.
+Above the fixtures' top degrees (JGM-3 70, Luna 80) `gravity` takes the degree-96 fields of tests/high_degree.py, whose extra rows
+are seeded draws; those shapes run in tests/test_gpu_high_degree.py."""
 import functools
 
 import numpy as np
@@ -29,6 +31,7 @@ import numpy as np
 import nyx_b200 as nb
 from nyx_b200.frames import EARTH
 from tests import fast_matrix as fm
+from tests import high_degree as hd
 
 S = 10**9
 N_F = 13
@@ -84,7 +87,11 @@ def almanac(config):
 
 def gravity(config, degree, order):
     if config == "lunar":
+        if degree > 80:
+            return nb.GravityField.new(hd.field_data("moon", degree, order))
         return nb.GravityField.new(nb.GravityFieldData.from_fixture("luna_jggrx_80x80", degree, order, nb.IAU_MOON_FRAME))
+    if degree > 70:
+        return nb.GravityField.new(hd.field_data("earth", degree, order))
     return fm.field(degree, order)
 
 

@@ -38,7 +38,8 @@ def _walk(gf, lanes, tables, rb):
     z = complex(s_, t_)
     rm = np.array([(z**k).real for k in range(N + 2)])
     im = np.array([(z**k).imag for k in range(N + 2)])
-    rp = np.array([rho**k * seed[k, 0] for k in range(N + 2)])
+    seed = np.vstack([seed, np.zeros(4)])   # row N + 2: the zero seed of the stop column
+    rp = np.array([rho**k * seed[k, 0] for k in range(N + 3)])
     X = Y = Z = W = 0.0
     for lane in range(lanes):
         starts = {int(col_start[lane, k]): int(col_m[lane, k]) for k in range(kmax) if col_start[lane, k] <= L}
@@ -86,19 +87,25 @@ def test_cooperative_table_reproduces_oracle_gravity(oracle, fixture, degree, or
     start columns on common entries)."""
     moon = fixture.startswith("luna")
     body_frame = nb.IAU_MOON_FRAME if moon else nb.IAU_EARTH_FRAME
-    # identity rotation: the harmonic sum is exercised directly in the integration frame
     gd = nb.GravityFieldData.from_fixture(fixture, degree, order, body_frame.with_rotation(None) if hasattr(body_frame, "with_rotation") else body_frame)
+    check_table(oracle, gd, nb.MOON_J2000 if moon else nb.EARTH_J2000, lanes)
+
+
+def check_table(oracle, gd, frame, lanes, radii=(1.03, 1.6), points=4):
+    """Schedule invariants of the field `gd` at `lanes`, and the walk against the oracle's harmonic acceleration at `points`
+    points between radii[0] and radii[1] x r_eq."""
     dyn = nb.SpacecraftDynamics.new(nb.OrbitalDynamics.from_model(nb.GravityField.new(gd)))
-    frame = nb.MOON_J2000 if moon else nb.EARTH_J2000
     packed = dyn.pack(frame, None)
     gf = packed.c.gravity.contents
-    gf.rot.kind = 0
+    gf.rot.kind = 0   # identity rotation: the harmonic sum is exercised directly in the integration frame
     tables = _dump(packed, lanes)
     L, kmax, recs, col_start, col_m, seed = tables
-    # schedule invariants: even column boundaries, every column m = 1..min(order, degree)+1 present exactly once
+    # schedule invariants: even column boundaries, every column m = 1..min(order, degree)+1 present exactly once, and stop columns
+    # (m = N + 2, zero seed) only where a column is followed by an idle gap
     real = col_start <= L
     assert L % 2 == 0 and (col_start[real] % 2 == 0).all()
-    assert sorted(col_m[real].tolist()) == list(range(1, min(gf.order + 1, gf.degree + 1) + 1))
+    cols = col_m[real & (col_m != gf.degree + 2)]
+    assert sorted(cols.tolist()) == list(range(1, min(gf.order + 1, gf.degree + 1) + 1))
     for lane in range(lanes):   # columns of a lane do not overlap and end inside the walk
         ends = 0
         for k in range(kmax):
@@ -111,9 +118,9 @@ def test_cooperative_table_reproduces_oracle_gravity(oracle, fixture, degree, or
         assert ends <= L
     rng = np.random.default_rng(5)
     R = gf.r_eq_km
-    for _ in range(4):
+    for _ in range(points):
         d = rng.normal(size=3)
-        rb = d / np.linalg.norm(d) * R * rng.uniform(1.03, 1.6)
+        rb = d / np.linalg.norm(d) * R * rng.uniform(*radii)
         y = np.concatenate([rb, [0.0, 0.0, 0.0, 1.8, 2.2, 0.0]])
         consts = np.array([100.0, 0.0, 1.0, 1.0])
         dy = np.zeros(9)
