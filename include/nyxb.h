@@ -35,7 +35,8 @@ extern "C" {
 #endif
 
 #define NYXB_ABI_VERSION 4 /* 4: nyxb_engine_set_kernel / nyxb_engine_last_kernel / nyxb_engine_set_tx_tuning, nyxb_tx_table_dump, nyxb_propagate_batch_multi, nyxb_reference_normals;
-                              nyxb_integ_opts.state_center, nyxb_gravity_field.body, nyxb_dynamics.n_gravity / n_point_masses / point_mass_order.  Earlier: 2: nyxb_srp gained `estimate`; STM, filter and dispersion entry points.  3: nyxb_traj_resample[_dev], nyxb_event_locate[_dev] */
+                              nyxb_integ_opts.state_center, nyxb_gravity_field.body, nyxb_dynamics.n_gravity / n_point_masses / point_mass_order; nyxb_od_predict_batch
+                              and nyxb_predict_outputs were added later without a bump (a pure addition: no existing type or entry point changed).  Earlier: 2: nyxb_srp gained `estimate`; STM, filter and dispersion entry points.  3: nyxb_traj_resample[_dev], nyxb_event_locate[_dev] */
 
 /* ---- IntegratorMethod — propagators/rk_methods/mod.rs:65-79 (same order) ---- */
 enum nyxb_method {
@@ -470,6 +471,36 @@ int32_t nyxb_od_ekf_batch(nyxb_engine* eng, const nyxb_od_config* cfg,
                           const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
                           const double* covar0_soa, const nyxb_od_outputs* out);
 
+/* ---- Covariance mapping over an ensemble: n independent `KalmanODProcess::predict_until` runs (od/process/mod.rs:440-486) in ONE
+ * kernel launch.  Record 0 is the initial estimate; then chunks of cfg->max_step_ns (`for_duration(max_step)`: adaptive steps, the
+ * last one cut to land on the chunk end; the adaptive step carries over, and the first chunk starts from opts.init_step: no
+ * set_step(max_step) here), each closed by `KalmanFilter::time_update` (P = Phi P Phi^T + SNC; CKF deviation Phi x, EKF zero) and an
+ * STM reset, until the first chunk end at or after end_epoch_ns[i].  So record k sits at epoch0_ns[i] + k*max_step_ns exactly, a run
+ * has 1 + max(1, ceil((end - epoch0) / max_step)) records, the last may overshoot the end by up to max_step - 1 ns, and an end at
+ * or before the start gives two records.
+ * Of cfg only variant, max_step_ns and the snc_* fields are read.  max_step_ns <= 0 is rejected with NYXB_RC_BAD_ARG (the reference
+ * does not check it and would loop forever).  The setups nyxb_propagate_batch_stm rejects return NYXB_RC_UNSUPPORTED.  A propagation
+ * error ends that run with its status; the records written up to then stay valid.  Kernel family as nyxb_od_ekf_batch. */
+typedef struct {
+    double* state_soa;           /* [9][n]  final nominal state */
+    int64_t* epoch_ns;           /* [n]     epoch of the last record */
+    double* covar_soa;           /* [81][n] final covariance, (r,c) at [(c*9+r)*n + i] */
+    double* state_dev_soa;       /* [9][n]  final state deviation, or NULL */
+    nyxb_details* details;       /* [n] or NULL: n_steps / n_rhs over the whole prediction */
+    int32_t* status;             /* [n] */
+    int64_t capacity;            /* records kept per run; records k >= capacity are dropped (as nyxb_traj_sink) */
+    double* rec_state;           /* [capacity][9][n] or NULL: estimate.state() = nominal + deviation (Cr clamped), [(k*9 + r)*n + i] */
+    double* rec_covar;           /* [capacity][81][n] or NULL: covariance, (r,c) at [(k*81 + c*9 + r)*n + i] */
+    int64_t* rec_count;          /* [n] or NULL: records produced by run i (kept or not) */
+} nyxb_predict_outputs;
+
+/* state_soa/consts_soa/epoch0_ns/covar0_soa as in nyxb_od_ekf_batch (initial_estimate.nominal_state, .covar);
+ * state_dev0_soa [9][n] initial state deviation (initial_estimate.state_deviation) or NULL = 0; HOST pointers everywhere. */
+int32_t nyxb_od_predict_batch(nyxb_engine* eng, const nyxb_od_config* cfg, size_t n,
+                              const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
+                              const int64_t* end_epoch_ns, const double* covar0_soa, const double* state_dev0_soa,
+                              const nyxb_predict_outputs* out);
+
 /* ---- On-device Monte Carlo dispersions (next row (f)-4): `MvnSpacecraft::sample` (mc/multivariate.rs:298-331) for the
  * runs [first_index, first_index + n): state_i = template + (sqrt_s_v * z_i + mean), z_i ~ N(0, I_9) drawn from a
  * counter-based stream keyed by (seed, run index) — Philox4x32-10 + Box-Muller, see nyx_b200/csrc/nyxb_mvn.cu — so that a
@@ -504,8 +535,9 @@ int32_t nyxb_ziggurat_tables(double* x257, double* f257);                       
 enum nyxb_kernel { NYXB_KERNEL_AUTO = 0, NYXB_KERNEL_THREAD = 1, NYXB_KERNEL_COOP = 2, NYXB_KERNEL_TRANSPOSED = 3 };
 int32_t nyxb_engine_set_kernel(nyxb_engine* eng, int32_t kernel);          /* enum nyxb_kernel; NYXB_RC_UNSUPPORTED if the setup cannot use it */
 int32_t nyxb_engine_last_kernel(const nyxb_engine* eng);                   /* family used by the last propagation launch */
-/* nyxb_propagate_batch_stm sets it to THREAD (one thread per trajectory, STRICT and FAST).  nyxb_od_ekf_batch sets it to COOP
- * when it ran the warp-cooperative filter (FAST, field of degree >= 8, kernel not forced to THREAD), else to THREAD. */
+/* nyxb_propagate_batch_stm sets it to THREAD (one thread per trajectory, STRICT and FAST).  nyxb_od_ekf_batch and
+ * nyxb_od_predict_batch set it to COOP when they ran the warp-cooperative kernel (FAST, field of degree >= 8, kernel not forced to
+ * THREAD), else to THREAD. */
 /* TRANSPOSED kernel: step attempts per time slice (default 64) and an upper bound on the persistent CTAs (0 = SMs x occupancy).
  * Sets are only parked when there are more sets than CTAs. */
 int32_t nyxb_engine_set_tx_tuning(nyxb_engine* eng, int32_t slice_attempts, int32_t max_ctas);

@@ -483,8 +483,8 @@ struct ProcessNoise3D {   // od/snc.rs:38-56, 118-134, 288-311
     }
 };
 
-struct KfEstimate {   // od/estimate/kfestimate.rs: nominal state + 9x9 covariance (row-major here)
-    Spacecraft nominal_state; double covar[81] = {0};
+struct KfEstimate {   // od/estimate/kfestimate.rs: nominal state + 9x9 covariance (row-major here) + state deviation
+    Spacecraft nominal_state; double covar[81] = {0}; double state_deviation[9] = {0};
     static KfEstimate from_diag(const Spacecraft& s, const double (&d)[9]) { KfEstimate e; e.nominal_state = s; for (int i = 0; i < 9; ++i) e.covar[i * 9 + i] = d[i]; return e; }
 };
 
@@ -498,6 +498,16 @@ struct ODSolution {
     Spacecraft final_state(const Spacecraft& tmpl, size_t i) const { return detail::unpack(tmpl, state, epoch, n, i); }
 };
 
+// Covariance mapping of one estimate (KalmanODProcess::predict_until): record k at epoch0 + k * max_step, k < count
+struct PredictionSolution {
+    int64_t epoch0 = 0, max_step = 0, count = 0;
+    std::vector<double> rec_state, rec_covar;   // [count][9] estimate.state(), [count][81] (c*9+r)
+    double state[9] = {0}, covar[81] = {0}, state_dev[9] = {0};   // final nominal state, covariance (c*9+r), deviation
+    int64_t epoch = 0; int32_t status = 0; nyxb_details details{};
+    int64_t record_epoch(int64_t k) const { return epoch0 + k * max_step; }
+    double record_covar(int64_t k, int r, int c) const { return rec_covar[(size_t)k * 81 + c * 9 + r]; }
+};
+
 // KalmanODProcess (od/process/{initializers.rs:60-113, mod.rs:128-497}); msr_size 2 = SpacecraftKalmanOD, 1 = SpacecraftKalmanScalarOD
 class KalmanODProcess {
   public:
@@ -507,6 +517,39 @@ class KalmanODProcess {
     KalmanODProcess(Propagator p, KalmanVariant v, std::optional<SigmaRejection> rej, std::vector<GroundStation> dev, const Almanac* alm = nullptr, int32_t msr = 2)
         : prop(std::move(p)), variant(v), sigma_reject(rej), devices(std::move(dev)), almanac(alm), msr_size(msr) {}
     KalmanODProcess& with_process_noise(ProcessNoise3D snc) { process_noise = snc; return *this; }
+
+    nyxb_od_config config() const {
+        nyxb_od_config cfg{};
+        cfg.variant = (int32_t)variant; cfg.msr_size = msr_size; cfg.reject_num_sigmas = sigma_reject ? sigma_reject->num_sigmas : -1.0;
+        cfg.max_step_ns = max_step; cfg.epoch_precision_ns = epoch_precision;
+        if (process_noise) { cfg.snc_enabled = 1; cfg.snc_frame = process_noise->ric ? 1 : 0; for (int i = 0; i < 3; ++i) cfg.snc_diag[i] = process_noise->diag[i]; cfg.snc_disable_time_ns = process_noise->disable_time; }
+        return cfg;
+    }
+
+    // KalmanODProcess::predict_until / predict_for (od/process/mod.rs:440-496): every record of the time updates
+    PredictionSolution predict_until(const KfEstimate& initial, int64_t end_epoch) const {
+        const Frame& frame = initial.nominal_state.frame;
+        auto eng = detail::make_engine(prop.dynamics, frame, almanac, prop.method, prop.opts, prop.mode, prop.device);
+        detail::Soa soa(std::vector<Spacecraft>{initial.nominal_state});
+        const nyxb_od_config cfg = config();
+        if (cfg.max_step_ns <= 0) throw std::runtime_error("StepSize: max_step must be positive");
+        double cov0[81];
+        for (int r = 0; r < 9; ++r) for (int c = 0; c < 9; ++c) cov0[c * 9 + r] = initial.covar[r * 9 + c];
+        const int64_t epoch0 = soa.epoch[0], span = end_epoch - epoch0;
+        const int64_t cap = 1 + (span > 0 ? (span + max_step - 1) / max_step : 1);
+        PredictionSolution s; s.epoch0 = epoch0; s.max_step = max_step;
+        s.rec_state.resize((size_t)cap * 9); s.rec_covar.resize((size_t)cap * 81);
+        nyxb_predict_outputs out{s.state, &s.epoch, s.covar, s.state_dev, &s.details, &s.status, cap, s.rec_state.data(), s.rec_covar.data(), &s.count};
+        if (nyxb_od_predict_batch(eng.get(), &cfg, 1, soa.state.data(), soa.consts.data(), soa.epoch.data(), &end_epoch, cov0,
+                                  initial.state_deviation, &out) != NYXB_RC_OK)
+            throw std::runtime_error(std::string("nyxb_od_predict_batch: ") + nyxb_last_error());
+        if (s.count > cap) s.count = cap;
+        s.rec_state.resize((size_t)s.count * 9); s.rec_covar.resize((size_t)s.count * 81);
+        return s;
+    }
+    PredictionSolution predict_for(const KfEstimate& initial, int64_t duration) const {
+        return predict_until(initial, initial.nominal_state.epoch() + duration);
+    }
 
     ODSolution process_arcs(const std::vector<KfEstimate>& initial, const TrackingDataArc& arc) const {
         const size_t n = initial.size(), m = arc.epoch_ns.size();
@@ -530,10 +573,7 @@ class KalmanODProcess {
         }
         std::vector<int32_t> trk(m);
         for (size_t k = 0; k < m; ++k) { trk[k] = -1; for (size_t j = 0; j < devices.size(); ++j) if (devices[j].name == arc.tracker[k]) trk[k] = (int32_t)j; }
-        nyxb_od_config cfg{};
-        cfg.variant = (int32_t)variant; cfg.msr_size = msr_size; cfg.reject_num_sigmas = sigma_reject ? sigma_reject->num_sigmas : -1.0;
-        cfg.max_step_ns = max_step; cfg.epoch_precision_ns = epoch_precision;
-        if (process_noise) { cfg.snc_enabled = 1; cfg.snc_frame = process_noise->ric ? 1 : 0; for (int i = 0; i < 3; ++i) cfg.snc_diag[i] = process_noise->diag[i]; cfg.snc_disable_time_ns = process_noise->disable_time; }
+        const nyxb_od_config cfg = config();
         nyxb_tracking_arc carc{(int64_t)m, arc.epoch_ns.data(), trk.data(), arc.obs.data()};
         ODSolution s; s.n = n; s.m = m;
         s.state.resize(9 * n); s.epoch.resize(n); s.covar.resize(81 * n); s.state_dev.resize(9 * n); s.resid_ratio.resize(m * 2 * n); s.prefit.resize(m * 2 * n);

@@ -20,7 +20,7 @@ from . import dhall
 from .config import PropagatorConfig, integrator_options_from, load_ground_stations, parse_duration
 from .event import Event, brent, locate_event
 from .od import (GroundStation, KalmanODProcess, KalmanVariant, KfEstimate, LocalFrame, MeasurementType, ODError, ODSolution,
-                 ProcessNoise3D, SigmaRejection, SpacecraftKalmanOD, SpacecraftKalmanScalarOD, SpacecraftUncertainty,
+                 PredictionSolution, ProcessNoise3D, SigmaRejection, SpacecraftKalmanOD, SpacecraftKalmanScalarOD, SpacecraftUncertainty,
                  StochasticNoise, TrackingDataArc, simulate_tracking, station_state)
 from .propagator import (Engine, ErrorControl, IntegrationDetails, IntegratorMethod, IntegratorOptions, PropagationError,
                          PropInstance, Propagator)

@@ -159,7 +159,8 @@ class EventC(C.Structure):
     ]
 
 
-# ---- orbit determination (SURVEY.md §8 (f)-2): mirrors of nyxb_ground_station / nyxb_od_config / nyxb_tracking_arc / nyxb_od_outputs
+# ---- orbit determination (SURVEY.md §8 (f)-2): mirrors of nyxb_ground_station / nyxb_od_config / nyxb_tracking_arc / nyxb_od_outputs /
+# nyxb_predict_outputs
 MSR_RANGE, MSR_DOPPLER = 0, 1
 KF_REFERENCE_UPDATE, KF_DEVIATION_TRACKING = 0, 1
 MSRF_PROCESSED, MSRF_REJECTED, MSRF_NOT_VISIBLE, MSRF_ABSENT = 1, 2, 4, 8
@@ -218,6 +219,21 @@ class OdOutputsC(C.Structure):
         ("est_covar_diag", C.c_void_p),
         ("details", C.c_void_p),
         ("status", C.c_void_p),
+    ]
+
+
+class PredictOutputsC(C.Structure):
+    _fields_ = [
+        ("state_soa", C.c_void_p),
+        ("epoch_ns", C.c_void_p),
+        ("covar_soa", C.c_void_p),
+        ("state_dev_soa", C.c_void_p),
+        ("details", C.c_void_p),
+        ("status", C.c_void_p),
+        ("capacity", C.c_int64),
+        ("rec_state", C.c_void_p),
+        ("rec_covar", C.c_void_p),
+        ("rec_count", C.c_void_p),
     ]
 
 
@@ -292,6 +308,8 @@ def _declare(lib):
     lib.nyxb_od_ekf_batch.restype = C.c_int32
     lib.nyxb_od_ekf_batch.argtypes = [vp, C.POINTER(OdConfigC), C.c_int32, C.POINTER(GroundStationC), C.POINTER(TrackingArcC),
                                       C.c_size_t, vp, vp, vp, vp, C.POINTER(OdOutputsC)]
+    lib.nyxb_od_predict_batch.restype = C.c_int32
+    lib.nyxb_od_predict_batch.argtypes = [vp, C.POINTER(OdConfigC), C.c_size_t, vp, vp, vp, vp, vp, vp, C.POINTER(PredictOutputsC)]
     lib.nyxb_mvn_sample.restype = C.c_int32
     lib.nyxb_mvn_sample.argtypes = [C.c_int32, C.c_uint64, C.c_uint64, C.c_size_t, vp, vp, vp, vp, vp]
     lib.nyxb_mvn_sample_dev.restype = C.c_int32
@@ -346,6 +364,7 @@ EXPORTED_SYMBOLS = [
     "nyxb_propagate_batch_event",
     "nyxb_propagate_batch_stm",
     "nyxb_od_ekf_batch",
+    "nyxb_od_predict_batch",
     "nyxb_mvn_sample",
     "nyxb_mvn_sample_dev",
     "nyxb_reference_normals",

@@ -27,6 +27,9 @@ extern "C" double nyxb_fp64_probe(int device, int iters);
 extern "C" cudaError_t nyxb_launch_frame_shift(const DevBody*, double, size_t, double*, const long long*, int*, cudaStream_t);
 extern "C" cudaError_t nyxb_launch_od_coop(const DevSetup*, const DevOd*, const int*, size_t, const double*, const double*, const long long*,
                                            double*, long long*, nyxb_details*, int*, cudaStream_t);
+extern "C" cudaError_t nyxb_launch_pred_coop(const DevSetup*, const DevOd*, const int*, size_t, const double*, const double*,
+                                             const long long*, const long long*, const double*, const OdRecords*, long long*, double*,
+                                             long long*, nyxb_details*, int*, cudaStream_t);
 extern "C" int nyxb_od_coop_kmax(void);
 extern "C" cudaError_t nyxb_launch_traj_resample(long long, const long long*, const double*, const long long*, size_t, size_t,
                                                  const long long*, double*, int*, cudaStream_t);
@@ -809,6 +812,29 @@ bool stm_supported(const nyxb_engine* e) {
     }
     return true;
 }
+// Kernel family of the filter and prediction calls.  FAST mode with a gravity field of degree >= 8: one WARP per filter, the harmonic
+// gradient split by columns over the lanes (nyxb_od_coop.cu); columns -> lanes by longest-processing-time, uploaded to d_cols.
+// nyxb_engine_set_kernel(NYXB_KERNEL_THREAD) forces the per-thread kernel, and so does a deal that needs more than
+// nyxb_od_coop_kmax() columns on one lane.  d_cols stays null for the per-thread kernel.
+int32_t od_coop_cols(const nyxb_engine* eng, DevBufs& B, cudaStream_t st, const int*& d_cols) {
+    d_cols = nullptr;
+    bool coop = eng->mode == NYXB_MODE_FAST && eng->S.has_grav && eng->S.grav.N >= 8 && eng->kernel != NYXB_KERNEL_THREAD;
+    if (!coop) return NYXB_RC_OK;
+    const int N = eng->S.grav.N, mtop = eng->S.grav.M < N ? eng->S.grav.M : N, kmax = nyxb_od_coop_kmax();
+    std::vector<int> cols(32 * (size_t)kmax, -1), cnt(32, 0);
+    std::vector<long long> load(32, 0);
+    for (int m = 0; m <= mtop; ++m) {   // columns in decreasing length order: m = 0, 1 (same length), 2, ...
+        int best = 0;
+        for (int l = 1; l < 32; ++l)
+            if (load[l] < load[best] || (load[l] == load[best] && cnt[l] < cnt[best])) best = l;
+        if (cnt[best] >= kmax) return NYXB_RC_OK;
+        cols[(size_t)best * kmax + cnt[best]++] = m;
+        load[best] += N - (m > 0 ? m : 1) + 1 + 6;   // entries + per-column overhead
+    }
+    d_cols = B.put(cols.data(), cols.size(), st);
+    if (!d_cols) { set_err("device allocation / upload failed"); return NYXB_RC_CUDA; }
+    return NYXB_RC_OK;
+}
 }  // namespace
 
 extern "C" int32_t nyxb_propagate_batch_stm(nyxb_engine* eng, size_t n, const double* state_soa, const double* consts_soa,
@@ -941,28 +967,9 @@ extern "C" int32_t nyxb_od_ekf_batch(nyxb_engine* eng, const nyxb_od_config* cfg
     if (od.flags) CUDA_TRY(cudaMemsetAsync(od.flags, 0, sizeof(int) * m * n, st));
     if (od.est_state) CUDA_TRY(cudaMemsetAsync(od.est_state, 0xFF, sizeof(double) * m * 9 * n, st));
     if (od.est_cov) CUDA_TRY(cudaMemsetAsync(od.est_cov, 0xFF, sizeof(double) * m * 9 * n, st));
-    // FAST mode with a gravity field: one WARP per filter, the harmonic gradient split by columns over the lanes
-    // (nyxb_od_coop.cu); columns -> lanes by longest-processing-time.  nyxb_engine_set_kernel(NYXB_KERNEL_THREAD) forces the
-    // per-thread kernel.
     const int* d_cols = nullptr;
-    bool coop = eng->mode == NYXB_MODE_FAST && eng->S.has_grav && eng->S.grav.N >= 8 && eng->kernel != NYXB_KERNEL_THREAD;
-    if (coop) {
-        const int N = eng->S.grav.N, mtop = eng->S.grav.M < N ? eng->S.grav.M : N, kmax = nyxb_od_coop_kmax();
-        std::vector<int> cols(32 * (size_t)kmax, -1), cnt(32, 0);
-        std::vector<long long> load(32, 0);
-        for (int m = 0; m <= mtop && coop; ++m) {   // columns in decreasing length order: m = 0, 1 (same length), 2, ...
-            int best = 0;
-            for (int l = 1; l < 32; ++l)
-                if (load[l] < load[best] || (load[l] == load[best] && cnt[l] < cnt[best])) best = l;
-            if (cnt[best] >= kmax) { coop = false; break; }
-            cols[(size_t)best * kmax + cnt[best]++] = m;
-            load[best] += N - (m > 0 ? m : 1) + 1 + 6;   // entries + per-column overhead
-        }
-        if (coop) {
-            d_cols = B.put(cols.data(), cols.size(), st);
-            if (!d_cols) { set_err("device allocation / upload failed"); return NYXB_RC_CUDA; }
-        }
-    }
+    if (int32_t rc = od_coop_cols(eng, B, st, d_cols)) return rc;
+    const bool coop = d_cols != nullptr;
     CUDA_TRY(cudaEventRecord(eng->ev0, st));
     cudaError_t err = coop
         ? nyxb_launch_od_coop(&eng->S, &od, d_cols, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
@@ -985,6 +992,85 @@ extern "C" int32_t nyxb_od_ekf_batch(nyxb_engine* eng, const nyxb_od_config* cfg
     if (od.est_cov) CUDA_TRY(cudaMemcpyAsync(out->est_covar_diag, od.est_cov, sizeof(double) * m * 9 * n, cudaMemcpyDeviceToHost, st));
     if (out->details) CUDA_TRY(cudaMemcpyAsync(out->details, d_det, sizeof(nyxb_details) * n, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(out->status, d_status, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    float ms = 0.f;
+    if (cudaEventElapsedTime(&ms, eng->ev0, eng->ev1) == cudaSuccess) eng->last_ms = ms;
+    return NYXB_RC_OK;
+}
+
+extern "C" int32_t nyxb_od_predict_batch(nyxb_engine* eng, const nyxb_od_config* cfg, size_t n, const double* state_soa,
+                                         const double* consts_soa, const int64_t* epoch0_ns, const int64_t* end_epoch_ns,
+                                         const double* covar0_soa, const double* state_dev0_soa, const nyxb_predict_outputs* out) {
+    if (!cfg) { set_err("null argument"); return NYXB_RC_BAD_ARG; }
+    if (cfg->variant != NYXB_KF_REFERENCE_UPDATE && cfg->variant != NYXB_KF_DEVIATION_TRACKING) { set_err("bad filter variant"); return NYXB_RC_BAD_ARG; }
+    // the reference does not check max_step here: a value <= 0 would never reach the end epoch
+    if (cfg->max_step_ns <= 0) { set_err("StepSize: max_step must be positive"); return NYXB_RC_BAD_ARG; }
+    if (!eng || !state_soa || !consts_soa || !epoch0_ns || !end_epoch_ns || !covar0_soa || !out || !out->state_soa || !out->epoch_ns ||
+        !out->covar_soa || !out->status) {
+        set_err("null argument");
+        return NYXB_RC_BAD_ARG;
+    }
+    if (out->capacity < 0) { set_err("negative record capacity"); return NYXB_RC_BAD_ARG; }
+    if (!stm_supported(eng)) return NYXB_RC_UNSUPPORTED;
+    if (n == 0) return NYXB_RC_OK;
+    CUDA_TRY(cudaSetDevice(eng->device));
+    if (!eng->stream) CUDA_TRY(cudaStreamCreateWithFlags(&eng->stream, cudaStreamNonBlocking));
+    cudaStream_t st = eng->stream;
+    const size_t cap = (size_t)out->capacity;
+    DevBufs B;
+    DevOd od{};
+    od.variant = cfg->variant;
+    od.max_step_ns = cfg->max_step_ns;
+    od.snc_enabled = cfg->snc_enabled; od.snc_frame = cfg->snc_frame;
+    for (int q = 0; q < 3; ++q) od.snc_diag[q] = cfg->snc_diag[q];
+    od.snc_disable_ns = cfg->snc_disable_time_ns;
+    od.covar0 = B.put(covar0_soa, 81 * n, st);
+    od.covar = B.alloc<double>(81 * n);
+    od.state_dev = out->state_dev_soa ? B.alloc<double>(9 * n) : nullptr;
+    double* d_state = B.put(state_soa, 9 * n, st);
+    double* d_consts = B.put(consts_soa, 4 * n, st);
+    long long* d_ep = B.put((const long long*)epoch0_ns, n, st);
+    long long* d_end = B.put((const long long*)end_epoch_ns, n, st);
+    double* d_dev0 = state_dev0_soa ? B.put(state_dev0_soa, 9 * n, st) : nullptr;
+    double* d_out = B.alloc<double>(9 * n);
+    long long* d_oep = B.alloc<long long>(n);
+    nyxb_details* d_det = B.alloc<nyxb_details>(n);
+    int* d_status = B.alloc<int>(n);
+    long long* d_cnt = out->rec_count ? B.alloc<long long>(n) : nullptr;
+    OdRecords rec{ (long long)cap, nullptr, nullptr };
+    if (cap && out->rec_state) rec.state = B.alloc<double>(cap * 9 * n);
+    if (cap && out->rec_covar) rec.covar = B.alloc<double>(cap * 81 * n);
+    if (!od.covar0 || !od.covar || (out->state_dev_soa && !od.state_dev) || !d_state || !d_consts || !d_ep || !d_end ||
+        (state_dev0_soa && !d_dev0) || !d_out || !d_oep || !d_det || !d_status || (out->rec_count && !d_cnt) ||
+        (cap && out->rec_state && !rec.state) || (cap && out->rec_covar && !rec.covar)) {
+        set_err("device allocation / upload failed");
+        return NYXB_RC_CUDA;
+    }
+    // records a run does not reach read back as NaN (0xFF bytes)
+    if (rec.state) CUDA_TRY(cudaMemsetAsync(rec.state, 0xFF, sizeof(double) * cap * 9 * n, st));
+    if (rec.covar) CUDA_TRY(cudaMemsetAsync(rec.covar, 0xFF, sizeof(double) * cap * 81 * n, st));
+    const int* d_cols = nullptr;
+    if (int32_t rc = od_coop_cols(eng, B, st, d_cols)) return rc;
+    const bool coop = d_cols != nullptr;
+    CUDA_TRY(cudaEventRecord(eng->ev0, st));
+    cudaError_t err = coop
+        ? nyxb_launch_pred_coop(&eng->S, &od, d_cols, n, d_state, d_consts, d_ep, d_end, d_dev0, &rec, d_cnt, d_out, d_oep, d_det, d_status, st)
+        : (eng->mode == NYXB_MODE_STRICT)
+            ? nyxb_launch_pred_strict(&eng->S, &od, n, d_state, d_consts, d_ep, d_end, d_dev0, &rec, d_cnt, d_out, d_oep, d_det, d_status, st)
+            : nyxb_launch_pred_fast(&eng->S, &od, n, d_state, d_consts, d_ep, d_end, d_dev0, &rec, d_cnt, d_out, d_oep, d_det, d_status, st);
+    if (err != cudaSuccess) { set_err(std::string("kernel launch: ") + cudaGetErrorString(err)); return NYXB_RC_CUDA; }
+    eng->launches += 1;
+    eng->last_kernel = coop ? NYXB_KERNEL_COOP : NYXB_KERNEL_THREAD;
+    CUDA_TRY(cudaEventRecord(eng->ev1, st));
+    CUDA_TRY(cudaMemcpyAsync(out->state_soa, d_out, sizeof(double) * 9 * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(out->epoch_ns, d_oep, sizeof(long long) * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(out->covar_soa, od.covar, sizeof(double) * 81 * n, cudaMemcpyDeviceToHost, st));
+    if (od.state_dev) CUDA_TRY(cudaMemcpyAsync(out->state_dev_soa, od.state_dev, sizeof(double) * 9 * n, cudaMemcpyDeviceToHost, st));
+    if (out->details) CUDA_TRY(cudaMemcpyAsync(out->details, d_det, sizeof(nyxb_details) * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(out->status, d_status, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
+    if (d_cnt) CUDA_TRY(cudaMemcpyAsync(out->rec_count, d_cnt, sizeof(long long) * n, cudaMemcpyDeviceToHost, st));
+    if (rec.state) CUDA_TRY(cudaMemcpyAsync(out->rec_state, rec.state, sizeof(double) * cap * 9 * n, cudaMemcpyDeviceToHost, st));
+    if (rec.covar) CUDA_TRY(cudaMemcpyAsync(out->rec_covar, rec.covar, sizeof(double) * cap * 81 * n, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     float ms = 0.f;
     if (cudaEventElapsedTime(&ms, eng->ev0, eng->ev1) == cudaSuccess) eng->last_ms = ms;

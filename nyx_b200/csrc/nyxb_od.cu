@@ -28,13 +28,17 @@
 #if NYXB_STRICT
 #define NYXB_KSTM nyxb_k_stm_strict
 #define NYXB_KOD nyxb_k_od_strict
+#define NYXB_KPRED nyxb_k_pred_strict
 #define NYXB_LAUNCH_STM nyxb_launch_stm_strict
 #define NYXB_LAUNCH_OD nyxb_launch_od_strict
+#define NYXB_LAUNCH_PRED nyxb_launch_pred_strict
 #else
 #define NYXB_KSTM nyxb_k_stm_fast
 #define NYXB_KOD nyxb_k_od_fast
+#define NYXB_KPRED nyxb_k_pred_fast
 #define NYXB_LAUNCH_STM nyxb_launch_stm_fast
 #define NYXB_LAUNCH_OD nyxb_launch_od_fast
+#define NYXB_LAUNCH_PRED nyxb_launch_pred_fast
 #endif
 
 // ------------------------------------------------------------------------- per-thread backend of nyxb_od_arc.cuh
@@ -107,6 +111,17 @@ NYXB_KOD(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od, s
     od_process_arc(od, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
 }
 
+__global__ void __launch_bounds__(64)
+NYXB_KPRED(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od, size_t n, const double* __restrict__ state,
+           const double* __restrict__ consts, const long long* __restrict__ epoch0, const long long* __restrict__ end_epoch,
+           const double* __restrict__ dev0, const OdRecords rec, long long* __restrict__ rec_count, double* __restrict__ out_state,
+           long long* __restrict__ out_epoch, nyxb_details* __restrict__ out_details, int* __restrict__ out_status) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    ThreadB b(S);
+    od_predict(od, b, i, n, state, consts, epoch0, end_epoch, dev0, rec, rec_count, out_state, out_epoch, out_details, out_status);
+}
+
 extern "C" cudaError_t NYXB_LAUNCH_STM(const DevSetup* S, size_t n, const double* state, const double* consts, const long long* epoch0,
                                        long long end_epoch, long long* step_io, const double* stm_in, double* out_state,
                                        long long* out_epoch, double* out_stm, nyxb_details* out_details, int* out_status,
@@ -126,5 +141,17 @@ extern "C" cudaError_t NYXB_LAUNCH_OD(const DevSetup* S, const DevOd* od, size_t
     const int block = 32;  // few, long-running threads: spread them over as many SMs as possible
     unsigned grid = (unsigned)((n + block - 1) / block);
     NYXB_KOD<<<grid, block, 0, stream>>>(*S, *od, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
+    return cudaGetLastError();
+}
+
+extern "C" cudaError_t NYXB_LAUNCH_PRED(const DevSetup* S, const DevOd* od, size_t n, const double* state, const double* consts,
+                                        const long long* epoch0, const long long* end_epoch, const double* dev0, const OdRecords* rec,
+                                        long long* rec_count, double* out_state, long long* out_epoch, nyxb_details* out_details,
+                                        int* out_status, cudaStream_t stream) {
+    if (n == 0) return cudaSuccess;
+    const int block = 32;  // as the filter kernel
+    unsigned grid = (unsigned)((n + block - 1) / block);
+    NYXB_KPRED<<<grid, block, 0, stream>>>(*S, *od, n, state, consts, epoch0, end_epoch, dev0, *rec, rec_count, out_state, out_epoch,
+                                           out_details, out_status);
     return cudaGetLastError();
 }

@@ -38,6 +38,15 @@ struct DevOd {
     double* est_cov;               // [m][9][n]
 };
 
+// Records of a covariance prediction (KalmanODProcess::predict_until): record k holds estimate.state() (nominal + deviation, Cr
+// clamped to [0, 2]: `Spacecraft + OVector<9>`, cosmic/spacecraft.rs:713-728) at [(k*9 + r)*n + i] and the covariance, (r, c) at
+// [(k*81 + c*9 + r)*n + i].  Records k >= cap are dropped; either array may be null.
+struct OdRecords {
+    long long cap;
+    double* state;   // [cap][9][n] or null
+    double* covar;   // [cap][81][n] or null
+};
+
 extern "C" cudaError_t nyxb_launch_stm_strict(const DevSetup*, size_t, const double*, const double*, const long long*, long long,
                                               long long*, const double*, double*, long long*, double*, nyxb_details*, int*, cudaStream_t);
 extern "C" cudaError_t nyxb_launch_stm_fast(const DevSetup*, size_t, const double*, const double*, const long long*, long long,
@@ -46,3 +55,9 @@ extern "C" cudaError_t nyxb_launch_od_strict(const DevSetup*, const DevOd*, size
                                              double*, long long*, nyxb_details*, int*, cudaStream_t);
 extern "C" cudaError_t nyxb_launch_od_fast(const DevSetup*, const DevOd*, size_t, const double*, const double*, const long long*,
                                            double*, long long*, nyxb_details*, int*, cudaStream_t);
+extern "C" cudaError_t nyxb_launch_pred_strict(const DevSetup*, const DevOd*, size_t, const double*, const double*, const long long*,
+                                               const long long*, const double*, const OdRecords*, long long*, double*, long long*,
+                                               nyxb_details*, int*, cudaStream_t);
+extern "C" cudaError_t nyxb_launch_pred_fast(const DevSetup*, const DevOd*, size_t, const double*, const double*, const long long*,
+                                             const long long*, const double*, const OdRecords*, long long*, double*, long long*,
+                                             nyxb_details*, int*, cudaStream_t);

@@ -428,3 +428,65 @@ __device__ void od_process_arc(const DevOd& od, B& b, size_t i, size_t n, const 
     if (od.state_dev) for (int r = b.first(); r < 9; r += B::stride) od.state_dev[(size_t)r * n + i] = f.xdev[r];
     od_store(b, in, rc, i, n, out_state, out_epoch, out_details, out_status);
 }
+
+// ------------------------------------------------------------------------- KalmanODProcess::predict_until (od/process/mod.rs:440-486)
+// record k of run i (layout: OdRecords, nyxb_od.cuh)
+template <class B>
+__device__ __forceinline__ void od_record(const OdRecords& rec, long long k, const OdInst& in, B& b, const typename B::Filt& f, size_t i,
+                                          size_t n) {
+    if (k >= rec.cap) return;
+    if (rec.state)
+        for (int r = b.first(); r < 9; r += B::stride) {
+            double v = in.y[r] + f.xdev[r];
+            if (r == 6) v = v < 0.0 ? 0.0 : (v > 2.0 ? 2.0 : v);
+            rec.state[((size_t)k * 9 + r) * n + i] = v;
+        }
+    if (rec.covar)
+        for (int e = b.first(); e < 81; e += B::stride) {
+            const int r = e / 9, c = e - 9 * r;
+            rec.covar[((size_t)k * 81 + c * 9 + r) * n + i] = f.P[e];
+        }
+}
+
+// Maps the covariance of estimate i from epoch0[i] until end_epoch[i]: the initial estimate is record 0, then chunks of max_step, each
+// closed by a time update.  Unlike process_arc there is no set_step(max_step) (:452): the first chunk starts from the initial step, and
+// the adaptive step carries over from chunk to chunk.  The loop stops at the first chunk end at or after end_epoch, so an end at or
+// before the start still gives one chunk.  `kf.initialize_process_noises()` is not called here in the reference: it only resets the SNC
+// decay, which DevOd does not carry, so there is nothing to skip.  A propagation error ends run i with that status; the records written
+// up to then stay valid and rec_count[i] counts them.  dev0: [9][n] initial state deviation or null (zero).
+template <class B>
+__device__ void od_predict(const DevOd& od, B& b, size_t i, size_t n, const double* state, const double* consts, const long long* epoch0,
+                           const long long* end_epoch, const double* dev0, const OdRecords& rec, long long* rec_count, double* out_state,
+                           long long* out_epoch, nyxb_details* out_details, int* out_status) {
+    const DevSetup& S = b.S;
+    OdInst in;
+    od_load(S, in, i, n, state, consts, epoch0, nullptr);
+    typename B::Filt f(b);
+    for (int e = b.first(); e < 81; e += B::stride) {
+        const int r = e / 9, c = e - 9 * r;
+        f.P[e] = od.covar0[(size_t)(c * 9 + r) * n + i];
+    }
+    for (int r = b.first(); r < 9; r += B::stride) f.xdev[r] = dev0 ? dev0[(size_t)r * n + i] : 0.0;
+    od_reset_stm(b);                                          // prop.with(nominal.with_stm()) :452
+    const long long end = end_epoch[i];
+    long long prev_epoch = in.epoch_ns;
+    long long k = 0;
+    od_record(rec, k++, in, b, f, i, n);                      // push_time_update(initial_estimate) :448
+    int rc = 0;
+    for (;;) {                                                // :466-483
+        rc = od_propagate(b, in, od.max_step_ns);             // for_duration(max_step)
+        if (rc) break;
+        od_time_update(od, in, prev_epoch, b, f);
+        od_record(rec, k++, in, b, f, i, n);
+        od_reset_stm(b);
+        if (in.epoch_ns >= end) break;
+    }
+    b.sync();
+    for (int e = b.first(); e < 81; e += B::stride) {
+        const int r = e / 9, c = e - 9 * r;
+        od.covar[(size_t)(c * 9 + r) * n + i] = f.P[e];
+    }
+    if (od.state_dev) for (int r = b.first(); r < 9; r += B::stride) od.state_dev[(size_t)r * n + i] = f.xdev[r];
+    if (rec_count && b.lead()) rec_count[i] = k;
+    od_store(b, in, rc, i, n, out_state, out_epoch, out_details, out_status);
+}

@@ -8,7 +8,8 @@
 * ``SigmaRejection``           od/process/rejectcrit.rs:35-46
 * ``KfEstimate``               od/estimate/kfestimate.rs (nominal state, covariance, state deviation)
 * ``SpacecraftUncertainty``    od/estimate/sc_uncertainty.rs:36-138
-* ``KalmanODProcess``          od/process/{initializers.rs:60-113, mod.rs:128-497}; `SpacecraftKalmanOD` = MsrSize 2,
+* ``KalmanODProcess``          od/process/{initializers.rs:60-113, mod.rs:128-497}; `predict_until` / `predict_for` mod.rs:440-496;
+                               `SpacecraftKalmanOD` = MsrSize 2,
                                `SpacecraftKalmanScalarOD` = MsrSize 1 (od/mod.rs:77-91)
 
 Nothing here runs the filter: ``KalmanODProcess.process_arcs`` packs the ensemble into the SoA arrays of
@@ -295,6 +296,13 @@ class KfEstimate:
         v[6] = min(max(v[6], 0.0), 2.0)
         return self.nominal_state.with_vector(self.nominal_state.epoch(), v)
 
+    def to_random_variable(self):
+        """`KfEstimate::to_random_variable` (od/estimate/kfestimate.rs:157-160): the multivariate normal of this estimate, centred on
+        the nominal state shifted by the state deviation (what a Monte Carlo of the estimate draws from)."""
+        from .monte_carlo import MvnSpacecraft
+
+        return MvnSpacecraft.from_spacecraft_cov(self.nominal_state, self.covar, mean=self.state_deviation)
+
 
 @dataclass
 class SpacecraftUncertainty:
@@ -328,6 +336,54 @@ class SpacecraftUncertainty:
         for i in range(6, 9):
             cov[i, i] = vals[i] ** 2
         return KfEstimate.from_covar(self.nominal, cov)
+
+
+_STATE_ITEMS = ("X", "Y", "Z", "Vx", "Vy", "Vz", "Cr", "Cd", "Mass")
+_STATE_UNITS = ("km", "km", "km", "km/s", "km/s", "km/s", "unitless", "unitless", "kg")
+
+
+def _state_columns(cols, schema, est, tmpl: Spacecraft, fields=None):
+    """The state-parameter columns of the OD exports (export.rs:159-171, 385-395): est [9][k] estimated states; a parameter the
+    state cannot give is left out."""
+    import pyarrow as pa
+
+    from .param import EXPORT_PARAMS, StateError, evaluate
+
+    frame = tmpl.orbit.frame
+    for f in (EXPORT_PARAMS if fields is None else fields):
+        try:
+            vals = evaluate(f, est[:6], frame.mu_km3_s2(), tmpl, cr=est[6], cd=est[7], prop_mass_kg=est[8])
+        except StateError:
+            continue
+        cols.append(pa.array(vals, type=pa.float64()))
+        schema.append(pa.field(str(f), pa.float64(), nullable=False, metadata={"unit": f.unit, "Frame": frame.name}))
+
+
+def _sigma_columns(cols, schema, diag, frame_name: str):
+    """"Sigma <item> (<frame>) (<unit>)" from the covariance diagonal, diag [k][n_items] (export.rs:235-243, 428-435)."""
+    import pyarrow as pa
+
+    sig = np.sqrt(np.maximum(diag, 0.0))
+    for q in range(diag.shape[1]):
+        cols.append(pa.array(sig[:, q], type=pa.float64()))
+        schema.append(pa.field(f"Sigma {_STATE_ITEMS[q]} ({frame_name}) ({_STATE_UNITS[q]})", pa.float64(), nullable=False))
+
+
+def _cov_units():
+    """Units of the upper-triangle covariance entries, row by row, as export.rs:186-215 assigns them."""
+    units = []
+    for i in range(9):
+        for j in range(i, 9):
+            if i < 3:
+                u = "km^2" if j < 3 else ("km^2/s" if j < 6 else ("km*kg" if j == 8 else "km"))
+            elif i < 6:
+                u = "km^2/s^2" if j < 6 else ("km/s*kg" if j == 8 else "km/s")
+            elif i == 8 or j == 8:
+                u = "kg^2"
+            else:
+                u = "unitless"
+            units.append(u)
+    return units
 
 
 @dataclass
@@ -371,7 +427,6 @@ class ODSolution:
         import pyarrow.parquet as pq
 
         from .cosmic import epochs_to_utc_iso
-        from .param import EXPORT_PARAMS, StateError, evaluate
 
         if self.est_state is None or self.est_covar_diag is None or self.arc is None:
             raise ODError("no per-measurement estimates recorded: run process_arcs(.., record_estimates=True)")
@@ -383,19 +438,8 @@ class ODSolution:
         est = self.est_state[rows, :, index].T          # [9][k]
         cols = [pa.array(epochs_to_utc_iso(self.arc.epoch_ns[rows]), type=pa.string())]
         schema = [pa.field("Epoch (UTC)", pa.string(), nullable=False)]
-        for f in (EXPORT_PARAMS if fields is None else fields):
-            try:
-                vals = evaluate(f, est[:6], frame.mu_km3_s2(), tmpl, cr=est[6], cd=est[7], prop_mass_kg=est[8])
-            except StateError:
-                continue
-            cols.append(pa.array(vals, type=pa.float64()))
-            schema.append(pa.field(str(f), pa.float64(), nullable=False, metadata={"unit": f.unit, "Frame": frame.name}))
-        items = ("X", "Y", "Z", "Vx", "Vy", "Vz", "Cr", "Cd", "Mass")
-        units = ("km", "km", "km", "km/s", "km/s", "km/s", "unitless", "unitless", "kg")
-        sig = np.sqrt(np.maximum(self.est_covar_diag[rows, :, index], 0.0))
-        for q, (it, un) in enumerate(zip(items, units)):
-            cols.append(pa.array(sig[:, q], type=pa.float64()))
-            schema.append(pa.field(f"Sigma {it} ({frame.name}) ({un})", pa.float64(), nullable=False))
+        _state_columns(cols, schema, est, tmpl, fields)
+        _sigma_columns(cols, schema, self.est_covar_diag[rows, :, index], frame.name)
         # residual slots follow the order of the tracker's measurement types (include/nyxb.h: nyxb_od_outputs)
         slot_type = np.full((len(rows), 2), -1)
         for a, r in enumerate(rows):
@@ -418,6 +462,108 @@ class ODSolution:
         schema.append(pa.field("Residual Rejected", pa.bool_(), nullable=True))
         cols.append(pa.array([self.arc.tracker[r] for r in rows], type=pa.string()))
         schema.append(pa.field("Tracker", pa.string(), nullable=True))
+        meta = {"Purpose": "Orbit determination results"}
+        meta.update(metadata or {})
+        pq.write_table(pa.Table.from_arrays(cols, schema=pa.schema(schema, metadata=meta)), str(path))
+        return path
+
+
+@dataclass
+class PredictionSolution:
+    """Results of n covariance predictions (`KalmanODProcess::predict_until`, od/process/mod.rs:440-486): the final estimates and
+    the records of the time updates.  Record k of run i sits at epoch0_ns[i] + k * max_step_ns; record 0 is the initial estimate.
+    rec_count[i] records were produced; the first min(rec_count[i], capacity) are stored."""
+
+    final_state_soa: np.ndarray          # [9][n] nominal state
+    final_epoch_ns: np.ndarray           # [n]
+    covar: np.ndarray                    # [n][9][9]
+    state_deviation: np.ndarray          # [9][n]
+    details: np.ndarray
+    status: np.ndarray
+    rec_count: np.ndarray                # [n]
+    rec_state: Optional[np.ndarray]      # [K][9][n] estimate.state() (nominal + deviation)
+    rec_covar: Optional[np.ndarray]      # [K][81][n], (r, c) at [k][c*9 + r][i]
+    epoch0_ns: np.ndarray                # [n]
+    max_step_ns: int
+    templates: Sequence[Spacecraft] = ()
+
+    @property
+    def capacity(self) -> int:
+        for a in (self.rec_state, self.rec_covar):
+            if a is not None:
+                return a.shape[0]
+        return 0
+
+    def stored(self, i: int) -> int:
+        return int(min(self.rec_count[i], self.capacity))
+
+    def record_epochs(self, i: int) -> np.ndarray:
+        """Epochs of the stored records of run i."""
+        return self.epoch0_ns[i] + np.arange(self.stored(i), dtype=np.int64) * self.max_step_ns
+
+    def record_covar(self, k: int, i: int) -> np.ndarray:
+        return self.rec_covar[k, :, i].reshape(9, 9).T.copy()
+
+    def final_estimate(self, i: int) -> KfEstimate:
+        sc = self.templates[i].with_vector(int(self.final_epoch_ns[i]), self.final_state_soa[:, i])
+        return KfEstimate(sc, self.covar[i].copy(), self.state_deviation[:, i].copy())
+
+    def to_parquet(self, path, index: int = 0, fields=None, metadata: Optional[dict] = None, msr_size: int = 2):
+        """`ODSolution::to_parquet` (od/process/solution/export.rs:60-470) of the solution `predict_until` returns, which has no
+        measurement types, for run `index`: "Epoch (UTC)", the state parameters of estimate.state() (default
+        `Spacecraft::export_params`), the 45 "Covariance <a>*<b> (<frame>) (<unit>)" entries, "Sigma <item> (<frame>) (<unit>)",
+        "Sigma <item> (RIC) (<unit>)", then the residual, gain and filter-smoother columns, all null.  The RIC sigmas follow the
+        as-coded product D C D^T with D = the RIC->inertial state DCM of estimate.state() (export.rs:430-446), its rate block taken
+        as zero (as SpacecraftUncertainty).  The per-element sigma columns of orbital-element parameters are not written."""
+        import pyarrow as pa
+        import pyarrow.parquet as pq
+
+        from .cosmic import epochs_to_utc_iso
+
+        if self.rec_state is None or self.rec_covar is None:
+            raise ODError("records of both states and covariances are needed: predict with a record capacity")
+        k = self.stored(index)
+        if k == 0:
+            raise ODError("TooFewMeasurements: need 1 estimate to export")
+        tmpl = self.templates[index]
+        frame = tmpl.orbit.frame
+        est = self.rec_state[:k, :, index].T                                   # [9][k]
+        cov = self.rec_covar[:k, :, index].reshape(k, 9, 9).transpose(0, 2, 1)   # [k][r][c]
+        cols = [pa.array(epochs_to_utc_iso(self.record_epochs(index)), type=pa.string())]
+        schema = [pa.field("Epoch (UTC)", pa.string(), nullable=False)]
+        _state_columns(cols, schema, est, tmpl, fields)
+        units = _cov_units()
+        q = 0
+        for a in range(9):
+            for b in range(a, 9):
+                cols.append(pa.array(cov[:, a, b], type=pa.float64()))
+                schema.append(pa.field(f"Covariance {_STATE_ITEMS[a]}*{_STATE_ITEMS[b]} ({frame.name}) ({units[q]})", pa.float64(),
+                                       nullable=False))
+                q += 1
+        _sigma_columns(cols, schema, np.diagonal(cov, axis1=1, axis2=2), frame.name)
+        ric = np.empty((k, 6))
+        for j in range(k):
+            d3 = dcm_ric_to_inertial(Orbit(*[float(v) for v in est[:6, j]], 0, frame))
+            d6 = np.zeros((6, 6))
+            d6[:3, :3] = d3
+            d6[3:, 3:] = d3
+            ric[j] = np.diag(d6 @ cov[j, :6, :6] @ d6.T)
+        _sigma_columns(cols, schema, ric, "RIC")
+
+        def nulls(name, typ):
+            cols.append(pa.nulls(k, type=typ))
+            schema.append(pa.field(name, typ, nullable=True))
+
+        for j in range(msr_size):
+            nulls(f"Whitened residual #{j}", pa.float64())
+        nulls("Residual ratio", pa.float64())
+        nulls("Residual Rejected", pa.bool_())
+        nulls("Tracker", pa.string())
+        for it in _STATE_ITEMS:                          # no measurement types: len 0 != MsrSize::DIM (export.rs:302-331)
+            for j in range(msr_size):
+                nulls(f"Gain {it}*[{j}]", pa.float64())
+        for a in range(9):                               # as coded: the first nine covariance units (export.rs:333-343)
+            nulls(f"Filter-smoother ratio {_STATE_ITEMS[a]} ({units[a]})", pa.float64())
         meta = {"Purpose": "Orbit determination results"}
         meta.update(metadata or {})
         pq.write_table(pa.Table.from_arrays(cols, schema=pa.schema(schema, metadata=meta)), str(path))
@@ -499,6 +645,49 @@ class KalmanODProcess:
 
     def process_arc(self, initial_estimate: KfEstimate, arc: TrackingDataArc) -> ODSolution:
         return self.process_arcs([initial_estimate], arc)
+
+    # ---- covariance mapping (od/process/mod.rs:440-496)
+    def predict_ensemble_until(self, estimates: Sequence[KfEstimate], end_epoch, capacity: Optional[int] = None,
+                               record_states: bool = True, record_covars: bool = True) -> PredictionSolution:
+        """n independent `predict_until(estimate_i, end_epoch_i)` runs in one launch; `end_epoch` is one epoch (ns) or one per
+        estimate.  Each run starts from its estimate's nominal state, covariance and state deviation (so a CKF
+        `ODSolution.final_estimate(i)` is predicted onward with its deviation).  `capacity` records are kept per run (default: as many
+        as the longest run produces; 0 keeps the final estimates only)."""
+        from .cosmic import pack_spacecraft
+
+        n = len(estimates)
+        if n == 0:
+            raise ODError("no estimate to predict")
+        cfg = self.config_c()
+        frame = estimates[0].nominal_state.orbit.frame
+        st, cs, ep = pack_spacecraft(e.nominal_state for e in estimates)
+        end = np.ascontiguousarray(np.broadcast_to(np.asarray(end_epoch, dtype=np.int64), (n,)))
+        if capacity is None:
+            span = np.maximum(end - ep, 1)
+            capacity = int(1 + ((span + cfg.max_step_ns - 1) // cfg.max_step_ns).max())
+        cov0 = np.empty((81, n))
+        dev0 = np.empty((9, n))
+        for i, e in enumerate(estimates):
+            cov0[:, i] = np.asarray(e.covar, dtype=np.float64).reshape(9, 9).T.reshape(81)  # (c*9 + r)
+            dev0[:, i] = np.asarray(e.state_deviation, dtype=np.float64)
+        eng = self.prop.engine(frame, self.almanac)
+        res = eng.od_predict_batch(cfg, st, cs, ep, end, cov0, dev0, capacity=capacity, record_states=record_states,
+                                   record_covars=record_covars)
+        res.templates = [e.nominal_state for e in estimates]
+        return res
+
+    def predict_ensemble_for(self, estimates: Sequence[KfEstimate], duration: int, **kw) -> PredictionSolution:
+        """`predict_ensemble_until` with end_i = epoch0_i + duration."""
+        end = np.array([e.nominal_state.epoch() for e in estimates], dtype=np.int64) + int(duration)
+        return self.predict_ensemble_until(estimates, end, **kw)
+
+    def predict_until(self, initial_estimate: KfEstimate, end_epoch: int, **kw) -> PredictionSolution:
+        """`KalmanODProcess::predict_until` (od/process/mod.rs:440-486)."""
+        return self.predict_ensemble_until([initial_estimate], int(end_epoch), **kw)
+
+    def predict_for(self, initial_estimate: KfEstimate, duration: int, **kw) -> PredictionSolution:
+        """`KalmanODProcess::predict_for` (od/process/mod.rs:489-496)."""
+        return self.predict_ensemble_for([initial_estimate], duration, **kw)
 
 
 def SpacecraftKalmanOD(prop, kf_variant, sigma_reject, devices, almanac) -> KalmanODProcess:

@@ -377,6 +377,45 @@ class Engine:
         covar = np.ascontiguousarray(out_cov.T.reshape(n, 9, 9).transpose(0, 2, 1))  # (c*9+r) -> [i][r][c]
         return ODSolution(out_state, out_epoch, covar, out_dev, ratio, prefit, postfit, flags, est_state, est_cov, details, status)
 
+    def od_predict_batch(self, cfg_c, state_soa, consts_soa, epoch0_ns, end_epoch_ns, covar0_soa, state_dev0_soa=None,
+                         capacity: int = 0, record_states: bool = True, record_covars: bool = True):
+        """`nyxb_od_predict_batch`: n covariance predictions (`KalmanODProcess::predict_until`, od/process/mod.rs:440-486) in ONE
+        launch.  Records 0 .. capacity-1 of each run are kept; `record_states` / `record_covars` = False skip an array."""
+        from .od import PredictionSolution
+
+        state_soa = np.ascontiguousarray(state_soa, dtype=np.float64)
+        consts_soa = np.ascontiguousarray(consts_soa, dtype=np.float64)
+        epoch0_ns = np.ascontiguousarray(epoch0_ns, dtype=np.int64)
+        end_epoch_ns = np.ascontiguousarray(end_epoch_ns, dtype=np.int64)
+        covar0_soa = np.ascontiguousarray(covar0_soa, dtype=np.float64)
+        n = state_soa.shape[1]
+        if state_soa.shape != (9, n) or consts_soa.shape != (4, n) or epoch0_ns.shape != (n,) or end_epoch_ns.shape != (n,) \
+                or covar0_soa.shape != (81, n):
+            raise ValueError("expected state[9][n], consts[4][n], epoch0[n], end_epoch[n], covar0[81][n]")
+        if state_dev0_soa is not None:
+            state_dev0_soa = np.ascontiguousarray(state_dev0_soa, dtype=np.float64)
+            if state_dev0_soa.shape != (9, n):
+                raise ValueError("expected state_dev0[9][n]")
+        cap = int(capacity)
+        out_state = np.empty((9, n)); out_epoch = np.empty(n, dtype=np.int64); out_cov = np.empty((81, n)); out_dev = np.empty((9, n))
+        details = np.zeros(n, dtype=abi.DETAILS_DTYPE)
+        status = np.zeros(n, dtype=np.int32)
+        count = np.zeros(n, dtype=np.int64)
+        rec_state = np.empty((cap, 9, n)) if cap and record_states else None
+        rec_covar = np.empty((cap, 81, n)) if cap and record_covars else None
+        out = abi.PredictOutputsC(out_state.ctypes.data, out_epoch.ctypes.data, out_cov.ctypes.data, out_dev.ctypes.data,
+                                  details.ctypes.data, status.ctypes.data, cap,
+                                  rec_state.ctypes.data if rec_state is not None else None,
+                                  rec_covar.ctypes.data if rec_covar is not None else None, count.ctypes.data)
+        rc = self._lib.nyxb_od_predict_batch(self._h, C.byref(cfg_c), n, state_soa.ctypes.data, consts_soa.ctypes.data,
+                                             epoch0_ns.ctypes.data, end_epoch_ns.ctypes.data, covar0_soa.ctypes.data,
+                                             state_dev0_soa.ctypes.data if state_dev0_soa is not None else None, C.byref(out))
+        if rc != 0:
+            raise PropagationError(f"nyxb_od_predict_batch rc={rc}: {abi.last_error()}")
+        covar = np.ascontiguousarray(out_cov.T.reshape(n, 9, 9).transpose(0, 2, 1))  # (c*9+r) -> [i][r][c]
+        return PredictionSolution(out_state, out_epoch, covar, out_dev, details, status, count, rec_state, rec_covar, epoch0_ns.copy(),
+                                  int(cfg_c.max_step_ns))
+
     def propagate_batch_dev(self, n, state_ptr, consts_ptr, epoch0_ptr, end_epoch_ns, step_ptr, out_state_ptr,
                             out_epoch_ptr, details_ptr, status_ptr, stream_ptr=None):
         """Device-pointer call (`nyxb_propagate_batch_dev`): asynchronous on `stream_ptr`."""
