@@ -36,7 +36,8 @@ extern "C" {
 
 #define NYXB_ABI_VERSION 4 /* 4: nyxb_engine_set_kernel / nyxb_engine_last_kernel / nyxb_engine_set_tx_tuning, nyxb_tx_table_dump, nyxb_propagate_batch_multi, nyxb_reference_normals;
                               nyxb_integ_opts.state_center, nyxb_gravity_field.body, nyxb_dynamics.n_gravity / n_point_masses / point_mass_order; nyxb_od_predict_batch
-                              and nyxb_predict_outputs were added later without a bump (a pure addition: no existing type or entry point changed).  Earlier: 2: nyxb_srp gained `estimate`; STM, filter and dispersion entry points.  3: nyxb_traj_resample[_dev], nyxb_event_locate[_dev] */
+                              and nyxb_predict_outputs, then nyxb_od_bls_batch, nyxb_od_bls_evaluate_batch, nyxb_bls_config, nyxb_bls_outputs and
+                              the status codes 6-8 were added later without a bump (a pure addition: no existing type or entry point changed).  Earlier: 2: nyxb_srp gained `estimate`; STM, filter and dispersion entry points.  3: nyxb_traj_resample[_dev], nyxb_event_locate[_dev] */
 
 /* ---- IntegratorMethod — propagators/rk_methods/mod.rs:65-79 (same order) ---- */
 enum nyxb_method {
@@ -200,6 +201,9 @@ enum nyxb_status {
     NYXB_ERR_MASSLESS = 3,       /* DynamicsError::MasslessSpacecraft      spacecraft.rs:201-203 */
     NYXB_ERR_EPHEMERIS = 4,      /* almanac error: epoch outside ephemeris coverage */
     NYXB_ERR_EVENT_NOT_FOUND = 5,/* PropagationError::NthEventError: end epoch reached first (event.rs:177-182) */
+    NYXB_ERR_TOO_FEW_MEASUREMENTS = 6, /* ODError::TooFewMeasurements (blse/mod.rs:155-161) */
+    NYXB_ERR_SINGULAR_INFORMATION = 7, /* ODError::SingularInformationMatrix (blse/mod.rs:312-315) */
+    NYXB_ERR_INVALID_MEASUREMENT = 8,  /* ODError::InvalidMeasurement: an observation that is not finite (blse/mod.rs:266-272) */
     NYXB_WARN_MAX_ATTEMPTS = 0x100 /* OR-ed flag: instance.rs:440-445 (warn only) */
 };
 
@@ -501,6 +505,67 @@ int32_t nyxb_od_predict_batch(nyxb_engine* eng, const nyxb_od_config* cfg, size_
                               const int64_t* end_epoch_ns, const double* covar0_soa, const double* state_dev0_soa,
                               const nyxb_predict_outputs* out);
 
+/* ---- Batch least squares over an ensemble: n independent `BatchLeastSquares::estimate` runs (od/blse/mod.rs:146-446) in ONE kernel
+ * launch.  The n problems share the schedule and the stations; each has its own initial guess, epoch and observation set (arc->obs,
+ * both NaN: the measurement is not in problem i's arc, as `rejected`).  Per iteration, as coded: a new STM propagation from the current
+ * estimate at opts.init_step (no set_step(max_step)); the information matrix starts at the IDENTITY; the walk to each measurement takes
+ * chunks of min(time left, current step, max_step); after each chunk stm_acc = Phi(t, t0) * stm_acc, where the STM is never reset inside
+ * the iteration, so stm_acc is a product of cumulative STMs; each measurement type is its own scalar residual in the station's type
+ * order, computed without bias (measure_instantaneous(state, None)), skipped when not visible; rms = sqrt(sum W dy^2 / count) where count
+ * is every measurement present in problem i (invisible, unknown-tracker and at-or-before-epoch ones included).  A measurement type the
+ * station does not carry is skipped.
+ * Per-problem failures are statuses and never abort the batch: NYXB_ERR_TOO_FEW_MEASUREMENTS (count < 2), NYXB_ERR_INVALID_MEASUREMENT,
+ * NYXB_ERR_SINGULAR_INFORMATION (normal equations only), or a propagation status.
+ * Earlier or stricter than the reference (NYXB_RC_BAD_ARG for the whole call): max_step_ns <= 0 (the reference would loop forever),
+ * max_iterations < 0 (a usize there), a station noise variance <= 0 (the reference fails with SingularNoiseRk at the first measurement
+ * of that station), and, for Levenberg-Marquardt, a lambda setting <= 0 (unchecked there).  The setups nyxb_propagate_batch_stm rejects
+ * return NYXB_RC_UNSUPPORTED.  Kernel family as nyxb_od_ekf_batch. */
+enum nyxb_bls_solver { NYXB_BLS_NORMAL_EQUATIONS = 0, NYXB_BLS_LEVENBERG_MARQUARDT = 1 };  /* od/blse/mod.rs BLSSolver */
+
+typedef struct {
+    int32_t solver;              /* enum nyxb_bls_solver; default NORMAL_EQUATIONS */
+    int32_t max_iterations;      /* default 10 */
+    double tolerance_pos_km;     /* convergence: |dx[0..3]| below this; default 1e-4 */
+    int64_t max_step_ns;         /* default 30 s */
+    int64_t epoch_precision_ns;  /* default 1 us */
+    double lm_lambda_init;       /* default 10 */
+    double lm_lambda_decrease;   /* default 10 */
+    double lm_lambda_increase;   /* default 10 */
+    double lm_lambda_min;        /* default 1e-12 */
+    double lm_lambda_max;        /* default 1e12 */
+    int32_t lm_use_diag_scaling; /* default 1 */
+    int32_t _pad;
+} nyxb_bls_config;
+
+typedef struct {
+    double* state_soa;           /* [9][n] estimated state (the last accepted correction applied; Cr clamped), or NULL */
+    int64_t* epoch_ns;           /* [n] its epoch (the guess epoch), or NULL */
+    double* covar_soa;           /* [81][n] (r,c) at [(c*9+r)*n + i], or NULL: the inverse of the information matrix of the last
+                                    accepted iteration (UDU^T), I when that factorisation fails, zeros when no iteration was accepted */
+    int32_t* iterations;         /* [n] or NULL */
+    double* final_rms;           /* [n] or NULL: the RMS at the last accepted linearisation point; DBL_MAX when none */
+    double* final_corr_pos_km;   /* [n] or NULL: DBL_MAX after a rejected Levenberg-Marquardt step or when none ran */
+    int32_t* converged;          /* [n] or NULL: 0 / 1 */
+    nyxb_details* details;       /* [n] or NULL: steps / RHS evaluations over all iterations */
+    int32_t* status;             /* [n] */
+} nyxb_bls_outputs;
+
+/* state_soa/consts_soa/epoch0_ns as in nyxb_od_ekf_batch (the initial guesses); HOST pointers everywhere. */
+int32_t nyxb_od_bls_batch(nyxb_engine* eng, const nyxb_bls_config* cfg,
+                          int32_t n_stations, const nyxb_ground_station* stations,
+                          const nyxb_tracking_arc* arc, size_t n,
+                          const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
+                          const nyxb_bls_outputs* out);
+
+/* `BatchLeastSquares::evaluate` (od/blse/mod.rs:450-541): the RMS of each state over the arc, the same pass without the STM product;
+ * NYXB_ERR_TOO_FEW_MEASUREMENTS when problem i has no measurement.  rms [n] may be NULL; status [n] is required.  Of cfg only
+ * max_step_ns and epoch_precision_ns are read. */
+int32_t nyxb_od_bls_evaluate_batch(nyxb_engine* eng, const nyxb_bls_config* cfg,
+                                   int32_t n_stations, const nyxb_ground_station* stations,
+                                   const nyxb_tracking_arc* arc, size_t n,
+                                   const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
+                                   double* rms, int32_t* status);
+
 /* ---- On-device Monte Carlo dispersions (next row (f)-4): `MvnSpacecraft::sample` (mc/multivariate.rs:298-331) for the
  * runs [first_index, first_index + n): state_i = template + (sqrt_s_v * z_i + mean), z_i ~ N(0, I_9) drawn from a
  * counter-based stream keyed by (seed, run index) — Philox4x32-10 + Box-Muller, see nyx_b200/csrc/nyxb_mvn.cu — so that a
@@ -535,8 +600,8 @@ int32_t nyxb_ziggurat_tables(double* x257, double* f257);                       
 enum nyxb_kernel { NYXB_KERNEL_AUTO = 0, NYXB_KERNEL_THREAD = 1, NYXB_KERNEL_COOP = 2, NYXB_KERNEL_TRANSPOSED = 3 };
 int32_t nyxb_engine_set_kernel(nyxb_engine* eng, int32_t kernel);          /* enum nyxb_kernel; NYXB_RC_UNSUPPORTED if the setup cannot use it */
 int32_t nyxb_engine_last_kernel(const nyxb_engine* eng);                   /* family used by the last propagation launch */
-/* nyxb_propagate_batch_stm sets it to THREAD (one thread per trajectory, STRICT and FAST).  nyxb_od_ekf_batch and
- * nyxb_od_predict_batch set it to COOP when they ran the warp-cooperative kernel (FAST, field of degree >= 8, kernel not forced to
+/* nyxb_propagate_batch_stm sets it to THREAD (one thread per trajectory, STRICT and FAST).  nyxb_od_ekf_batch,
+ * nyxb_od_predict_batch, nyxb_od_bls_batch and nyxb_od_bls_evaluate_batch set it to COOP when they ran the warp-cooperative kernel (FAST, field of degree >= 8, kernel not forced to
  * THREAD), else to THREAD. */
 /* TRANSPOSED kernel: step attempts per time slice (default 64) and an upper bound on the persistent CTAs (0 = SMs x occupancy).
  * Sets are only parked when there are more sets than CTAs. */

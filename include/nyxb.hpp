@@ -508,6 +508,30 @@ struct PredictionSolution {
     double record_covar(int64_t k, int r, int c) const { return rec_covar[(size_t)k * 81 + c * 9 + r]; }
 };
 
+namespace detail {
+// the devices as nyxb_ground_station, in order; a station on another body than the integration centre needs its ephemeris
+inline std::vector<nyxb_ground_station> pack_stations(const std::vector<GroundStation>& devices, const Frame& frame, const Almanac* almanac) {
+    std::vector<nyxb_ground_station> st;
+    for (auto& d : devices) {
+        int32_t bi = NYXB_CENTRAL_BODY;
+        if (d.frame.ephemeris_id != frame.ephemeris_id) {
+            if (!almanac) throw std::runtime_error("an almanac with the station's body is needed");
+            bi = -2;
+            for (size_t j = 0; j < almanac->bodies.size(); ++j) if (almanac->bodies[j].ephemeris_id == d.frame.ephemeris_id) bi = (int32_t)j;
+            if (bi == -2) throw std::runtime_error("no ephemeris loaded for the station's body");
+        }
+        st.push_back(d.to_c(frame, bi, frame.mean_equatorial_radius_km));
+    }
+    return st;
+}
+// index of each measurement's tracker in `devices`; -1 for an unknown tracker
+inline std::vector<int32_t> tracker_index(const std::vector<GroundStation>& devices, const TrackingDataArc& arc) {
+    std::vector<int32_t> trk(arc.epoch_ns.size());
+    for (size_t k = 0; k < trk.size(); ++k) { trk[k] = -1; for (size_t j = 0; j < devices.size(); ++j) if (devices[j].name == arc.tracker[k]) trk[k] = (int32_t)j; }
+    return trk;
+}
+}  // namespace detail
+
 // KalmanODProcess (od/process/{initializers.rs:60-113, mod.rs:128-497}); msr_size 2 = SpacecraftKalmanOD, 1 = SpacecraftKalmanScalarOD
 class KalmanODProcess {
   public:
@@ -560,19 +584,8 @@ class KalmanODProcess {
         detail::Soa soa(noms);
         std::vector<double> cov0(81 * n);
         for (size_t i = 0; i < n; ++i) for (int r = 0; r < 9; ++r) for (int c = 0; c < 9; ++c) cov0[(size_t)(c * 9 + r) * n + i] = initial[i].covar[r * 9 + c];
-        std::vector<nyxb_ground_station> st;
-        for (auto& d : devices) {
-            int32_t bi = NYXB_CENTRAL_BODY;
-            if (d.frame.ephemeris_id != frame.ephemeris_id) {
-                if (!almanac) throw std::runtime_error("an almanac with the station's body is needed");
-                bi = -2;
-                for (size_t j = 0; j < almanac->bodies.size(); ++j) if (almanac->bodies[j].ephemeris_id == d.frame.ephemeris_id) bi = (int32_t)j;
-                if (bi == -2) throw std::runtime_error("no ephemeris loaded for the station's body");
-            }
-            st.push_back(d.to_c(frame, bi, frame.mean_equatorial_radius_km));
-        }
-        std::vector<int32_t> trk(m);
-        for (size_t k = 0; k < m; ++k) { trk[k] = -1; for (size_t j = 0; j < devices.size(); ++j) if (devices[j].name == arc.tracker[k]) trk[k] = (int32_t)j; }
+        std::vector<nyxb_ground_station> st = detail::pack_stations(devices, frame, almanac);
+        std::vector<int32_t> trk = detail::tracker_index(devices, arc);
         const nyxb_od_config cfg = config();
         nyxb_tracking_arc carc{(int64_t)m, arc.epoch_ns.data(), trk.data(), arc.obs.data()};
         ODSolution s; s.n = n; s.m = m;
@@ -583,6 +596,92 @@ class KalmanODProcess {
         if (nyxb_od_ekf_batch(eng.get(), &cfg, (int32_t)st.size(), st.data(), &carc, n, soa.state.data(), soa.consts.data(), soa.epoch.data(), cov0.data(), &out) != NYXB_RC_OK)
             throw std::runtime_error(std::string("nyxb_od_ekf_batch: ") + nyxb_last_error());
         return s;
+    }
+};
+
+// BatchLeastSquares (od/blse/mod.rs:30-541) with the reference's builder defaults; estimate / evaluate of one problem through
+// nyxb_od_bls_batch / nyxb_od_bls_evaluate_batch.  A per-problem status is thrown as the reference's ODError.
+enum class BLSSolver : int32_t { NormalEquations = NYXB_BLS_NORMAL_EQUATIONS, LevenbergMarquardt = NYXB_BLS_LEVENBERG_MARQUARDT };
+
+struct BLSSolution {   // od/blse/solution.rs
+    Spacecraft estimated_state; double covariance[81] = {0};   // row-major
+    int32_t num_iterations = 0; double final_rms = 0.0, final_corr_pos_km = 0.0; bool converged = false;
+    nyxb_details details{};
+    // From<BLSSolution> for KfEstimate (solution.rs:75-93): the Cr, Cd and mass variances zeroed
+    KfEstimate to_kf_estimate() const {
+        KfEstimate e; e.nominal_state = estimated_state;
+        for (int q = 0; q < 81; ++q) e.covar[q] = covariance[q];
+        e.covar[60] = e.covar[70] = e.covar[80] = 0.0;
+        return e;
+    }
+};
+
+class BatchLeastSquares {
+  public:
+    Propagator prop; std::vector<GroundStation> devices; const Almanac* almanac = nullptr;
+    BLSSolver solver = BLSSolver::NormalEquations;
+    double tolerance_pos_km = 1e-4; int32_t max_iterations = 10;
+    int64_t max_step = 30 * NS_PER_S, epoch_precision = 1000;
+    double lm_lambda_init = 10.0, lm_lambda_decrease = 10.0, lm_lambda_increase = 10.0, lm_lambda_min = 1e-12, lm_lambda_max = 1e12;
+    bool lm_use_diag_scaling = true;
+    BatchLeastSquares(Propagator p, std::vector<GroundStation> dev, const Almanac* alm = nullptr) : prop(std::move(p)), devices(std::move(dev)), almanac(alm) {}
+
+    nyxb_bls_config config() const {
+        nyxb_bls_config c{};
+        c.solver = (int32_t)solver; c.max_iterations = max_iterations; c.tolerance_pos_km = tolerance_pos_km;
+        c.max_step_ns = max_step; c.epoch_precision_ns = epoch_precision;
+        c.lm_lambda_init = lm_lambda_init; c.lm_lambda_decrease = lm_lambda_decrease; c.lm_lambda_increase = lm_lambda_increase;
+        c.lm_lambda_min = lm_lambda_min; c.lm_lambda_max = lm_lambda_max; c.lm_use_diag_scaling = lm_use_diag_scaling ? 1 : 0;
+        return c;
+    }
+
+    // BatchLeastSquares::estimate (od/blse/mod.rs:146-446); arc with one observation set
+    BLSSolution estimate(const Spacecraft& guess, const TrackingDataArc& arc) const {
+        Ctx c(*this, guess, arc);
+        BLSSolution s; s.estimated_state = guess;
+        double state[9], cov[81], rms = 0.0, corr = 0.0; int64_t epoch = 0; int32_t iters = 0, conv = 0, status = 0;
+        nyxb_bls_outputs out{state, &epoch, cov, &iters, &rms, &corr, &conv, &s.details, &status};
+        if (nyxb_od_bls_batch(c.eng.get(), &c.cfg, (int32_t)c.st.size(), c.st.data(), &c.carc, 1, c.soa.state.data(), c.soa.consts.data(),
+                              c.soa.epoch.data(), &out) != NYXB_RC_OK)
+            throw std::runtime_error(std::string("nyxb_od_bls_batch: ") + nyxb_last_error());
+        throw_status(status);
+        s.estimated_state = detail::unpack(guess, std::vector<double>(state, state + 9), std::vector<int64_t>{epoch}, 1, 0);
+        for (int r = 0; r < 9; ++r) for (int q = 0; q < 9; ++q) s.covariance[r * 9 + q] = cov[q * 9 + r];
+        s.num_iterations = iters; s.final_rms = rms; s.final_corr_pos_km = corr; s.converged = conv != 0;
+        return s;
+    }
+
+    // BatchLeastSquares::evaluate (od/blse/mod.rs:450-541)
+    double evaluate(const Spacecraft& state, const TrackingDataArc& arc) const {
+        Ctx c(*this, state, arc);
+        double rms = 0.0; int32_t status = 0;
+        if (nyxb_od_bls_evaluate_batch(c.eng.get(), &c.cfg, (int32_t)c.st.size(), c.st.data(), &c.carc, 1, c.soa.state.data(), c.soa.consts.data(),
+                                       c.soa.epoch.data(), &rms, &status) != NYXB_RC_OK)
+            throw std::runtime_error(std::string("nyxb_od_bls_evaluate_batch: ") + nyxb_last_error());
+        throw_status(status);
+        return rms;
+    }
+
+  private:
+    struct Ctx {
+        detail::Soa soa; detail::EnginePtr eng;
+        std::vector<nyxb_ground_station> st; std::vector<int32_t> trk; nyxb_bls_config cfg; nyxb_tracking_arc carc;
+        Ctx(const BatchLeastSquares& b, const Spacecraft& s, const TrackingDataArc& arc)
+            : soa(std::vector<Spacecraft>{s}), eng(detail::make_engine(b.prop.dynamics, s.frame, b.almanac, b.prop.method, b.prop.opts, b.prop.mode, b.prop.device)),
+              st(detail::pack_stations(b.devices, s.frame, b.almanac)), trk(detail::tracker_index(b.devices, arc)), cfg(b.config()) {
+            const size_t m = arc.epoch_ns.size();
+            if (arc.n != 1 || arc.obs.size() != m * 2 || arc.tracker.size() != m) throw std::runtime_error("arc shape: one observation set expected");
+            carc = nyxb_tracking_arc{(int64_t)m, arc.epoch_ns.data(), trk.data(), arc.obs.data()};
+        }
+    };
+    static void throw_status(int32_t status) {
+        switch (status & 0xFF) {
+            case 0: return;
+            case NYXB_ERR_TOO_FEW_MEASUREMENTS: throw std::runtime_error("TooFewMeasurements");
+            case NYXB_ERR_SINGULAR_INFORMATION: throw std::runtime_error("SingularInformationMatrix");
+            case NYXB_ERR_INVALID_MEASUREMENT: throw std::runtime_error("InvalidMeasurement");
+            default: throw std::runtime_error("ODPropError: status " + std::to_string(status & 0xFF));
+        }
     }
 };
 

@@ -19,7 +19,7 @@ from .trajectory import Traj, TrajError, hermite_eval
 from . import dhall
 from .config import PropagatorConfig, integrator_options_from, load_ground_stations, parse_duration
 from .event import Event, brent, locate_event
-from .od import (GroundStation, KalmanODProcess, KalmanVariant, KfEstimate, LocalFrame, MeasurementType, ODError, ODSolution,
+from .od import (BatchLeastSquares, BLSEnsembleSolution, BLSSolution, BLSSolver, GroundStation, KalmanODProcess, KalmanVariant, KfEstimate, LocalFrame, MeasurementType, ODError, ODSolution,
                  PredictionSolution, ProcessNoise3D, SigmaRejection, SpacecraftKalmanOD, SpacecraftKalmanScalarOD, SpacecraftUncertainty,
                  StochasticNoise, TrackingDataArc, simulate_tracking, station_state)
 from .propagator import (Engine, ErrorControl, IntegrationDetails, IntegratorMethod, IntegratorOptions, PropagationError,

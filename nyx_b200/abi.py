@@ -160,10 +160,12 @@ class EventC(C.Structure):
 
 
 # ---- orbit determination (SURVEY.md §8 (f)-2): mirrors of nyxb_ground_station / nyxb_od_config / nyxb_tracking_arc / nyxb_od_outputs /
-# nyxb_predict_outputs
+# nyxb_predict_outputs / nyxb_bls_config / nyxb_bls_outputs
 MSR_RANGE, MSR_DOPPLER = 0, 1
 KF_REFERENCE_UPDATE, KF_DEVIATION_TRACKING = 0, 1
 MSRF_PROCESSED, MSRF_REJECTED, MSRF_NOT_VISIBLE, MSRF_ABSENT = 1, 2, 4, 8
+BLS_NORMAL_EQUATIONS, BLS_LEVENBERG_MARQUARDT = 0, 1
+ERR_TOO_FEW_MEASUREMENTS, ERR_SINGULAR_INFORMATION, ERR_INVALID_MEASUREMENT = 6, 7, 8
 
 
 class GroundStationC(C.Structure):
@@ -234,6 +236,37 @@ class PredictOutputsC(C.Structure):
         ("rec_state", C.c_void_p),
         ("rec_covar", C.c_void_p),
         ("rec_count", C.c_void_p),
+    ]
+
+
+class BlsConfigC(C.Structure):
+    _fields_ = [
+        ("solver", C.c_int32),
+        ("max_iterations", C.c_int32),
+        ("tolerance_pos_km", C.c_double),
+        ("max_step_ns", C.c_int64),
+        ("epoch_precision_ns", C.c_int64),
+        ("lm_lambda_init", C.c_double),
+        ("lm_lambda_decrease", C.c_double),
+        ("lm_lambda_increase", C.c_double),
+        ("lm_lambda_min", C.c_double),
+        ("lm_lambda_max", C.c_double),
+        ("lm_use_diag_scaling", C.c_int32),
+        ("_pad", C.c_int32),
+    ]
+
+
+class BlsOutputsC(C.Structure):
+    _fields_ = [
+        ("state_soa", C.c_void_p),
+        ("epoch_ns", C.c_void_p),
+        ("covar_soa", C.c_void_p),
+        ("iterations", C.c_void_p),
+        ("final_rms", C.c_void_p),
+        ("final_corr_pos_km", C.c_void_p),
+        ("converged", C.c_void_p),
+        ("details", C.c_void_p),
+        ("status", C.c_void_p),
     ]
 
 
@@ -310,6 +343,12 @@ def _declare(lib):
                                       C.c_size_t, vp, vp, vp, vp, C.POINTER(OdOutputsC)]
     lib.nyxb_od_predict_batch.restype = C.c_int32
     lib.nyxb_od_predict_batch.argtypes = [vp, C.POINTER(OdConfigC), C.c_size_t, vp, vp, vp, vp, vp, vp, C.POINTER(PredictOutputsC)]
+    lib.nyxb_od_bls_batch.restype = C.c_int32
+    lib.nyxb_od_bls_batch.argtypes = [vp, C.POINTER(BlsConfigC), C.c_int32, C.POINTER(GroundStationC), C.POINTER(TrackingArcC),
+                                      C.c_size_t, vp, vp, vp, C.POINTER(BlsOutputsC)]
+    lib.nyxb_od_bls_evaluate_batch.restype = C.c_int32
+    lib.nyxb_od_bls_evaluate_batch.argtypes = [vp, C.POINTER(BlsConfigC), C.c_int32, C.POINTER(GroundStationC), C.POINTER(TrackingArcC),
+                                               C.c_size_t, vp, vp, vp, vp, vp]
     lib.nyxb_mvn_sample.restype = C.c_int32
     lib.nyxb_mvn_sample.argtypes = [C.c_int32, C.c_uint64, C.c_uint64, C.c_size_t, vp, vp, vp, vp, vp]
     lib.nyxb_mvn_sample_dev.restype = C.c_int32
@@ -365,6 +404,8 @@ EXPORTED_SYMBOLS = [
     "nyxb_propagate_batch_stm",
     "nyxb_od_ekf_batch",
     "nyxb_od_predict_batch",
+    "nyxb_od_bls_batch",
+    "nyxb_od_bls_evaluate_batch",
     "nyxb_mvn_sample",
     "nyxb_mvn_sample_dev",
     "nyxb_reference_normals",

@@ -30,6 +30,8 @@ extern "C" cudaError_t nyxb_launch_od_coop(const DevSetup*, const DevOd*, const 
 extern "C" cudaError_t nyxb_launch_pred_coop(const DevSetup*, const DevOd*, const int*, size_t, const double*, const double*,
                                              const long long*, const long long*, const double*, const OdRecords*, long long*, double*,
                                              long long*, nyxb_details*, int*, cudaStream_t);
+extern "C" cudaError_t nyxb_launch_bls_coop(const DevSetup*, const DevOd*, const DevBls*, const int*, size_t, const double*, const double*,
+                                            const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
 extern "C" int nyxb_od_coop_kmax(void);
 extern "C" cudaError_t nyxb_launch_traj_resample(long long, const long long*, const double*, const long long*, size_t, size_t,
                                                  const long long*, double*, int*, cudaStream_t);
@@ -41,6 +43,7 @@ extern "C" cudaError_t nyxb_launch_mvn(unsigned long long, unsigned long long, s
 // layout of the PODs the host mirrors rely on (nyx_b200/abi.py, tests/test_abi.py)
 static_assert(sizeof(nyxb_integ_opts) == 56 && sizeof(nyxb_gravity_field) == 104 && sizeof(nyxb_dynamics) == 96 && sizeof(nyxb_rotation) == 56 && sizeof(nyxb_srp) == 40 && sizeof(nyxb_details) == 48, "ABI layout");
 static_assert(sizeof(nyxb_ground_station) == 176 && sizeof(nyxb_od_config) == 72 && sizeof(nyxb_tracking_arc) == 32 && sizeof(nyxb_od_outputs) == 96, "ABI layout");
+static_assert(sizeof(nyxb_bls_config) == 80 && sizeof(nyxb_bls_outputs) == 72, "ABI layout");
 
 static thread_local std::string g_err;
 static void set_err(const std::string& s) { g_err = s; }
@@ -1075,6 +1078,138 @@ extern "C" int32_t nyxb_od_predict_batch(nyxb_engine* eng, const nyxb_od_config*
     float ms = 0.f;
     if (cudaEventElapsedTime(&ms, eng->ev0, eng->ev1) == cudaSuccess) eng->last_ms = ms;
     return NYXB_RC_OK;
+}
+
+namespace {
+// nyxb_od_bls_batch / nyxb_od_bls_evaluate_batch: argument checks, packing, one launch, read-back.  `bl` carries the solver settings;
+// its output pointers are filled here.  out_* host pointers may be null except status.
+int32_t od_bls_run(nyxb_engine* eng, const nyxb_bls_config* cfg, int32_t n_stations, const nyxb_ground_station* stations,
+                   const nyxb_tracking_arc* arc, size_t n, const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
+                   DevBls bl, double* out_state, int64_t* out_epoch, double* out_covar, int32_t* out_iters, double* out_rms,
+                   double* out_corr, int32_t* out_conv, nyxb_details* out_details, int32_t* out_status) {
+    if (!eng || !cfg || !arc || !state_soa || !consts_soa || !epoch0_ns || !out_status || (n_stations > 0 && !stations) || n_stations < 0) {
+        set_err("null argument");
+        return NYXB_RC_BAD_ARG;
+    }
+    // stricter than the reference, which would loop forever (max_step <= 0) or take a usize (max_iterations)
+    if (cfg->max_step_ns <= 0) { set_err("StepSize: max_step must be positive"); return NYXB_RC_BAD_ARG; }
+    if (!bl.evaluate) {
+        if (cfg->solver != NYXB_BLS_NORMAL_EQUATIONS && cfg->solver != NYXB_BLS_LEVENBERG_MARQUARDT) { set_err("bad BLS solver"); return NYXB_RC_BAD_ARG; }
+        if (cfg->max_iterations < 0) { set_err("max_iterations must not be negative"); return NYXB_RC_BAD_ARG; }
+        if (cfg->solver == NYXB_BLS_LEVENBERG_MARQUARDT &&
+            !(cfg->lm_lambda_init > 0.0 && cfg->lm_lambda_decrease > 0.0 && cfg->lm_lambda_increase > 0.0 && cfg->lm_lambda_min > 0.0 &&
+              cfg->lm_lambda_max > 0.0)) {
+            set_err("Levenberg-Marquardt lambda settings must be positive");
+            return NYXB_RC_BAD_ARG;
+        }
+    }
+    if (arc->n_msr < 0 || (arc->n_msr > 0 && (!arc->epoch_ns || !arc->tracker || !arc->obs))) { set_err("null tracking arc arrays"); return NYXB_RC_BAD_ARG; }
+    if (!stm_supported(eng)) return NYXB_RC_UNSUPPORTED;
+    for (int32_t s = 0; s < n_stations; ++s) {
+        const nyxb_ground_station& g = stations[s];
+        if (g.n_types < 1 || g.n_types > 2 || (g.body != NYXB_CENTRAL_BODY && (g.body < 0 || g.body >= eng->S.n_bodies))) {
+            set_err("bad ground station descriptor");
+            return NYXB_RC_BAD_ARG;
+        }
+        for (int q = 0; q < g.n_types; ++q) {
+            if (g.types[q] != NYXB_MSR_RANGE && g.types[q] != NYXB_MSR_DOPPLER) { set_err("unsupported measurement type"); return NYXB_RC_UNSUPPORTED; }
+            // earlier than the reference, which fails with SingularNoiseRk at the first measurement of this station
+            if (!(g.noise_var[q] > 0.0)) { set_err("SingularNoiseRk: a station's noise variance must be positive"); return NYXB_RC_BAD_ARG; }
+        }
+    }
+    if (n == 0) return NYXB_RC_OK;
+    CUDA_TRY(cudaSetDevice(eng->device));
+    if (!eng->stream) CUDA_TRY(cudaStreamCreateWithFlags(&eng->stream, cudaStreamNonBlocking));
+    cudaStream_t st = eng->stream;
+    const size_t m = (size_t)arc->n_msr;
+    DevBufs B;
+    std::vector<DevStation> hs((size_t)n_stations);
+    for (int32_t s = 0; s < n_stations; ++s) {
+        const nyxb_ground_station& g = stations[s];
+        DevStation& d = hs[s];
+        for (int q = 0; q < 3; ++q) { d.pos[q] = g.pos_fixed_km[q]; d.up[q] = g.up_fixed[q]; }
+        d.mask_deg = g.elevation_mask_deg; d.rot = pack_rot(g.rot); d.body = g.body; d.n_types = g.n_types;
+        for (int q = 0; q < 2; ++q) { d.types[q] = g.types[q]; d.noise_var[q] = g.noise_var[q]; d.bias[q] = g.bias[q]; }
+        d.body_radius = g.body_radius_km;
+    }
+    DevOd od{};
+    od.msr_size = 1;
+    od.max_step_ns = cfg->max_step_ns; od.eps_ns = cfg->epoch_precision_ns;
+    od.n_stations = n_stations;
+    od.stations = n_stations ? B.put(hs.data(), hs.size(), st) : nullptr;
+    od.n_msr = arc->n_msr;
+    od.msr_epoch = m ? B.put((const long long*)arc->epoch_ns, m, st) : nullptr;
+    od.msr_tracker = m ? B.put((const int*)arc->tracker, m, st) : nullptr;
+    od.obs = m ? B.put(arc->obs, m * 2 * n, st) : nullptr;
+    double* d_state = B.put(state_soa, 9 * n, st);
+    double* d_consts = B.put(consts_soa, 4 * n, st);
+    long long* d_ep = B.put((const long long*)epoch0_ns, n, st);
+    double* d_out = B.alloc<double>(9 * n);
+    long long* d_oep = B.alloc<long long>(n);
+    nyxb_details* d_det = B.alloc<nyxb_details>(n);
+    int* d_status = B.alloc<int>(n);
+    bl.covar = out_covar ? B.alloc<double>(81 * n) : nullptr;
+    bl.iters = out_iters ? B.alloc<int>(n) : nullptr;
+    bl.rms = out_rms ? B.alloc<double>(n) : nullptr;
+    bl.corr_pos_km = out_corr ? B.alloc<double>(n) : nullptr;
+    bl.converged = out_conv ? B.alloc<int>(n) : nullptr;
+    if ((n_stations && !od.stations) || (m && (!od.msr_epoch || !od.msr_tracker || !od.obs)) || !d_state || !d_consts || !d_ep || !d_out ||
+        !d_oep || !d_det || !d_status || (out_covar && !bl.covar) || (out_iters && !bl.iters) || (out_rms && !bl.rms) ||
+        (out_corr && !bl.corr_pos_km) || (out_conv && !bl.converged)) {
+        set_err("device allocation / upload failed");
+        return NYXB_RC_CUDA;
+    }
+    const int* d_cols = nullptr;
+    if (int32_t rc = od_coop_cols(eng, B, st, d_cols)) return rc;
+    const bool coop = d_cols != nullptr;
+    CUDA_TRY(cudaEventRecord(eng->ev0, st));
+    cudaError_t err = coop
+        ? nyxb_launch_bls_coop(&eng->S, &od, &bl, d_cols, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
+        : (eng->mode == NYXB_MODE_STRICT)
+            ? nyxb_launch_bls_strict(&eng->S, &od, &bl, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
+            : nyxb_launch_bls_fast(&eng->S, &od, &bl, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st);
+    if (err != cudaSuccess) { set_err(std::string("kernel launch: ") + cudaGetErrorString(err)); return NYXB_RC_CUDA; }
+    eng->launches += 1;
+    eng->last_kernel = coop ? NYXB_KERNEL_COOP : NYXB_KERNEL_THREAD;
+    CUDA_TRY(cudaEventRecord(eng->ev1, st));
+    if (out_state) CUDA_TRY(cudaMemcpyAsync(out_state, d_out, sizeof(double) * 9 * n, cudaMemcpyDeviceToHost, st));
+    if (out_epoch) CUDA_TRY(cudaMemcpyAsync(out_epoch, d_oep, sizeof(long long) * n, cudaMemcpyDeviceToHost, st));
+    if (bl.covar) CUDA_TRY(cudaMemcpyAsync(out_covar, bl.covar, sizeof(double) * 81 * n, cudaMemcpyDeviceToHost, st));
+    if (bl.iters) CUDA_TRY(cudaMemcpyAsync(out_iters, bl.iters, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
+    if (bl.rms) CUDA_TRY(cudaMemcpyAsync(out_rms, bl.rms, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
+    if (bl.corr_pos_km) CUDA_TRY(cudaMemcpyAsync(out_corr, bl.corr_pos_km, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
+    if (bl.converged) CUDA_TRY(cudaMemcpyAsync(out_conv, bl.converged, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
+    if (out_details) CUDA_TRY(cudaMemcpyAsync(out_details, d_det, sizeof(nyxb_details) * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(out_status, d_status, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    float ms = 0.f;
+    if (cudaEventElapsedTime(&ms, eng->ev0, eng->ev1) == cudaSuccess) eng->last_ms = ms;
+    return NYXB_RC_OK;
+}
+}  // namespace
+
+extern "C" int32_t nyxb_od_bls_batch(nyxb_engine* eng, const nyxb_bls_config* cfg, int32_t n_stations, const nyxb_ground_station* stations,
+                                     const nyxb_tracking_arc* arc, size_t n, const double* state_soa, const double* consts_soa,
+                                     const int64_t* epoch0_ns, const nyxb_bls_outputs* out) {
+    if (!cfg || !out) { set_err("null argument"); return NYXB_RC_BAD_ARG; }
+    DevBls bl{};
+    bl.evaluate = 0;
+    bl.solver = cfg->solver; bl.max_iter = cfg->max_iterations; bl.lm_diag = cfg->lm_use_diag_scaling;
+    bl.tol_pos_km = cfg->tolerance_pos_km;
+    bl.lm_init = cfg->lm_lambda_init; bl.lm_dec = cfg->lm_lambda_decrease; bl.lm_inc = cfg->lm_lambda_increase;
+    bl.lm_min = cfg->lm_lambda_min; bl.lm_max = cfg->lm_lambda_max;
+    return od_bls_run(eng, cfg, n_stations, stations, arc, n, state_soa, consts_soa, epoch0_ns, bl, out->state_soa, out->epoch_ns,
+                      out->covar_soa, out->iterations, out->final_rms, out->final_corr_pos_km, out->converged, out->details, out->status);
+}
+
+extern "C" int32_t nyxb_od_bls_evaluate_batch(nyxb_engine* eng, const nyxb_bls_config* cfg, int32_t n_stations,
+                                              const nyxb_ground_station* stations, const nyxb_tracking_arc* arc, size_t n,
+                                              const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns, double* rms,
+                                              int32_t* status) {
+    DevBls bl{};
+    bl.evaluate = 1;
+    return od_bls_run(eng, cfg, n_stations, stations, arc, n, state_soa, consts_soa, epoch0_ns, bl, nullptr, nullptr, nullptr, nullptr,
+                      rms, nullptr, nullptr, nullptr, status);
 }
 
 extern "C" int32_t nyxb_mvn_sample_dev(int32_t device, uint64_t seed, uint64_t first_index, size_t n, const double* template_state,

@@ -16,6 +16,7 @@
 //   PropInstance::{propagate, single_step, derive}             propagators/instance.rs:87-262, 343-493
 //   KalmanODProcess::process_arc                               od/process/mod.rs:128-497
 //   KalmanFilter::{time_update, measurement_update}            od/kalman/filtering.rs:59-316
+//   BatchLeastSquares::{estimate, evaluate}                    od/blse/mod.rs:146-541
 //   ProcessNoise::propagate                                    od/snc.rs:175-286
 //   GroundStation::measure_instantaneous, ScalarSensitivity    od/ground_station/trk_device.rs:154-200, od/msr/sensitivity.rs:118-239
 // The reference gets the partials from forward-mode dual numbers (hyperdual 1.5.0); so does this file, with a 3-partial
@@ -32,6 +33,8 @@
 #define NYXB_LAUNCH_STM nyxb_launch_stm_strict
 #define NYXB_LAUNCH_OD nyxb_launch_od_strict
 #define NYXB_LAUNCH_PRED nyxb_launch_pred_strict
+#define NYXB_KBLS nyxb_k_bls_strict
+#define NYXB_LAUNCH_BLS nyxb_launch_bls_strict
 #else
 #define NYXB_KSTM nyxb_k_stm_fast
 #define NYXB_KOD nyxb_k_od_fast
@@ -39,6 +42,8 @@
 #define NYXB_LAUNCH_STM nyxb_launch_stm_fast
 #define NYXB_LAUNCH_OD nyxb_launch_od_fast
 #define NYXB_LAUNCH_PRED nyxb_launch_pred_fast
+#define NYXB_KBLS nyxb_k_bls_fast
+#define NYXB_LAUNCH_BLS nyxb_launch_bls_fast
 #endif
 
 // ------------------------------------------------------------------------- per-thread backend of nyxb_od_arc.cuh
@@ -122,6 +127,17 @@ NYXB_KPRED(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od,
     od_predict(od, b, i, n, state, consts, epoch0, end_epoch, dev0, rec, rec_count, out_state, out_epoch, out_details, out_status);
 }
 
+__global__ void __launch_bounds__(64)
+NYXB_KBLS(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od, const __grid_constant__ DevBls bl, size_t n,
+          const double* __restrict__ state, const double* __restrict__ consts, const long long* __restrict__ epoch0,
+          double* __restrict__ out_state, long long* __restrict__ out_epoch, nyxb_details* __restrict__ out_details,
+          int* __restrict__ out_status) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    ThreadB b(S);
+    od_bls(od, bl, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
+}
+
 extern "C" cudaError_t NYXB_LAUNCH_STM(const DevSetup* S, size_t n, const double* state, const double* consts, const long long* epoch0,
                                        long long end_epoch, long long* step_io, const double* stm_in, double* out_state,
                                        long long* out_epoch, double* out_stm, nyxb_details* out_details, int* out_status,
@@ -153,5 +169,15 @@ extern "C" cudaError_t NYXB_LAUNCH_PRED(const DevSetup* S, const DevOd* od, size
     unsigned grid = (unsigned)((n + block - 1) / block);
     NYXB_KPRED<<<grid, block, 0, stream>>>(*S, *od, n, state, consts, epoch0, end_epoch, dev0, *rec, rec_count, out_state, out_epoch,
                                            out_details, out_status);
+    return cudaGetLastError();
+}
+
+extern "C" cudaError_t NYXB_LAUNCH_BLS(const DevSetup* S, const DevOd* od, const DevBls* bl, size_t n, const double* state,
+                                       const double* consts, const long long* epoch0, double* out_state, long long* out_epoch,
+                                       nyxb_details* out_details, int* out_status, cudaStream_t stream) {
+    if (n == 0) return cudaSuccess;
+    const int block = 32;  // as the filter kernel
+    unsigned grid = (unsigned)((n + block - 1) / block);
+    NYXB_KBLS<<<grid, block, 0, stream>>>(*S, *od, *bl, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
     return cudaGetLastError();
 }

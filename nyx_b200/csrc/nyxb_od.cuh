@@ -47,6 +47,22 @@ struct OdRecords {
     double* covar;   // [cap][81][n] or null
 };
 
+// Batch least squares (BatchLeastSquares::estimate / evaluate, od/blse/mod.rs:146-541).  The schedule, stations, observations,
+// max_step and epoch precision come from DevOd; this holds the solver settings and the per-problem outputs ([n], covar [81][n]).
+struct DevBls {
+    int evaluate;                  // 1: evaluate() (the RMS of the given state), 0: estimate()
+    int solver;                    // enum nyxb_bls_solver
+    int max_iter;
+    int lm_diag;                   // lm_use_diag_scaling
+    double tol_pos_km;
+    double lm_init, lm_dec, lm_inc, lm_min, lm_max;
+    double* covar;                 // (r, c) at [(c*9 + r)*n + i]
+    int* iters;
+    double* rms;
+    double* corr_pos_km;
+    int* converged;
+};
+
 extern "C" cudaError_t nyxb_launch_stm_strict(const DevSetup*, size_t, const double*, const double*, const long long*, long long,
                                               long long*, const double*, double*, long long*, double*, nyxb_details*, int*, cudaStream_t);
 extern "C" cudaError_t nyxb_launch_stm_fast(const DevSetup*, size_t, const double*, const double*, const long long*, long long,
@@ -61,3 +77,7 @@ extern "C" cudaError_t nyxb_launch_pred_strict(const DevSetup*, const DevOd*, si
 extern "C" cudaError_t nyxb_launch_pred_fast(const DevSetup*, const DevOd*, size_t, const double*, const double*, const long long*,
                                              const long long*, const double*, const OdRecords*, long long*, double*, long long*,
                                              nyxb_details*, int*, cudaStream_t);
+extern "C" cudaError_t nyxb_launch_bls_strict(const DevSetup*, const DevOd*, const DevBls*, size_t, const double*, const double*,
+                                              const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
+extern "C" cudaError_t nyxb_launch_bls_fast(const DevSetup*, const DevOd*, const DevBls*, size_t, const double*, const double*,
+                                            const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);

@@ -17,6 +17,7 @@
 // The scratch types let the per-thread backend keep its temporaries in scoped locals; the warp backend points them into its slab.
 // Every scalar below (OdInst, h, the window, the gain inputs) is computed by every lane alike, so all lanes take the same branches.
 #pragma once
+#include <cfloat>
 #include "nyxb_od_device.cuh"
 
 // PropInstance scalars of one trajectory or filter (instance.rs:87-262)
@@ -488,5 +489,255 @@ __device__ void od_predict(const DevOd& od, B& b, size_t i, size_t n, const doub
     }
     if (od.state_dev) for (int r = b.first(); r < 9; r += B::stride) od.state_dev[(size_t)r * n + i] = f.xdev[r];
     if (rec_count && b.lead()) rec_count[i] = k;
+    od_store(b, in, rc, i, n, out_state, out_epoch, out_details, out_status);
+}
+
+// ------------------------------------------------------------------------- BatchLeastSquares::estimate / evaluate (od/blse/mod.rs:146-541)
+// The 9x9 algebra below is scalar code that every lane runs alike, so the decisions it feeds are uniform.  It reads the backend's arrays
+// and writes each entry of its result exactly once, with a value that is the same on every lane, from sums kept in registers: a lane
+// that runs ahead never changes an entry a slower lane has still to read.  Row-major 9x9 throughout.
+
+// Cholesky factor L (lower triangle of L) of A + diag(add): the column-oriented ("gaxpy") algorithm of Golub & Van Loan, Matrix
+// Computations, 4th ed., Alg. 4.2.2.  False when a pivot is not positive (nalgebra's `cholesky()` returning None).
+__device__ __forceinline__ bool bls_chol(const double* A, const double add[9], double* L) {
+    for (int j = 0; j < 9; ++j) {
+        double d = A[j * 9 + j] + add[j];
+        for (int k = 0; k < j; ++k) d -= L[j * 9 + k] * L[j * 9 + k];
+        if (!(d > 0.0)) return false;
+        d = sqrt(d);
+        L[j * 9 + j] = d;
+        for (int r = j + 1; r < 9; ++r) {
+            double s = A[r * 9 + j];
+            for (int k = 0; k < j; ++k) s -= L[r * 9 + k] * L[j * 9 + k];
+            L[r * 9 + j] = s / d;
+        }
+    }
+    return true;
+}
+
+// x = (L L^T)^-1 b: forward then back substitution
+__device__ __forceinline__ void bls_chol_solve(const double* L, const double* b, double x[9]) {
+    double y[9];
+    for (int r = 0; r < 9; ++r) {
+        double s = b[r];
+        for (int k = 0; k < r; ++k) s -= L[r * 9 + k] * y[k];
+        y[r] = s / L[r * 9 + r];
+    }
+    for (int r = 8; r >= 0; --r) {
+        double s = y[r];
+        for (int k = r + 1; k < 9; ++k) s -= L[k * 9 + r] * x[k];
+        x[r] = s / L[r * 9 + r];
+    }
+}
+
+// A = U D U^T with U unit upper triangular (Bierman, Factorization Methods for Discrete Sequential Estimation, 1977, the UDU^T
+// factorisation, columns from the last to the first; the order nalgebra's `udu()` uses).  U goes to U (entries on and above the
+// diagonal), D to d.  False when a d_j is zero.
+__device__ __forceinline__ bool bls_udu(const double* A, double* U, double d[9]) {
+    d[8] = A[80];
+    if (d[8] == 0.0) return false;
+    for (int i = 0; i < 9; ++i) U[i * 9 + 8] = (1.0 / d[8]) * A[i * 9 + 8];
+    for (int j = 7; j >= 0; --j) {
+        double dj = 0.0;
+        for (int k = j + 1; k < 9; ++k) dj += d[k] * (U[j * 9 + k] * U[j * 9 + k]);
+        d[j] = A[j * 9 + j] - dj;
+        if (d[j] == 0.0) return false;
+        for (int i = j - 1; i >= 0; --i) {
+            double u = 0.0;
+            for (int k = j + 1; k < 9; ++k) u += (d[k] * U[j * 9 + k]) * U[i * 9 + k];
+            U[i * 9 + j] = (A[i * 9 + j] - u) / d[j];
+        }
+        U[j * 9 + j] = 1.0;
+    }
+    return true;
+}
+
+// V = U^-1 of a unit upper-triangular U (back substitution, column by column; entries above and on the diagonal)
+__device__ __forceinline__ void bls_unit_upper_inv(const double* U, double* V) {
+    for (int c = 0; c < 9; ++c) {
+        V[c * 9 + c] = 1.0;
+        for (int r = c - 1; r >= 0; --r) {
+            double s = 0.0;
+            for (int k = r + 1; k <= c; ++k) s += U[r * 9 + k] * V[k * 9 + c];
+            V[r * 9 + c] = -s;
+        }
+    }
+}
+
+// Problem i of a batch: estimate() from the guess (state, epoch0) or, with bl.evaluate, the RMS of that state.  Storage: the
+// information matrix in f.P, the accumulated STM product in f.Pb, the product scratch and U^-1 in f.T, the Cholesky / UDU factor in
+// f.F, the normal vector in f.xdev.  The STM is set to the identity at the start of each iteration (`with_stm()`) and never reset
+// inside it, so after each chunk phi = Phi(t, t0) and `stm_acc = phi * stm_acc` is the product of cumulative STMs, as coded (:219-222).
+// A failed problem stores its status and the estimate it had reached.
+template <class B>
+__device__ void od_bls(const DevOd& od, const DevBls& bl, B& b, size_t i, size_t n, const double* state, const double* consts,
+                       const long long* epoch0, double* out_state, long long* out_epoch, nyxb_details* out_details, int* out_status) {
+    const DevSetup& S = b.S;
+    OdInst in;
+    od_load(S, in, i, n, state, consts, epoch0, nullptr);
+    const long long t0 = in.epoch_ns;
+    double x[9];
+#pragma unroll
+    for (int r = 0; r < 9; ++r) x[r] = in.y[r];
+    typename B::Filt f(b);
+    long long n_msr = 0;                                     // :152 the non-rejected (present) measurements of problem i
+    for (long long k = 0; k < od.n_msr; ++k) {
+        const double o0 = od.obs[((size_t)k * 2 + 0) * n + i], o1 = od.obs[((size_t)k * 2 + 1) * n + i];
+        if (!(o0 != o0 && o1 != o1)) ++n_msr;
+    }
+    const bool lm = bl.solver == NYXB_BLS_LEVENBERG_MARQUARDT;
+    double lambda = bl.lm_init, cur_rms = DBL_MAX, corr = DBL_MAX, rms = 0.0;
+    int iter = 0, rc = 0;
+    bool converged = false;
+    if (!bl.evaluate && bl.covar)                            // :170 zeros until an iteration is accepted
+        for (int e = b.first(); e < 81; e += B::stride) bl.covar[(size_t)e * n + i] = 0.0;
+    if (n_msr < (bl.evaluate ? 1 : 2)) rc = NYXB_ERR_TOO_FEW_MEASUREMENTS;   // :155-161, :459-465
+    const int passes = bl.evaluate ? 1 : bl.max_iter;
+    while (rc == 0 && iter < passes) {
+        ++iter;
+        // prop.with(current_estimate.with_stm()): a new instance at the initial step (no set_step(max_step)); the counters carry on
+#pragma unroll
+        for (int r = 0; r < 9; ++r) in.y[r] = x[r];
+        in.epoch_ns = t0;
+        in.step_ns = S.init_step_ns;
+        in.fixed = S.fixed_step;
+        in.det_step_ns = S.init_step_ns; in.det_error = 0.0; in.det_attempts = 1;
+        for (int e = b.first(); e < 81; e += B::stride) {    // info = I, stm_acc = I, STM = I (:186-197)
+            const double v = ((e / 9) == (e % 9)) ? 1.0 : 0.0;
+            f.P[e] = v; f.Pb[e] = v; b.phi[e] = v;
+        }
+        for (int r = b.first(); r < 9; r += B::stride) f.xdev[r] = 0.0;
+        b.sync();
+        double ssq = 0.0;
+        long long epoch = t0;
+        for (long long k = 0; k < od.n_msr && rc == 0; ++k) {
+            const long long t_k = od.msr_epoch[k];
+            const double o[2] = { od.obs[((size_t)k * 2 + 0) * n + i], od.obs[((size_t)k * 2 + 1) * n + i] };
+            if (o[0] != o[0] && o[1] != o[1]) continue;      // absent from problem i: `rejected`
+            for (;;) {
+                const long long delta_t = t_k - epoch;
+                if (delta_t <= 0) break;                     // :207-210
+                long long next_step = delta_t;               // :213
+                if (in.step_ns < next_step) next_step = in.step_ns;
+                if (od.max_step_ns < next_step) next_step = od.max_step_ns;
+                rc = od_propagate(b, in, next_step);
+                if (rc) break;
+                epoch = in.epoch_ns;
+                if (!bl.evaluate) {                          // stm_acc = phi * stm_acc (:220-222)
+                    for (int e = b.first(); e < 81; e += B::stride) {
+                        const int r = e / 9, c = e - 9 * r;
+                        double s = 0.0;
+#pragma unroll
+                        for (int q = 0; q < 9; ++q) s += b.phi[q * 9 + r] * f.Pb[q * 9 + c];
+                        f.T[e] = s;
+                    }
+                    b.sync();
+                    for (int e = b.first(); e < 81; e += B::stride) f.Pb[e] = f.T[e];
+                    b.sync();
+                }
+                long long gap = epoch - t_k;
+                if (gap < 0) gap = -gap;
+                if (!(gap < od.eps_ns)) continue;            // :224
+                const int trk = od.msr_tracker[k];
+                if (trk < 0 || trk >= od.n_stations) continue;   // unknown tracker :226-237
+                const DevStation& gs = od.stations[trk];
+                for (int wno = 0; wno < gs.n_types; ++wno) {     // each type of msr.data on its own, as U1 (:240-297)
+                    OdWindow w;
+                    const int wrc = od_window_setup<false>(S, gs, 1, wno, o, epoch, in.y, w);
+                    if (wrc == OD_WIN_UNAVAILABLE || wrc == OD_WIN_NOT_VISIBLE) continue;   // type not in msr.data / not visible
+                    if (wrc == OD_WIN_EPHEMERIS) { rc = NYXB_ERR_EPHEMERIS; break; }
+                    const double real_obs = w.real_obs[0];
+                    if (!isfinite(real_obs)) { rc = NYXB_ERR_INVALID_MEASUREMENT; break; }   // :266-272
+                    const double resid = real_obs - w.comp[0];
+                    const double weight = 1.0 / w.Rk[0];     // Rk > 0: checked by the host (:282)
+                    if (!bl.evaluate) {
+                        double h[9];                         // h = h_tilde * stm_acc (:286)
+#pragma unroll
+                        for (int c = 0; c < 9; ++c) {
+                            double s = 0.0;
+#pragma unroll
+                            for (int q = 0; q < 9; ++q) s += w.H[0][q] * f.Pb[q * 9 + c];
+                            h[c] = s;
+                        }
+                        for (int e = b.first(); e < 81; e += B::stride) {   // info += h^T h W (:290)
+                            const int r = e / 9, c = e - 9 * r;
+                            f.P[e] += (h[r] * h[c]) * weight;
+                        }
+                        for (int r = b.first(); r < 9; r += B::stride) f.xdev[r] += (h[r] * resid) * weight;   // :293
+                        b.sync();
+                    }
+                    ssq += (weight * resid) * resid;         // :296
+                }
+            }
+        }
+        if (rc) break;
+        rms = sqrt(ssq / (double)n_msr);                     // :307
+        if (bl.evaluate) break;
+        // ---- solve (:309-379)
+        double add[9], dx[9];
+        if (lm) {
+            for (int q = 0; q < 9; ++q) {
+                double d = 1.0;
+                if (bl.lm_diag && q < 6) { d = f.P[q * 9 + q]; if (d <= 0.0) d = 1e-6; }
+                add[q] = d * lambda;
+            }
+        } else {
+            for (int q = 0; q < 9; ++q) add[q] = 0.0;
+        }
+        const bool ok = bls_chol(f.P, add, f.F);
+        if (ok) bls_chol_solve(f.F, f.xdev, dx);
+        b.sync();
+        bool accept;
+        if (!lm) {
+            if (!ok) { rc = NYXB_ERR_SINGULAR_INFORMATION; break; }
+            accept = true;
+            cur_rms = rms;
+        } else if (!ok) {                                    // :369-377 singular: raise lambda, the iteration is spent
+            lambda *= bl.lm_inc * 10.0;
+            lambda = fmin(lambda, bl.lm_max);
+            continue;
+        } else if (rms < cur_rms) {
+            accept = true;
+            lambda /= bl.lm_dec;
+            lambda = fmax(lambda, bl.lm_min);
+            cur_rms = rms;
+        } else {
+            accept = false;
+            lambda *= bl.lm_inc;
+            lambda = fmin(lambda, bl.lm_max);
+        }
+        if (!accept) { corr = DBL_MAX; continue; }           // :424-430
+        // ---- `Spacecraft + OVector<9>`, correction size, covariance (:384-423)
+#pragma unroll
+        for (int r = 0; r < 9; ++r) x[r] = x[r] + dx[r];
+        x[6] = x[6] < 0.0 ? 0.0 : (x[6] > 2.0 ? 2.0 : x[6]);
+        corr = sqrt((dx[0] * dx[0] + dx[1] * dx[1]) + dx[2] * dx[2]);
+        if (bl.covar) {
+            double d[9];
+            const bool udu = bls_udu(f.P, f.F, d);
+            if (udu) bls_unit_upper_inv(f.F, f.T);
+            b.sync();
+            for (int e = b.first(); e < 81; e += B::stride) { // U^-T (D^-1 U^-1), or I when the factorisation fails
+                const int r = e / 9, c = e - 9 * r;
+                double s = (r == c) ? 1.0 : 0.0;
+                if (udu) {
+                    s = 0.0;
+                    for (int k = 0; k <= (r < c ? r : c); ++k) s += f.T[k * 9 + r] * ((1.0 / d[k]) * f.T[k * 9 + c]);
+                }
+                bl.covar[(size_t)(c * 9 + r) * n + i] = s;
+            }
+            b.sync();
+        }
+        if (corr < bl.tol_pos_km) { converged = true; break; }
+    }
+#pragma unroll
+    for (int r = 0; r < 9; ++r) in.y[r] = x[r];
+    in.epoch_ns = t0;
+    if (b.lead()) {
+        if (bl.iters) bl.iters[i] = iter;
+        if (bl.rms) bl.rms[i] = bl.evaluate ? rms : cur_rms;
+        if (bl.corr_pos_km) bl.corr_pos_km[i] = corr;
+        if (bl.converged) bl.converged[i] = converged ? 1 : 0;
+    }
     od_store(b, in, rc, i, n, out_state, out_epoch, out_details, out_status);
 }

@@ -273,6 +273,26 @@ nyxb_k_pred_coop(const __grid_constant__ DevSetup S, const __grid_constant__ Dev
     od_predict(od, b, i, n, state, consts, epoch0, end_epoch, dev0, rec, rec_count, out_state, out_epoch, out_details, out_status);
 }
 
+// batch least squares (BatchLeastSquares::estimate / evaluate), one warp per problem: same slab and column deal as the filter kernel
+__global__ void __launch_bounds__(32 * ODC_WPB)
+nyxb_k_bls_coop(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od, const __grid_constant__ DevBls bl,
+                const int* __restrict__ cols, size_t n, const double* __restrict__ state, const double* __restrict__ consts,
+                const long long* __restrict__ epoch0, double* __restrict__ out_state, long long* __restrict__ out_epoch,
+                nyxb_details* __restrict__ out_details, int* __restrict__ out_status) {
+    extern __shared__ __align__(16) unsigned char smem[];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    const size_t i = (size_t)blockIdx.x * ODC_WPB + wib;
+    if (i >= n) return;   // whole warps leave together
+    const int npw = S.has_grav ? 3 * (S.grav.N + 2) : 0;
+    const size_t slab = (sizeof(WarpS) + sizeof(D3) * (size_t)npw + 15) & ~(size_t)15;
+    WarpS& W = *reinterpret_cast<WarpS*>(smem + slab * wib);
+    Ctx cx;
+    cx.S = &S; cx.mycols = cols + lane * ODC_KMAX; cx.W = &W; cx.lane = lane;
+    cx.pw = reinterpret_cast<D3*>(smem + slab * wib + sizeof(WarpS));
+    WarpB b(cx);
+    od_bls(od, bl, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
+}
+
 extern "C" size_t nyxb_od_coop_smem_bytes(int degree_or_zero) {
     const size_t npw = degree_or_zero > 0 ? 3 * (size_t)(degree_or_zero + 2) : 0;
     const size_t slab = (sizeof(WarpS) + sizeof(D3) * npw + 15) & ~(size_t)15;
@@ -305,5 +325,18 @@ extern "C" cudaError_t nyxb_launch_pred_coop(const DevSetup* S, const DevOd* od,
     unsigned grid = (unsigned)((n + ODC_WPB - 1) / ODC_WPB);
     nyxb_k_pred_coop<<<grid, 32 * ODC_WPB, smem, stream>>>(*S, *od, cols, n, state, consts, epoch0, end_epoch, dev0, *rec, rec_count,
                                                            out_state, out_epoch, out_details, out_status);
+    return cudaGetLastError();
+}
+
+extern "C" cudaError_t nyxb_launch_bls_coop(const DevSetup* S, const DevOd* od, const DevBls* bl, const int* cols, size_t n,
+                                            const double* state, const double* consts, const long long* epoch0, double* out_state,
+                                            long long* out_epoch, nyxb_details* out_details, int* out_status, cudaStream_t stream) {
+    if (n == 0) return cudaSuccess;
+    const size_t smem = nyxb_od_coop_smem_bytes(S->has_grav ? S->grav.N : 0);
+    cudaError_t e = cudaFuncSetAttribute(nyxb_k_bls_coop, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    unsigned grid = (unsigned)((n + ODC_WPB - 1) / ODC_WPB);
+    nyxb_k_bls_coop<<<grid, 32 * ODC_WPB, smem, stream>>>(*S, *od, *bl, cols, n, state, consts, epoch0, out_state, out_epoch, out_details,
+                                                          out_status);
     return cudaGetLastError();
 }

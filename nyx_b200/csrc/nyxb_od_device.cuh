@@ -233,6 +233,8 @@ __device__ static bool station_state(const DevSetup& S, const DevStation& st, lo
 // the tracker geometry (range, range rate, elevation mask, line-of-sight obstruction), `h_tilde` (msr/sensitivity.rs:88-239:
 // identity rows unless the type is in msr.data; the observed range / Doppler in the denominators, as coded), the measurement
 // noise and the computed observation minus the device bias.  Shared by the per-thread and the warp-cooperative filter kernels.
+// SUB_BIAS = false leaves the bias in: the batch least-squares estimator compares with measure_instantaneous(state, None), which
+// has no noise and no bias (blse/mod.rs:248-249).
 struct OdWindow {
     int ncur;
     int cur[2];
@@ -242,6 +244,7 @@ struct OdWindow {
 };
 enum { OD_WIN_OK = 0, OD_WIN_EMPTY = 1, OD_WIN_UNAVAILABLE = 2, OD_WIN_NOT_VISIBLE = 3, OD_WIN_EPHEMERIS = 4 };
 
+template <bool SUB_BIAS = true>
 __device__ static int od_window_setup(const DevSetup& S, const DevStation& gs, int M, int wno, const double o[2], long long t_k,
                                       const double y[9], OdWindow& w) {
     w.ncur = 0;
@@ -275,7 +278,8 @@ __device__ static int od_window_setup(const DevSetup& S, const DevStation& gs, i
     for (int q = 0; q < w.ncur; ++q) {
         const int slot = wno * M + q;  // position of the type in the device's list
         w.Rk[q] = gs.noise_var[slot];
-        w.comp[q] = ((w.cur[q] == NYXB_MSR_RANGE) ? rng : rr) - gs.bias[slot];
+        w.comp[q] = ((w.cur[q] == NYXB_MSR_RANGE) ? rng : rr);
+        if (SUB_BIAS) w.comp[q] -= gs.bias[slot];
         if (!w.avail[q]) continue;
         if (w.cur[q] == NYXB_MSR_DOPPLER) {
             const double rho = rng, rho_dot = o[NYXB_MSR_DOPPLER], rho2 = rho * rho;

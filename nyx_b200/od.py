@@ -11,6 +11,8 @@
 * ``KalmanODProcess``          od/process/{initializers.rs:60-113, mod.rs:128-497}; `predict_until` / `predict_for` mod.rs:440-496;
                                `SpacecraftKalmanOD` = MsrSize 2,
                                `SpacecraftKalmanScalarOD` = MsrSize 1 (od/mod.rs:77-91)
+* ``BatchLeastSquares``        od/blse/mod.rs:30-541 (``BLSSolver``, ``BLSSolution``; `estimate` / `evaluate` through
+                               ``nyxb_od_bls_batch`` / ``nyxb_od_bls_evaluate_batch``, n problems in one launch)
 
 Nothing here runs the filter: ``KalmanODProcess.process_arcs`` packs the ensemble into the SoA arrays of
 ``nyxb_od_ekf_batch`` (include/nyxb.h) — ONE kernel launch runs every filter from the first to the last measurement
@@ -226,6 +228,18 @@ class TrackingDataArc:
         order = np.argsort(ep, kind="stable")
         trk = tab["Tracking device"].to_pylist()
         return cls(ep[order], [trk[i] for i in order], obs[order][:, :, None])
+
+    def filter_by_offset(self, start_ns: Optional[int] = None, end_ns: Optional[int] = None) -> "TrackingDataArc":
+        """`TrackingDataArc::filter_by_offset` (od/msr/trackingdata/mod.rs:394-410) as coded: the measurements in
+        [first + start, first + end), first being the first epoch of the schedule.  Whatever the bound kind, the end is exclusive, and
+        an open end stands for the last epoch, so that the last measurement is dropped; an open start keeps from the first."""
+        if len(self) == 0:
+            return self
+        first, last = int(self.epoch_ns[0]), int(self.epoch_ns[-1])
+        lo = first if start_ns is None else first + int(start_ns)
+        hi = last if end_ns is None else first + int(end_ns)
+        keep = (self.epoch_ns >= lo) & (self.epoch_ns < hi)
+        return TrackingDataArc(self.epoch_ns[keep], [t for t, k in zip(self.tracker, keep) if k], self.obs[keep])
 
     @classmethod
     def stack(cls, arcs: Sequence["TrackingDataArc"]) -> "TrackingDataArc":
@@ -696,6 +710,153 @@ def SpacecraftKalmanOD(prop, kf_variant, sigma_reject, devices, almanac) -> Kalm
 
 def SpacecraftKalmanScalarOD(prop, kf_variant, sigma_reject, devices, almanac) -> KalmanODProcess:
     return KalmanODProcess(prop, kf_variant, sigma_reject, devices, almanac, msr_size=1)
+
+
+class BLSSolver(enum.IntEnum):
+    NormalEquations = abi.BLS_NORMAL_EQUATIONS
+    LevenbergMarquardt = abi.BLS_LEVENBERG_MARQUARDT
+
+
+_BLS_ERRORS = {abi.ERR_TOO_FEW_MEASUREMENTS: "TooFewMeasurements", abi.ERR_SINGULAR_INFORMATION: "SingularInformationMatrix",
+               abi.ERR_INVALID_MEASUREMENT: "InvalidMeasurement"}
+
+
+def _bls_error(status: int) -> Optional[str]:
+    """The ODError a non-zero per-problem status stands for (propagation errors keep their status number)."""
+    code = int(status) & 0xFF
+    if code == 0:
+        return None
+    return _BLS_ERRORS.get(code, f"ODPropError (status {code})")
+
+
+@dataclass
+class BLSSolution:
+    """`BLSSolution` (od/blse/solution.rs) of one problem."""
+
+    estimated_state: Spacecraft
+    covariance: np.ndarray           # [9][9]
+    num_iterations: int
+    final_rms: float
+    final_corr_pos_km: float
+    converged: bool
+
+    def to_kf_estimate(self) -> KfEstimate:
+        """`From<BLSSolution> for KfEstimate` (od/blse/solution.rs:75-93): the covariance with entries (6,6), (7,7) and (8,8) zeroed."""
+        cov = np.array(self.covariance, dtype=np.float64).copy()
+        for q in (6, 7, 8):
+            cov[q, q] = 0.0
+        return KfEstimate(self.estimated_state, cov)
+
+
+@dataclass
+class BLSEnsembleSolution:
+    """Results of n batch least-squares problems solved in one launch; `solution(i)` is problem i's `BLSSolution`, `status[i]` its
+    error (0: Ok; see `ODError` for the single-problem calls)."""
+
+    state_soa: np.ndarray            # [9][n]
+    epoch_ns: np.ndarray             # [n]
+    covar: np.ndarray                # [n][9][9]
+    iterations: np.ndarray           # [n]
+    final_rms: np.ndarray            # [n]
+    final_corr_pos_km: np.ndarray    # [n]
+    converged: np.ndarray            # [n] bool
+    details: np.ndarray
+    status: np.ndarray
+    templates: Sequence[Spacecraft] = ()
+
+    def __len__(self):
+        return self.status.shape[0]
+
+    def error(self, i: int) -> Optional[str]:
+        return _bls_error(self.status[i])
+
+    def solution(self, i: int) -> BLSSolution:
+        err = self.error(i)
+        if err is not None:
+            raise ODError(f"{err} (problem {i})")
+        sc = self.templates[i].with_vector(int(self.epoch_ns[i]), self.state_soa[:, i])
+        return BLSSolution(sc, self.covar[i].copy(), int(self.iterations[i]), float(self.final_rms[i]), float(self.final_corr_pos_km[i]),
+                           bool(self.converged[i]))
+
+
+class BatchLeastSquares:
+    """`BatchLeastSquares<SpacecraftDynamics, GroundStation>` (od/blse/mod.rs:30-541) on the batched GPU path, with the reference's
+    builder defaults (od/blse/mod.rs:80-135).  Every problem of an ensemble shares the devices and the schedule of
+    the arc; each has its own initial guess and observation set."""
+
+    def __init__(self, prop, devices: Dict[str, GroundStation], almanac: Optional[Almanac], solver: BLSSolver = BLSSolver.NormalEquations,
+                 tolerance_pos_km: float = 1e-4, max_iterations: int = 10, max_step: int = 30 * NS_PER_S, epoch_precision: int = 1_000,
+                 lm_lambda_init: float = 10.0, lm_lambda_decrease: float = 10.0, lm_lambda_increase: float = 10.0,
+                 lm_lambda_min: float = 1e-12, lm_lambda_max: float = 1e12, lm_use_diag_scaling: bool = True):
+        self.prop = prop
+        self.devices = dict(devices)
+        self.almanac = almanac
+        self.solver = BLSSolver(solver)
+        self.tolerance_pos_km = float(tolerance_pos_km)
+        self.max_iterations = int(max_iterations)
+        self.max_step = int(max_step)
+        self.epoch_precision = int(epoch_precision)
+        self.lm_lambda_init = float(lm_lambda_init)
+        self.lm_lambda_decrease = float(lm_lambda_decrease)
+        self.lm_lambda_increase = float(lm_lambda_increase)
+        self.lm_lambda_min = float(lm_lambda_min)
+        self.lm_lambda_max = float(lm_lambda_max)
+        self.lm_use_diag_scaling = bool(lm_use_diag_scaling)
+
+    def config_c(self) -> abi.BlsConfigC:
+        c = abi.BlsConfigC()
+        c.solver = int(self.solver)
+        c.max_iterations = self.max_iterations
+        c.tolerance_pos_km = self.tolerance_pos_km
+        c.max_step_ns = self.max_step
+        c.epoch_precision_ns = self.epoch_precision
+        c.lm_lambda_init, c.lm_lambda_decrease, c.lm_lambda_increase = self.lm_lambda_init, self.lm_lambda_decrease, self.lm_lambda_increase
+        c.lm_lambda_min, c.lm_lambda_max = self.lm_lambda_min, self.lm_lambda_max
+        c.lm_use_diag_scaling = int(self.lm_use_diag_scaling)
+        return c
+
+    def _pack(self, guesses: Sequence[Spacecraft], arc: TrackingDataArc):
+        from .cosmic import pack_spacecraft
+
+        n = len(guesses)
+        if n == 0:
+            raise ODError("no initial guess")
+        if arc.n != n:
+            raise ODError(f"arc carries {arc.n} observation sets for {n} problems")
+        frame = guesses[0].orbit.frame
+        st, cs, ep = pack_spacecraft(guesses)
+        eng = self.prop.engine(frame, self.almanac)
+        names = list(self.devices)
+        st_c = (abi.GroundStationC * max(len(names), 1))()
+        for i, nme in enumerate(names):
+            st_c[i] = self.devices[nme].to_c(frame, self.almanac)
+        tracker = np.array([names.index(t) if t in names else -1 for t in arc.tracker], dtype=np.int32)
+        return eng, (self.config_c(), len(names), st_c, arc.epoch_ns, tracker, arc.obs, st, cs, ep)
+
+    def estimate_ensemble(self, guesses: Sequence[Spacecraft], arc: TrackingDataArc) -> BLSEnsembleSolution:
+        """n independent `estimate(guess_i, arc_i)` runs in one launch; failures are per-problem statuses."""
+        guesses = list(guesses)
+        eng, args = self._pack(guesses, arc)
+        r = eng.od_bls_batch(*args)
+        return BLSEnsembleSolution(r["state"], r["epoch"], r["covar"], r["iterations"], r["final_rms"], r["final_corr_pos_km"],
+                                   r["converged"] != 0, r["details"], r["status"], guesses)
+
+    def estimate(self, initial_guess: Spacecraft, arc: TrackingDataArc) -> BLSSolution:
+        """`BatchLeastSquares::estimate` (od/blse/mod.rs:146-446); raises ODError where the reference returns Err."""
+        return self.estimate_ensemble([initial_guess], arc).solution(0)
+
+    def evaluate_ensemble(self, states: Sequence[Spacecraft], arc: TrackingDataArc):
+        """n independent `evaluate(state_i, arc_i)` runs in one launch: (rms[n], status[n])."""
+        eng, args = self._pack(list(states), arc)
+        return eng.od_bls_evaluate_batch(*args)
+
+    def evaluate(self, state: Spacecraft, arc: TrackingDataArc) -> float:
+        """`BatchLeastSquares::evaluate` (od/blse/mod.rs:450-541): the RMS of the weighted residuals of `state` over the arc."""
+        rms, status = self.evaluate_ensemble([state], arc)
+        err = _bls_error(status[0])
+        if err is not None:
+            raise ODError(err)
+        return float(rms[0])
 
 
 # --------------------------------------------------------------------------- measurement simulation (host-side data generation)

@@ -377,6 +377,50 @@ class Engine:
         covar = np.ascontiguousarray(out_cov.T.reshape(n, 9, 9).transpose(0, 2, 1))  # (c*9+r) -> [i][r][c]
         return ODSolution(out_state, out_epoch, covar, out_dev, ratio, prefit, postfit, flags, est_state, est_cov, details, status)
 
+    def _bls_args(self, msr_epoch_ns, msr_tracker, obs, state_soa, consts_soa, epoch0_ns):
+        state_soa = np.ascontiguousarray(state_soa, dtype=np.float64)
+        consts_soa = np.ascontiguousarray(consts_soa, dtype=np.float64)
+        epoch0_ns = np.ascontiguousarray(epoch0_ns, dtype=np.int64)
+        msr_epoch_ns = np.ascontiguousarray(msr_epoch_ns, dtype=np.int64)
+        msr_tracker = np.ascontiguousarray(msr_tracker, dtype=np.int32)
+        obs = np.ascontiguousarray(obs, dtype=np.float64)
+        n = state_soa.shape[1]
+        m = msr_epoch_ns.shape[0]
+        if state_soa.shape != (9, n) or consts_soa.shape != (4, n) or epoch0_ns.shape != (n,):
+            raise ValueError("expected state[9][n], consts[4][n], epoch0[n]")
+        if obs.shape != (m, 2, n) or msr_tracker.shape != (m,):
+            raise ValueError("expected obs[m][2][n], tracker[m]")
+        arc = abi.TrackingArcC(m, msr_epoch_ns.ctypes.data, msr_tracker.ctypes.data, obs.ctypes.data)
+        return n, arc, (msr_epoch_ns, msr_tracker, obs), state_soa, consts_soa, epoch0_ns
+
+    def od_bls_batch(self, cfg_c, n_stations, stations_c, msr_epoch_ns, msr_tracker, obs, state_soa, consts_soa, epoch0_ns):
+        """`nyxb_od_bls_batch`: n batch least-squares estimates (`BatchLeastSquares::estimate`, od/blse/mod.rs:146-446) over one
+        tracking schedule in ONE launch.  Returns a dict of the output arrays; covariances as [n][9][9]."""
+        n, arc, keep, state_soa, consts_soa, epoch0_ns = self._bls_args(msr_epoch_ns, msr_tracker, obs, state_soa, consts_soa, epoch0_ns)
+        r = dict(state=np.empty((9, n)), epoch=np.empty(n, dtype=np.int64), covar=np.empty((81, n)), iterations=np.zeros(n, dtype=np.int32),
+                 final_rms=np.empty(n), final_corr_pos_km=np.empty(n), converged=np.zeros(n, dtype=np.int32),
+                 details=np.zeros(n, dtype=abi.DETAILS_DTYPE), status=np.zeros(n, dtype=np.int32))
+        out = abi.BlsOutputsC(*(r[k].ctypes.data for k in ("state", "epoch", "covar", "iterations", "final_rms", "final_corr_pos_km",
+                                                           "converged", "details", "status")))
+        rc = self._lib.nyxb_od_bls_batch(self._h, C.byref(cfg_c), int(n_stations), stations_c, C.byref(arc), n, state_soa.ctypes.data,
+                                         consts_soa.ctypes.data, epoch0_ns.ctypes.data, C.byref(out))
+        if rc != 0:
+            raise PropagationError(f"nyxb_od_bls_batch rc={rc}: {abi.last_error()}")
+        r["covar"] = np.ascontiguousarray(r["covar"].T.reshape(n, 9, 9).transpose(0, 2, 1))  # (c*9+r) -> [i][r][c]
+        return r
+
+    def od_bls_evaluate_batch(self, cfg_c, n_stations, stations_c, msr_epoch_ns, msr_tracker, obs, state_soa, consts_soa, epoch0_ns):
+        """`nyxb_od_bls_evaluate_batch` (`BatchLeastSquares::evaluate`, od/blse/mod.rs:450-541): (rms[n], status[n])."""
+        n, arc, keep, state_soa, consts_soa, epoch0_ns = self._bls_args(msr_epoch_ns, msr_tracker, obs, state_soa, consts_soa, epoch0_ns)
+        rms = np.empty(n)
+        status = np.zeros(n, dtype=np.int32)
+        rc = self._lib.nyxb_od_bls_evaluate_batch(self._h, C.byref(cfg_c), int(n_stations), stations_c, C.byref(arc), n,
+                                                  state_soa.ctypes.data, consts_soa.ctypes.data, epoch0_ns.ctypes.data, rms.ctypes.data,
+                                                  status.ctypes.data)
+        if rc != 0:
+            raise PropagationError(f"nyxb_od_bls_evaluate_batch rc={rc}: {abi.last_error()}")
+        return rms, status
+
     def od_predict_batch(self, cfg_c, state_soa, consts_soa, epoch0_ns, end_epoch_ns, covar0_soa, state_dev0_soa=None,
                          capacity: int = 0, record_states: bool = True, record_covars: bool = True):
         """`nyxb_od_predict_batch`: n covariance predictions (`KalmanODProcess::predict_until`, od/process/mod.rs:440-486) in ONE

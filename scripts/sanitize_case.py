@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Small launches of every shared-memory-cooperating kernel, meant to run under compute-sanitizer (SURVEY.md section 5):
 
-    compute-sanitizer --tool racecheck python scripts/sanitize_case.py coop|strict|tx|od
+    compute-sanitizer --tool racecheck python scripts/sanitize_case.py coop|strict|tx|od|blse
     compute-sanitizer --tool memcheck  python scripts/sanitize_case.py all
 
 Sizes are tiny (the tools slow kernels down ~100x): a few trajectories over a few steps, with rejections and a recording sink."""
@@ -57,9 +57,19 @@ def run(which):
         sol = sc["odp"].process_arcs(sc["ests"], sc["arc"], record_estimates=True)
         assert (sol.status == 0).all()
         print(which, "filters", 3, "accepted", int(sol.accepted().sum()))
+    elif which == "blse":   # nyxb_k_bls_coop: 3 problems, 4 measurements, LM with a rejected step (lambda0 = 1e-12)
+        from oracle import pyoracle
+        from tests.blse_util import blse_scenario
+
+        sc = blse_scenario(pyoracle, n=3, n_msr=4, cadence_s=30, degree=12, mode=nb.MODE_FAST)
+        b = nb.BatchLeastSquares(sc["prop"], sc["devices"], None, solver=nb.BLSSolver.LevenbergMarquardt, max_iterations=3,
+                                 lm_lambda_init=1e-12)
+        sol = b.estimate_ensemble(sc["guesses"], sc["arc"])
+        assert sc["prop"].engine(sc["frame"], None).last_kernel() == nb.KERNEL_COOP and (sol.status == 0).all()
+        print(which, "problems", 3, "iterations", sol.iterations.tolist())
 
 
 if __name__ == "__main__":
     which = sys.argv[1] if len(sys.argv) > 1 else "all"
-    for w in (["thread", "coop", "strict", "tx", "od"] if which == "all" else [which]):
+    for w in (["thread", "coop", "strict", "tx", "od", "blse"] if which == "all" else [which]):
         run(w)
