@@ -37,7 +37,8 @@ extern "C" {
 #define NYXB_ABI_VERSION 4 /* 4: nyxb_engine_set_kernel / nyxb_engine_last_kernel / nyxb_engine_set_tx_tuning, nyxb_tx_table_dump, nyxb_propagate_batch_multi, nyxb_reference_normals;
                               nyxb_integ_opts.state_center, nyxb_gravity_field.body, nyxb_dynamics.n_gravity / n_point_masses / point_mass_order; nyxb_od_predict_batch
                               and nyxb_predict_outputs, then nyxb_od_bls_batch, nyxb_od_bls_evaluate_batch, nyxb_bls_config, nyxb_bls_outputs and
-                              the status codes 6-8 were added later without a bump (a pure addition: no existing type or entry point changed).  Earlier: 2: nyxb_srp gained `estimate`; STM, filter and dispersion entry points.  3: nyxb_traj_resample[_dev], nyxb_event_locate[_dev] */
+                              the status codes 6-8, then nyxb_od_records, nyxb_od_ekf_record_batch, nyxb_smooth_outputs, nyxb_od_smooth_batch
+                              and the status codes 9-10 were added later without a bump (a pure addition: no existing type or entry point changed).  Earlier: 2: nyxb_srp gained `estimate`; STM, filter and dispersion entry points.  3: nyxb_traj_resample[_dev], nyxb_event_locate[_dev] */
 
 /* ---- IntegratorMethod — propagators/rk_methods/mod.rs:65-79 (same order) ---- */
 enum nyxb_method {
@@ -204,6 +205,8 @@ enum nyxb_status {
     NYXB_ERR_TOO_FEW_MEASUREMENTS = 6, /* ODError::TooFewMeasurements (blse/mod.rs:155-161) */
     NYXB_ERR_SINGULAR_INFORMATION = 7, /* ODError::SingularInformationMatrix (blse/mod.rs:312-315) */
     NYXB_ERR_INVALID_MEASUREMENT = 8,  /* ODError::InvalidMeasurement: an observation that is not finite (blse/mod.rs:266-272) */
+    NYXB_ERR_SINGULAR_STM = 9,         /* ODError::SingularStateTransitionMatrix (solution/smooth.rs:149-154) */
+    NYXB_ERR_RECORDS_TRUNCATED = 10,   /* the estimate records of a filter exceed their capacity: nothing to smooth from */
     NYXB_WARN_MAX_ATTEMPTS = 0x100 /* OR-ed flag: instance.rs:440-445 (warn only) */
 };
 
@@ -474,6 +477,79 @@ int32_t nyxb_od_ekf_batch(nyxb_engine* eng, const nyxb_od_config* cfg,
                           const nyxb_tracking_arc* arc, size_t n,
                           const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
                           const double* covar0_soa, const nyxb_od_outputs* out);
+
+/* ---- Every estimate of a filter run, for the smoother.  nyxb_od_ekf_record_batch runs nyxb_od_ekf_batch (same arguments, same
+ * kernel family, bit-identical `out`) and also writes one record per entry the reference pushes to ODSolution.estimates
+ * (process/mod.rs:211-426), in push order:
+ *   - a time update per propagation chunk that does not land on a measurement (several per gap when the step is below max_step);
+ *   - a measurement update per residual window that reaches `measurement_update`, sigma-rejected ones included (their estimate is the
+ *     time update made inside it, filtering.rs:186-200).  With msr_size 1 and two types, one epoch gives two records, the second with
+ *     STM = I.
+ * Nothing is recorded for absent measurements, unknown trackers or windows that are not visible; the STM is not reset there either, so
+ * the next record's STM spans back to the previous record.  Per record: nominal_state (for an EKF measurement update, the PRE-update
+ * nominal), state_deviation (EKF: x-hat after a measurement update, zero after a time update; CKF: the deviation, Phi x after a time
+ * update), covariance, and the STM since the previous record (Phi), as KfEstimate holds them; estimate.state() = nominal + deviation
+ * with Cr clamped to [0, 2].  Residuals are not repeated here: the tag leads to prefit / postfit / resid_ratio of nyxb_od_outputs.
+ * Records k >= capacity are dropped; count[i] counts all of them (as nyxb_traj_sink).  1 456 bytes per record. */
+#define NYXB_OD_TAG_TIME_UPDATE (-1)
+/* tag of a measurement-update record: ((k*2 + w)*2 + rejected)*2 + (msr_size - 1), with k the measurement index, w the residual
+ * window (the types w*msr_size .. of the tracker) and rejected 1 for a sigma-rejected window */
+#define NYXB_OD_TAG(k, w, rejected, msr_size) ((((int64_t)(k) * 2 + (w)) * 2 + (rejected)) * 2 + ((msr_size) - 1))
+#define NYXB_OD_TAG_MSR(tag) ((tag) >> 3)
+#define NYXB_OD_TAG_WINDOW(tag) (((tag) >> 2) & 1)
+#define NYXB_OD_TAG_REJECTED(tag) (((tag) >> 1) & 1)
+#define NYXB_OD_TAG_MSR_SIZE(tag) (((tag) & 1) + 1)
+
+typedef struct {
+    int64_t capacity;            /* records kept per filter */
+    int64_t* epoch_ns;           /* [capacity][n] */
+    int64_t* tag;                /* [capacity][n] NYXB_OD_TAG_TIME_UPDATE or NYXB_OD_TAG(..) */
+    double* nominal;             /* [capacity][9][n] [(k*9 + r)*n + i] */
+    double* deviation;           /* [capacity][9][n] */
+    double* covar;               /* [capacity][81][n] (r,c) at [(k*81 + c*9 + r)*n + i] */
+    double* stm;                 /* [capacity][81][n] Phi from the previous record, same layout */
+    int64_t* count;              /* [n] records produced by filter i (kept or not) */
+} nyxb_od_records;
+
+/* Arguments as nyxb_od_ekf_batch, plus the records: every array of *rec non-NULL (the record arrays may be NULL when capacity is 0).
+ * Records a filter does not reach are left as NaN (tag and epoch: -1). */
+int32_t nyxb_od_ekf_record_batch(nyxb_engine* eng, const nyxb_od_config* cfg,
+                                 int32_t n_stations, const nyxb_ground_station* stations,
+                                 const nyxb_tracking_arc* arc, size_t n,
+                                 const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
+                                 const double* covar0_soa, const nyxb_od_outputs* out, const nyxb_od_records* rec);
+
+/* ---- ODSolution::smooth (od/process/solution/smooth.rs:104-249) for n filters in ONE launch, from their records.  As coded, each
+ * estimate k < l (l the last) is smoothed from the FILTER estimate k+1 (not a smoothed one): x_s = Phi^-1 x_{k+1},
+ * P_s = Phi^-1 P_{k+1} Phi^-T, Phi the STM of record k+1, inverted by LU (singular: an exactly zero pivot); the nominal stays record
+ * k's.  The last estimate is copied unchanged.  Outputs, [capacity][..][n] like the records, each NULL to skip, NaN where the
+ * reference has None or a record is past count:
+ *   state     estimate.state() of the smoothed estimate (nominal + deviation, Cr clamped);
+ *   deviation, covar (layout of the records);
+ *   fs_ratio  filter-smoother ratios (state_f - state_s)_q / sqrt((P_f - P_s)_qq), NaN / +-inf kept; NaN for the last estimate;
+ *   postfit   [capacity][2][n]: position k holds the reference's residuals[k+1] recomputed (off by one, as coded): real_obs of
+ *             measurement k+1's window (0 for an absent type) minus measure_instantaneous(smoothed state k) at record k's EPOCH minus
+ *             the station bias, slot = position of the type in the device's list as nyxb_od_outputs; NaN when record k+1 is a time
+ *             update or the smoothed state is not visible.  The last position is the filter's own residual, unchanged: it is
+ *             nyxb_od_outputs.postfit at the last record's tag and is left NaN here.
+ *   status    [n] required: 0, the filter's status when filter_status[i] != 0 (not smoothed), NYXB_ERR_TOO_FEW_MEASUREMENTS for
+ *             fewer than two records (the reference panics), NYXB_ERR_RECORDS_TRUNCATED when count > capacity,
+ *             NYXB_ERR_SINGULAR_STM, or NYXB_ERR_EPHEMERIS; the batch is never aborted, and every output of a filter with a nonzero
+ *             status is NaN.
+ * stations, arc and cfg->msr_size must be those of the filter run (records tagged with another msr_size, or pointing at a measurement
+ * or tracker that is not there, are NYXB_RC_BAD_ARG); of cfg only msr_size is read.  HOST pointers everywhere. */
+typedef struct {
+    double* state;               /* [capacity][9][n] or NULL */
+    double* deviation;           /* [capacity][9][n] or NULL */
+    double* covar;               /* [capacity][81][n] or NULL */
+    double* fs_ratio;            /* [capacity][9][n] or NULL */
+    double* postfit;             /* [capacity][2][n] or NULL */
+    int32_t* status;             /* [n] */
+} nyxb_smooth_outputs;
+
+int32_t nyxb_od_smooth_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations, const nyxb_ground_station* stations,
+                             const nyxb_tracking_arc* arc, size_t n, const nyxb_od_records* rec, const int32_t* filter_status,
+                             nyxb_smooth_outputs* out);
 
 /* ---- Covariance mapping over an ensemble: n independent `KalmanODProcess::predict_until` runs (od/process/mod.rs:440-486) in ONE
  * kernel launch.  Record 0 is the initial estimate; then chunks of cfg->max_step_ns (`for_duration(max_step)`: adaptive steps, the

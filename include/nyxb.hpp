@@ -491,11 +491,28 @@ struct KfEstimate {   // od/estimate/kfestimate.rs: nominal state + 9x9 covarian
 // one tracking schedule, n observation sets: obs[(k*2 + type)*n + i], NaN = type not in the measurement's data
 struct TrackingDataArc { std::vector<int64_t> epoch_ns; std::vector<std::string> tracker; std::vector<double> obs; size_t n = 0; };
 
+class KalmanODProcess;
+
 struct ODSolution {
     size_t n = 0, m = 0;
     std::vector<double> state, covar, state_dev, resid_ratio, prefit, postfit;   // [9][n], [81][n] (c*9+r), [9][n], [m][2][n] x3
     std::vector<int64_t> epoch; std::vector<int32_t> msr_flags, status; std::vector<nyxb_details> details;
+    // every estimate (ODSolution.estimates) when process_arcs ran with an estimates capacity (nyxb_od_records): epoch / tag
+    // [cap][n], nominal / deviation [cap][9][n], covar / stm [cap][81][n] with (r, c) at [(k*81 + c*9 + r)*n + i], count [n]
+    int64_t rec_capacity = 0;
+    std::vector<int64_t> rec_epoch, rec_tag, rec_count;
+    std::vector<double> rec_nominal, rec_deviation, rec_covar, rec_stm;
+    // set by smooth(): smoothed state() / deviation / filter-smoother ratios [cap][9][n], covar [cap][81][n], postfit [cap][2][n]
+    // by estimate position (NaN where the reference has None), and the status of each filter's smoothing
+    Frame frame = EARTH_J2000();   // integration frame of the run
+    bool smoother_run = false;
+    std::vector<double> sm_state, sm_deviation, sm_covar, sm_fs_ratio, sm_postfit;
+    std::vector<int32_t> sm_status;
     Spacecraft final_state(const Spacecraft& tmpl, size_t i) const { return detail::unpack(tmpl, state, epoch, n, i); }
+    int64_t n_estimates(size_t i) const { return rec_count.empty() ? 0 : std::min(rec_count[i], rec_capacity); }
+    bool is_smoother_run() const { return smoother_run; }
+    // ODSolution::smooth (od/process/solution/smooth.rs:104-249) of all n filters in one launch; `odp` and `arc` are those of the run
+    inline ODSolution smooth(const KalmanODProcess& odp, const TrackingDataArc& arc) const;
 };
 
 // Covariance mapping of one estimate (KalmanODProcess::predict_until): record k at epoch0 + k * max_step, k < count
@@ -575,7 +592,9 @@ class KalmanODProcess {
         return predict_until(initial, initial.nominal_state.epoch() + duration);
     }
 
-    ODSolution process_arcs(const std::vector<KfEstimate>& initial, const TrackingDataArc& arc) const {
+    // estimates_capacity >= 0: also record the first estimates_capacity entries of each filter's ODSolution.estimates
+    // (nyxb_od_ekf_record_batch); the filter's outputs are the same bits
+    ODSolution process_arcs(const std::vector<KfEstimate>& initial, const TrackingDataArc& arc, int64_t estimates_capacity = -1) const {
         const size_t n = initial.size(), m = arc.epoch_ns.size();
         if (arc.n != n || arc.obs.size() != m * 2 * n || arc.tracker.size() != m) throw std::runtime_error("arc shape does not match the filters");
         std::vector<Spacecraft> noms; for (auto& e : initial) noms.push_back(e.nominal_state);
@@ -588,16 +607,52 @@ class KalmanODProcess {
         std::vector<int32_t> trk = detail::tracker_index(devices, arc);
         const nyxb_od_config cfg = config();
         nyxb_tracking_arc carc{(int64_t)m, arc.epoch_ns.data(), trk.data(), arc.obs.data()};
-        ODSolution s; s.n = n; s.m = m;
+        ODSolution s; s.n = n; s.m = m; s.frame = frame;
         s.state.resize(9 * n); s.epoch.resize(n); s.covar.resize(81 * n); s.state_dev.resize(9 * n); s.resid_ratio.resize(m * 2 * n); s.prefit.resize(m * 2 * n);
         s.postfit.resize(m * 2 * n); s.msr_flags.resize(m * n); s.details.resize(n); s.status.resize(n);
         nyxb_od_outputs out{s.state.data(), s.epoch.data(), s.covar.data(), s.state_dev.data(), s.resid_ratio.data(), s.prefit.data(), s.postfit.data(),
                             s.msr_flags.data(), nullptr, nullptr, s.details.data(), s.status.data()};
-        if (nyxb_od_ekf_batch(eng.get(), &cfg, (int32_t)st.size(), st.data(), &carc, n, soa.state.data(), soa.consts.data(), soa.epoch.data(), cov0.data(), &out) != NYXB_RC_OK)
-            throw std::runtime_error(std::string("nyxb_od_ekf_batch: ") + nyxb_last_error());
+        if (estimates_capacity < 0) {
+            if (nyxb_od_ekf_batch(eng.get(), &cfg, (int32_t)st.size(), st.data(), &carc, n, soa.state.data(), soa.consts.data(), soa.epoch.data(), cov0.data(), &out) != NYXB_RC_OK)
+                throw std::runtime_error(std::string("nyxb_od_ekf_batch: ") + nyxb_last_error());
+            return s;
+        }
+        const size_t cap = (size_t)estimates_capacity;
+        s.rec_capacity = estimates_capacity;
+        s.rec_epoch.resize(cap * n); s.rec_tag.resize(cap * n); s.rec_count.resize(n);
+        s.rec_nominal.resize(cap * 9 * n); s.rec_deviation.resize(cap * 9 * n); s.rec_covar.resize(cap * 81 * n); s.rec_stm.resize(cap * 81 * n);
+        nyxb_od_records rec{estimates_capacity, s.rec_epoch.data(), s.rec_tag.data(), s.rec_nominal.data(), s.rec_deviation.data(), s.rec_covar.data(),
+                            s.rec_stm.data(), s.rec_count.data()};
+        if (nyxb_od_ekf_record_batch(eng.get(), &cfg, (int32_t)st.size(), st.data(), &carc, n, soa.state.data(), soa.consts.data(), soa.epoch.data(),
+                                     cov0.data(), &out, &rec) != NYXB_RC_OK)
+            throw std::runtime_error(std::string("nyxb_od_ekf_record_batch: ") + nyxb_last_error());
         return s;
     }
 };
+
+inline ODSolution ODSolution::smooth(const KalmanODProcess& odp, const TrackingDataArc& arc) const {
+    if (rec_count.empty()) throw std::runtime_error("no estimate records: run process_arcs(.., estimates_capacity)");
+    if (smoother_run) throw std::runtime_error("already smoothed");
+    // the engine of the filter run (its dynamics and integration frame) supplies the stations' ephemerides
+    const Frame& integ = frame;
+    auto eng = detail::make_engine(odp.prop.dynamics, integ, odp.almanac, odp.prop.method, odp.prop.opts, odp.prop.mode, odp.prop.device);
+    std::vector<nyxb_ground_station> st = detail::pack_stations(odp.devices, integ, odp.almanac);
+    std::vector<int32_t> trk = detail::tracker_index(odp.devices, arc);
+    const nyxb_od_config cfg = odp.config();
+    nyxb_tracking_arc carc{(int64_t)m, arc.epoch_ns.data(), trk.data(), arc.obs.data()};
+    nyxb_od_records rec{rec_capacity, const_cast<int64_t*>(rec_epoch.data()), const_cast<int64_t*>(rec_tag.data()), const_cast<double*>(rec_nominal.data()),
+                        const_cast<double*>(rec_deviation.data()), const_cast<double*>(rec_covar.data()), const_cast<double*>(rec_stm.data()),
+                        const_cast<int64_t*>(rec_count.data())};
+    ODSolution s = *this;
+    const size_t cap = (size_t)rec_capacity;
+    s.smoother_run = true;
+    s.sm_state.resize(cap * 9 * n); s.sm_deviation.resize(cap * 9 * n); s.sm_covar.resize(cap * 81 * n); s.sm_fs_ratio.resize(cap * 9 * n);
+    s.sm_postfit.resize(cap * 2 * n); s.sm_status.resize(n);
+    nyxb_smooth_outputs out{s.sm_state.data(), s.sm_deviation.data(), s.sm_covar.data(), s.sm_fs_ratio.data(), s.sm_postfit.data(), s.sm_status.data()};
+    if (nyxb_od_smooth_batch(eng.get(), &cfg, (int32_t)st.size(), st.data(), &carc, n, &rec, status.data(), &out) != NYXB_RC_OK)
+        throw std::runtime_error(std::string("nyxb_od_smooth_batch: ") + nyxb_last_error());
+    return s;
+}
 
 // BatchLeastSquares (od/blse/mod.rs:30-541) with the reference's builder defaults; estimate / evaluate of one problem through
 // nyxb_od_bls_batch / nyxb_od_bls_evaluate_batch.  A per-problem status is thrown as the reference's ODError.

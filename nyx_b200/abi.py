@@ -160,12 +160,23 @@ class EventC(C.Structure):
 
 
 # ---- orbit determination (SURVEY.md §8 (f)-2): mirrors of nyxb_ground_station / nyxb_od_config / nyxb_tracking_arc / nyxb_od_outputs /
-# nyxb_predict_outputs / nyxb_bls_config / nyxb_bls_outputs
+# nyxb_od_records / nyxb_smooth_outputs / nyxb_predict_outputs / nyxb_bls_config / nyxb_bls_outputs
 MSR_RANGE, MSR_DOPPLER = 0, 1
 KF_REFERENCE_UPDATE, KF_DEVIATION_TRACKING = 0, 1
 MSRF_PROCESSED, MSRF_REJECTED, MSRF_NOT_VISIBLE, MSRF_ABSENT = 1, 2, 4, 8
 BLS_NORMAL_EQUATIONS, BLS_LEVENBERG_MARQUARDT = 0, 1
 ERR_TOO_FEW_MEASUREMENTS, ERR_SINGULAR_INFORMATION, ERR_INVALID_MEASUREMENT = 6, 7, 8
+ERR_SINGULAR_STM, ERR_RECORDS_TRUNCATED = 9, 10
+OD_TAG_TIME_UPDATE = -1   # estimate-record tags: NYXB_OD_TAG(k, w, rejected, msr_size) = ((k*2 + w)*2 + rejected)*2 + msr_size - 1
+
+
+def od_tag(k, window, rejected, msr_size):
+    return ((int(k) * 2 + int(window)) * 2 + int(rejected)) * 2 + int(msr_size) - 1
+
+
+def od_tag_fields(tag):
+    """(measurement index, window, rejected, msr_size) of measurement-update tags (arrays or ints)."""
+    return tag >> 3, (tag >> 2) & 1, (tag >> 1) & 1, (tag & 1) + 1
 
 
 class GroundStationC(C.Structure):
@@ -236,6 +247,30 @@ class PredictOutputsC(C.Structure):
         ("rec_state", C.c_void_p),
         ("rec_covar", C.c_void_p),
         ("rec_count", C.c_void_p),
+    ]
+
+
+class OdRecordsC(C.Structure):
+    _fields_ = [
+        ("capacity", C.c_int64),
+        ("epoch_ns", C.c_void_p),
+        ("tag", C.c_void_p),
+        ("nominal", C.c_void_p),
+        ("deviation", C.c_void_p),
+        ("covar", C.c_void_p),
+        ("stm", C.c_void_p),
+        ("count", C.c_void_p),
+    ]
+
+
+class SmoothOutputsC(C.Structure):
+    _fields_ = [
+        ("state", C.c_void_p),
+        ("deviation", C.c_void_p),
+        ("covar", C.c_void_p),
+        ("fs_ratio", C.c_void_p),
+        ("postfit", C.c_void_p),
+        ("status", C.c_void_p),
     ]
 
 
@@ -341,6 +376,12 @@ def _declare(lib):
     lib.nyxb_od_ekf_batch.restype = C.c_int32
     lib.nyxb_od_ekf_batch.argtypes = [vp, C.POINTER(OdConfigC), C.c_int32, C.POINTER(GroundStationC), C.POINTER(TrackingArcC),
                                       C.c_size_t, vp, vp, vp, vp, C.POINTER(OdOutputsC)]
+    lib.nyxb_od_ekf_record_batch.restype = C.c_int32
+    lib.nyxb_od_ekf_record_batch.argtypes = [vp, C.POINTER(OdConfigC), C.c_int32, C.POINTER(GroundStationC), C.POINTER(TrackingArcC),
+                                             C.c_size_t, vp, vp, vp, vp, C.POINTER(OdOutputsC), C.POINTER(OdRecordsC)]
+    lib.nyxb_od_smooth_batch.restype = C.c_int32
+    lib.nyxb_od_smooth_batch.argtypes = [vp, C.POINTER(OdConfigC), C.c_int32, C.POINTER(GroundStationC), C.POINTER(TrackingArcC),
+                                         C.c_size_t, C.POINTER(OdRecordsC), vp, C.POINTER(SmoothOutputsC)]
     lib.nyxb_od_predict_batch.restype = C.c_int32
     lib.nyxb_od_predict_batch.argtypes = [vp, C.POINTER(OdConfigC), C.c_size_t, vp, vp, vp, vp, vp, vp, C.POINTER(PredictOutputsC)]
     lib.nyxb_od_bls_batch.restype = C.c_int32
@@ -403,6 +444,8 @@ EXPORTED_SYMBOLS = [
     "nyxb_propagate_batch_event",
     "nyxb_propagate_batch_stm",
     "nyxb_od_ekf_batch",
+    "nyxb_od_ekf_record_batch",
+    "nyxb_od_smooth_batch",
     "nyxb_od_predict_batch",
     "nyxb_od_bls_batch",
     "nyxb_od_bls_evaluate_batch",

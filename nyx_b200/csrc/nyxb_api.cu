@@ -27,6 +27,8 @@ extern "C" double nyxb_fp64_probe(int device, int iters);
 extern "C" cudaError_t nyxb_launch_frame_shift(const DevBody*, double, size_t, double*, const long long*, int*, cudaStream_t);
 extern "C" cudaError_t nyxb_launch_od_coop(const DevSetup*, const DevOd*, const int*, size_t, const double*, const double*, const long long*,
                                            double*, long long*, nyxb_details*, int*, cudaStream_t);
+extern "C" cudaError_t nyxb_launch_od_rec_coop(const DevSetup*, const DevOd*, const OdEstRecords*, const int*, size_t, const double*,
+                                               const double*, const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
 extern "C" cudaError_t nyxb_launch_pred_coop(const DevSetup*, const DevOd*, const int*, size_t, const double*, const double*,
                                              const long long*, const long long*, const double*, const OdRecords*, long long*, double*,
                                              long long*, nyxb_details*, int*, cudaStream_t);
@@ -44,6 +46,7 @@ extern "C" cudaError_t nyxb_launch_mvn(unsigned long long, unsigned long long, s
 static_assert(sizeof(nyxb_integ_opts) == 56 && sizeof(nyxb_gravity_field) == 104 && sizeof(nyxb_dynamics) == 96 && sizeof(nyxb_rotation) == 56 && sizeof(nyxb_srp) == 40 && sizeof(nyxb_details) == 48, "ABI layout");
 static_assert(sizeof(nyxb_ground_station) == 176 && sizeof(nyxb_od_config) == 72 && sizeof(nyxb_tracking_arc) == 32 && sizeof(nyxb_od_outputs) == 96, "ABI layout");
 static_assert(sizeof(nyxb_bls_config) == 80 && sizeof(nyxb_bls_outputs) == 72, "ABI layout");
+static_assert(sizeof(nyxb_od_records) == 64 && sizeof(nyxb_smooth_outputs) == 48, "ABI layout");
 
 static thread_local std::string g_err;
 static void set_err(const std::string& s) { g_err = s; }
@@ -888,13 +891,19 @@ extern "C" int32_t nyxb_propagate_batch_stm(nyxb_engine* eng, size_t n, const do
     return NYXB_RC_OK;
 }
 
-extern "C" int32_t nyxb_od_ekf_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations,
-                                     const nyxb_ground_station* stations, const nyxb_tracking_arc* arc, size_t n,
-                                     const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
-                                     const double* covar0_soa, const nyxb_od_outputs* out) {
+namespace {
+// nyxb_od_ekf_batch and nyxb_od_ekf_record_batch: argument checks, packing, one launch, read-back.  rec: null, or the estimate records.
+int32_t od_ekf_run(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations, const nyxb_ground_station* stations,
+                   const nyxb_tracking_arc* arc, size_t n, const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
+                   const double* covar0_soa, const nyxb_od_outputs* out, const nyxb_od_records* rec) {
     if (!eng || !cfg || !arc || !state_soa || !consts_soa || !epoch0_ns || !covar0_soa || !out || !out->state_soa || !out->epoch_ns ||
         !out->covar_soa || !out->status || (n_stations > 0 && !stations) || n_stations < 0) {
         set_err("null argument");
+        return NYXB_RC_BAD_ARG;
+    }
+    if (rec && (rec->capacity < 0 || !rec->count ||
+                (rec->capacity > 0 && (!rec->epoch_ns || !rec->tag || !rec->nominal || !rec->deviation || !rec->covar || !rec->stm)))) {
+        set_err("bad estimate records: count is required, and every record array when capacity > 0");
         return NYXB_RC_BAD_ARG;
     }
     if (!stm_supported(eng)) return NYXB_RC_UNSUPPORTED;
@@ -970,11 +979,43 @@ extern "C" int32_t nyxb_od_ekf_batch(nyxb_engine* eng, const nyxb_od_config* cfg
     if (od.flags) CUDA_TRY(cudaMemsetAsync(od.flags, 0, sizeof(int) * m * n, st));
     if (od.est_state) CUDA_TRY(cudaMemsetAsync(od.est_state, 0xFF, sizeof(double) * m * 9 * n, st));
     if (od.est_cov) CUDA_TRY(cudaMemsetAsync(od.est_cov, 0xFF, sizeof(double) * m * 9 * n, st));
+    OdEstRecords er{};
+    const size_t rcap = rec ? (size_t)rec->capacity : 0;
+    if (rec) {
+        er.cap = (long long)rcap;
+        er.count = B.alloc<long long>(n);
+        if (rcap) {
+            er.epoch = B.alloc<long long>(rcap * n);
+            er.tag = B.alloc<long long>(rcap * n);
+            er.nominal = B.alloc<double>(rcap * 9 * n);
+            er.dev = B.alloc<double>(rcap * 9 * n);
+            er.covar = B.alloc<double>(rcap * 81 * n);
+            er.stm = B.alloc<double>(rcap * 81 * n);
+        }
+        if (!er.count || (rcap && (!er.epoch || !er.tag || !er.nominal || !er.dev || !er.covar || !er.stm))) {
+            set_err("device allocation failed (estimate records)");
+            return NYXB_RC_CUDA;
+        }
+        CUDA_TRY(cudaMemsetAsync(er.count, 0, sizeof(long long) * n, st));
+        if (rcap) {                                  // records a filter does not reach: -1 / NaN
+            CUDA_TRY(cudaMemsetAsync(er.epoch, 0xFF, sizeof(long long) * rcap * n, st));
+            CUDA_TRY(cudaMemsetAsync(er.tag, 0xFF, sizeof(long long) * rcap * n, st));
+            CUDA_TRY(cudaMemsetAsync(er.nominal, 0xFF, sizeof(double) * rcap * 9 * n, st));
+            CUDA_TRY(cudaMemsetAsync(er.dev, 0xFF, sizeof(double) * rcap * 9 * n, st));
+            CUDA_TRY(cudaMemsetAsync(er.covar, 0xFF, sizeof(double) * rcap * 81 * n, st));
+            CUDA_TRY(cudaMemsetAsync(er.stm, 0xFF, sizeof(double) * rcap * 81 * n, st));
+        }
+    }
     const int* d_cols = nullptr;
     if (int32_t rc = od_coop_cols(eng, B, st, d_cols)) return rc;
     const bool coop = d_cols != nullptr;
     CUDA_TRY(cudaEventRecord(eng->ev0, st));
-    cudaError_t err = coop
+    cudaError_t err = rec
+        ? (coop ? nyxb_launch_od_rec_coop(&eng->S, &od, &er, d_cols, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
+                : (eng->mode == NYXB_MODE_STRICT)
+                    ? nyxb_launch_od_rec_strict(&eng->S, &od, &er, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
+                    : nyxb_launch_od_rec_fast(&eng->S, &od, &er, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st))
+        : coop
         ? nyxb_launch_od_coop(&eng->S, &od, d_cols, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
         : (eng->mode == NYXB_MODE_STRICT)
             ? nyxb_launch_od_strict(&eng->S, &od, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
@@ -995,9 +1036,152 @@ extern "C" int32_t nyxb_od_ekf_batch(nyxb_engine* eng, const nyxb_od_config* cfg
     if (od.est_cov) CUDA_TRY(cudaMemcpyAsync(out->est_covar_diag, od.est_cov, sizeof(double) * m * 9 * n, cudaMemcpyDeviceToHost, st));
     if (out->details) CUDA_TRY(cudaMemcpyAsync(out->details, d_det, sizeof(nyxb_details) * n, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(out->status, d_status, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
+    if (rec) {
+        CUDA_TRY(cudaMemcpyAsync(rec->count, er.count, sizeof(long long) * n, cudaMemcpyDeviceToHost, st));
+        if (rcap) {
+            CUDA_TRY(cudaMemcpyAsync(rec->epoch_ns, er.epoch, sizeof(long long) * rcap * n, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(rec->tag, er.tag, sizeof(long long) * rcap * n, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(rec->nominal, er.nominal, sizeof(double) * rcap * 9 * n, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(rec->deviation, er.dev, sizeof(double) * rcap * 9 * n, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(rec->covar, er.covar, sizeof(double) * rcap * 81 * n, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(rec->stm, er.stm, sizeof(double) * rcap * 81 * n, cudaMemcpyDeviceToHost, st));
+        }
+    }
     CUDA_TRY(cudaStreamSynchronize(st));
     float ms = 0.f;
     if (cudaEventElapsedTime(&ms, eng->ev0, eng->ev1) == cudaSuccess) eng->last_ms = ms;
+    return NYXB_RC_OK;
+}
+}  // namespace
+
+extern "C" int32_t nyxb_od_ekf_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations,
+                                     const nyxb_ground_station* stations, const nyxb_tracking_arc* arc, size_t n,
+                                     const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
+                                     const double* covar0_soa, const nyxb_od_outputs* out) {
+    return od_ekf_run(eng, cfg, n_stations, stations, arc, n, state_soa, consts_soa, epoch0_ns, covar0_soa, out, nullptr);
+}
+
+extern "C" int32_t nyxb_od_ekf_record_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations,
+                                            const nyxb_ground_station* stations, const nyxb_tracking_arc* arc, size_t n,
+                                            const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
+                                            const double* covar0_soa, const nyxb_od_outputs* out, const nyxb_od_records* rec) {
+    if (!rec) { set_err("null argument"); return NYXB_RC_BAD_ARG; }
+    return od_ekf_run(eng, cfg, n_stations, stations, arc, n, state_soa, consts_soa, epoch0_ns, covar0_soa, out, rec);
+}
+
+extern "C" int32_t nyxb_od_smooth_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations, const nyxb_ground_station* stations,
+                                        const nyxb_tracking_arc* arc, size_t n, const nyxb_od_records* rec, const int32_t* filter_status,
+                                        nyxb_smooth_outputs* out) {
+    if (!eng || !cfg || !arc || !rec || !filter_status || !out || !out->status || (n_stations > 0 && !stations) || n_stations < 0) {
+        set_err("null argument");
+        return NYXB_RC_BAD_ARG;
+    }
+    if (cfg->msr_size != 1 && cfg->msr_size != 2) { set_err("msr_size must be 1 or 2"); return NYXB_RC_BAD_ARG; }
+    if (rec->capacity < 0 || !rec->count ||
+        (rec->capacity > 0 && (!rec->epoch_ns || !rec->tag || !rec->nominal || !rec->deviation || !rec->covar || !rec->stm))) {
+        set_err("bad estimate records: count is required, and every record array when capacity > 0");
+        return NYXB_RC_BAD_ARG;
+    }
+    if (arc->n_msr < 0 || (arc->n_msr > 0 && (!arc->tracker || !arc->obs))) { set_err("null tracking arc arrays"); return NYXB_RC_BAD_ARG; }
+    for (int32_t s = 0; s < n_stations; ++s) {
+        const nyxb_ground_station& g = stations[s];
+        if (g.n_types < 1 || g.n_types > 2 || (g.body != NYXB_CENTRAL_BODY && (g.body < 0 || g.body >= eng->S.n_bodies))) {
+            set_err("bad ground station descriptor");
+            return NYXB_RC_BAD_ARG;
+        }
+    }
+    const size_t cap = (size_t)rec->capacity;
+    const int M = cfg->msr_size;
+    // per-filter statuses decided on the host; the records of the filters left to smooth must belong to this arc and msr_size
+    std::vector<int> pre(n);
+    for (size_t i = 0; i < n; ++i) {
+        const long long cnt = rec->count[i];
+        pre[i] = filter_status[i] ? filter_status[i]
+               : (cnt > (long long)cap) ? NYXB_ERR_RECORDS_TRUNCATED
+               : (cnt < 2) ? NYXB_ERR_TOO_FEW_MEASUREMENTS : 0;
+        if (pre[i]) continue;
+        for (long long k = 0; k < cnt; ++k) {
+            const int64_t tg = rec->tag[(size_t)k * n + i];
+            if (tg == NYXB_OD_TAG_TIME_UPDATE) continue;
+            const int64_t mk = NYXB_OD_TAG_MSR(tg);
+            const int w = (int)NYXB_OD_TAG_WINDOW(tg);
+            if (tg < 0 || NYXB_OD_TAG_MSR_SIZE(tg) != M) { set_err("estimate records written with another msr_size"); return NYXB_RC_BAD_ARG; }
+            if (mk >= arc->n_msr || arc->tracker[mk] < 0 || arc->tracker[mk] >= n_stations ||
+                (w + 1) * M > stations[arc->tracker[mk]].n_types) {
+                set_err("estimate records do not match this tracking arc");
+                return NYXB_RC_BAD_ARG;
+            }
+        }
+    }
+    for (size_t i = 0; i < n; ++i) out->status[i] = pre[i];
+    if (n == 0 || cap == 0) return NYXB_RC_OK;
+    CUDA_TRY(cudaSetDevice(eng->device));
+    if (!eng->stream) CUDA_TRY(cudaStreamCreateWithFlags(&eng->stream, cudaStreamNonBlocking));
+    cudaStream_t st = eng->stream;
+    const size_t m = (size_t)arc->n_msr;
+    DevBufs B;
+    std::vector<DevStation> hs((size_t)n_stations);
+    for (int32_t s = 0; s < n_stations; ++s) {
+        const nyxb_ground_station& g = stations[s];
+        DevStation& d = hs[s];
+        for (int q = 0; q < 3; ++q) { d.pos[q] = g.pos_fixed_km[q]; d.up[q] = g.up_fixed[q]; }
+        d.mask_deg = g.elevation_mask_deg; d.rot = pack_rot(g.rot); d.body = g.body; d.n_types = g.n_types;
+        for (int q = 0; q < 2; ++q) { d.types[q] = g.types[q]; d.noise_var[q] = g.noise_var[q]; d.bias[q] = g.bias[q]; }
+        d.body_radius = g.body_radius_km;
+    }
+    DevSmooth sm{};
+    sm.msr_size = M;
+    sm.n_stations = n_stations;
+    sm.stations = n_stations ? B.put(hs.data(), hs.size(), st) : nullptr;
+    sm.msr_tracker = m ? B.put((const int*)arc->tracker, m, st) : nullptr;
+    sm.obs = m ? B.put(arc->obs, m * 2 * n, st) : nullptr;
+    sm.cap = (long long)cap;
+    sm.epoch = B.put((const long long*)rec->epoch_ns, cap * n, st);
+    sm.tag = B.put((const long long*)rec->tag, cap * n, st);
+    sm.nominal = B.put(rec->nominal, cap * 9 * n, st);
+    sm.dev = B.put(rec->deviation, cap * 9 * n, st);
+    sm.covar = B.put(rec->covar, cap * 81 * n, st);
+    sm.stm = B.put(rec->stm, cap * 81 * n, st);
+    sm.count = B.put((const long long*)rec->count, n, st);
+    sm.pre_status = B.put(pre.data(), n, st);
+    sm.state = out->state ? B.alloc<double>(cap * 9 * n) : nullptr;
+    sm.sdev = out->deviation ? B.alloc<double>(cap * 9 * n) : nullptr;
+    sm.scov = out->covar ? B.alloc<double>(cap * 81 * n) : nullptr;
+    sm.ratio = out->fs_ratio ? B.alloc<double>(cap * 9 * n) : nullptr;
+    sm.postfit = out->postfit ? B.alloc<double>(cap * 2 * n) : nullptr;
+    sm.err_key = B.alloc<long long>(n);
+    if ((n_stations && !sm.stations) || (m && (!sm.msr_tracker || !sm.obs)) || !sm.epoch || !sm.tag || !sm.nominal || !sm.dev || !sm.covar ||
+        !sm.stm || !sm.count || !sm.pre_status || (out->state && !sm.state) || (out->deviation && !sm.sdev) || (out->covar && !sm.scov) ||
+        (out->fs_ratio && !sm.ratio) || (out->postfit && !sm.postfit) || !sm.err_key) {
+        set_err("device allocation / upload failed");
+        return NYXB_RC_CUDA;
+    }
+    if (sm.state) CUDA_TRY(cudaMemsetAsync(sm.state, 0xFF, sizeof(double) * cap * 9 * n, st));
+    if (sm.sdev) CUDA_TRY(cudaMemsetAsync(sm.sdev, 0xFF, sizeof(double) * cap * 9 * n, st));
+    if (sm.scov) CUDA_TRY(cudaMemsetAsync(sm.scov, 0xFF, sizeof(double) * cap * 81 * n, st));
+    if (sm.ratio) CUDA_TRY(cudaMemsetAsync(sm.ratio, 0xFF, sizeof(double) * cap * 9 * n, st));
+    if (sm.postfit) CUDA_TRY(cudaMemsetAsync(sm.postfit, 0xFF, sizeof(double) * cap * 2 * n, st));
+    CUDA_TRY(cudaMemsetAsync(sm.err_key, 0xFF, sizeof(long long) * n, st));
+    CUDA_TRY(cudaEventRecord(eng->ev0, st));
+    cudaError_t err = nyxb_launch_smooth(&eng->S, &sm, n, st);
+    if (err != cudaSuccess) { set_err(std::string("kernel launch: ") + cudaGetErrorString(err)); return NYXB_RC_CUDA; }
+    eng->launches += 1;
+    eng->last_kernel = NYXB_KERNEL_THREAD;
+    CUDA_TRY(cudaEventRecord(eng->ev1, st));
+    std::vector<long long> key(n);
+    CUDA_TRY(cudaMemcpyAsync(key.data(), sm.err_key, sizeof(long long) * n, cudaMemcpyDeviceToHost, st));
+    if (sm.state) CUDA_TRY(cudaMemcpyAsync(out->state, sm.state, sizeof(double) * cap * 9 * n, cudaMemcpyDeviceToHost, st));
+    if (sm.sdev) CUDA_TRY(cudaMemcpyAsync(out->deviation, sm.sdev, sizeof(double) * cap * 9 * n, cudaMemcpyDeviceToHost, st));
+    if (sm.scov) CUDA_TRY(cudaMemcpyAsync(out->covar, sm.scov, sizeof(double) * cap * 81 * n, cudaMemcpyDeviceToHost, st));
+    if (sm.ratio) CUDA_TRY(cudaMemcpyAsync(out->fs_ratio, sm.ratio, sizeof(double) * cap * 9 * n, cudaMemcpyDeviceToHost, st));
+    if (sm.postfit) CUDA_TRY(cudaMemcpyAsync(out->postfit, sm.postfit, sizeof(double) * cap * 2 * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    float ms = 0.f;
+    if (cudaEventElapsedTime(&ms, eng->ev0, eng->ev1) == cudaSuccess) eng->last_ms = ms;
+    // the reference's error is the first one met going backwards from the last estimate: the largest k (singular before measure);
+    // the outputs of such a filter were set to NaN on the device
+    for (size_t i = 0; i < n; ++i)
+        if (key[i] >= 0) out->status[i] = (key[i] & 1) ? NYXB_ERR_SINGULAR_STM : NYXB_ERR_EPHEMERIS;
     return NYXB_RC_OK;
 }
 

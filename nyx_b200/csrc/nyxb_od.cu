@@ -35,6 +35,8 @@
 #define NYXB_LAUNCH_PRED nyxb_launch_pred_strict
 #define NYXB_KBLS nyxb_k_bls_strict
 #define NYXB_LAUNCH_BLS nyxb_launch_bls_strict
+#define NYXB_KODREC nyxb_k_od_rec_strict
+#define NYXB_LAUNCH_ODREC nyxb_launch_od_rec_strict
 #else
 #define NYXB_KSTM nyxb_k_stm_fast
 #define NYXB_KOD nyxb_k_od_fast
@@ -44,6 +46,8 @@
 #define NYXB_LAUNCH_PRED nyxb_launch_pred_fast
 #define NYXB_KBLS nyxb_k_bls_fast
 #define NYXB_LAUNCH_BLS nyxb_launch_bls_fast
+#define NYXB_KODREC nyxb_k_od_rec_fast
+#define NYXB_LAUNCH_ODREC nyxb_launch_od_rec_fast
 #endif
 
 // ------------------------------------------------------------------------- per-thread backend of nyxb_od_arc.cuh
@@ -116,6 +120,18 @@ NYXB_KOD(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od, s
     od_process_arc(od, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
 }
 
+// the filter with every estimate recorded (ODSolution.estimates, for ODSolution::smooth)
+__global__ void __launch_bounds__(64)
+NYXB_KODREC(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od, const OdEstRecords er, size_t n,
+            const double* __restrict__ state, const double* __restrict__ consts, const long long* __restrict__ epoch0,
+            double* __restrict__ out_state, long long* __restrict__ out_epoch, nyxb_details* __restrict__ out_details,
+            int* __restrict__ out_status) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    ThreadB b(S);
+    od_process_arc<ThreadB, true>(od, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status, &er);
+}
+
 __global__ void __launch_bounds__(64)
 NYXB_KPRED(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od, size_t n, const double* __restrict__ state,
            const double* __restrict__ consts, const long long* __restrict__ epoch0, const long long* __restrict__ end_epoch,
@@ -157,6 +173,16 @@ extern "C" cudaError_t NYXB_LAUNCH_OD(const DevSetup* S, const DevOd* od, size_t
     const int block = 32;  // few, long-running threads: spread them over as many SMs as possible
     unsigned grid = (unsigned)((n + block - 1) / block);
     NYXB_KOD<<<grid, block, 0, stream>>>(*S, *od, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
+    return cudaGetLastError();
+}
+
+extern "C" cudaError_t NYXB_LAUNCH_ODREC(const DevSetup* S, const DevOd* od, const OdEstRecords* er, size_t n, const double* state,
+                                         const double* consts, const long long* epoch0, double* out_state, long long* out_epoch,
+                                         nyxb_details* out_details, int* out_status, cudaStream_t stream) {
+    if (n == 0) return cudaSuccess;
+    const int block = 32;  // as the filter kernel
+    unsigned grid = (unsigned)((n + block - 1) / block);
+    NYXB_KODREC<<<grid, block, 0, stream>>>(*S, *od, *er, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
     return cudaGetLastError();
 }
 

@@ -47,6 +47,46 @@ struct OdRecords {
     double* covar;   // [cap][81][n] or null
 };
 
+// Estimate records of a filter run (nyxb_od_records, include/nyxb.h): one record per entry the reference pushes to
+// ODSolution.estimates, in push order.  Record k of filter i: epoch [k*n + i], tag [k*n + i] (-1: time update, else the measurement,
+// window, rejection and msr_size bits of NYXB_OD_TAG in nyxb.h), nominal state and deviation [(k*9 + r)*n + i], covariance and the STM
+// from the previous record, (r, c) at [(k*81 + c*9 + r)*n + i].  Records k >= cap are dropped; count[i] counts all of them.  Every
+// array is non-null.
+struct OdEstRecords {
+    long long cap;
+    long long* epoch;    // [cap][n]
+    long long* tag;      // [cap][n]
+    double* nominal;     // [cap][9][n]
+    double* dev;         // [cap][9][n]
+    double* covar;       // [cap][81][n]
+    double* stm;         // [cap][81][n]
+    long long* count;    // [n]
+};
+
+// ODSolution::smooth over the records of n filters (nyxb_smooth.cu)
+struct DevSmooth {
+    int msr_size;
+    int n_stations;
+    const DevStation* stations;
+    const int* msr_tracker;        // [m]
+    const double* obs;             // [m][2][n]
+    long long cap;
+    const long long* epoch;        // records, layout of OdEstRecords (nyxb_od.cuh)
+    const long long* tag;
+    const double* nominal;
+    const double* dev;
+    const double* covar;
+    const double* stm;
+    const long long* count;        // [n]
+    const int* pre_status;         // [n] nonzero: filter i is not smoothed (failed filter, too few or truncated records)
+    double* state;                 // [cap][9][n] or null, NaN-filled by the host
+    double* sdev;                  // [cap][9][n] or null
+    double* scov;                  // [cap][81][n] or null
+    double* ratio;                 // [cap][9][n] or null
+    double* postfit;               // [cap][2][n] or null
+    long long* err_key;            // [n] -1, or the largest 2k + (1: singular Phi, 0: ephemeris) among the failing estimates k
+};
+
 // Batch least squares (BatchLeastSquares::estimate / evaluate, od/blse/mod.rs:146-541).  The schedule, stations, observations,
 // max_step and epoch precision come from DevOd; this holds the solver settings and the per-problem outputs ([n], covar [81][n]).
 struct DevBls {
@@ -77,7 +117,12 @@ extern "C" cudaError_t nyxb_launch_pred_strict(const DevSetup*, const DevOd*, si
 extern "C" cudaError_t nyxb_launch_pred_fast(const DevSetup*, const DevOd*, size_t, const double*, const double*, const long long*,
                                              const long long*, const double*, const OdRecords*, long long*, double*, long long*,
                                              nyxb_details*, int*, cudaStream_t);
+extern "C" cudaError_t nyxb_launch_od_rec_strict(const DevSetup*, const DevOd*, const OdEstRecords*, size_t, const double*, const double*,
+                                                 const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
+extern "C" cudaError_t nyxb_launch_od_rec_fast(const DevSetup*, const DevOd*, const OdEstRecords*, size_t, const double*, const double*,
+                                               const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
 extern "C" cudaError_t nyxb_launch_bls_strict(const DevSetup*, const DevOd*, const DevBls*, size_t, const double*, const double*,
                                               const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
 extern "C" cudaError_t nyxb_launch_bls_fast(const DevSetup*, const DevOd*, const DevBls*, size_t, const double*, const double*,
                                             const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
+extern "C" cudaError_t nyxb_launch_smooth(const DevSetup*, const DevSmooth*, size_t, cudaStream_t);

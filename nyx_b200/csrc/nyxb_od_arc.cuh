@@ -263,10 +263,32 @@ __device__ __forceinline__ void od_time_update(const DevOd& od, const OdInst& in
 }
 
 // ------------------------------------------------------------------------- KalmanODProcess::process_arc (od/process/mod.rs:128-497)
-// Loads filter i, runs the whole arc and stores the final covariance, deviation, state, details and status.
+// One estimate record (OdEstRecords, nyxb_od.cuh) at the reference's push points: the nominal state, deviation and covariance of the
+// estimate just formed and the STM since the previous record, before the STM reset.
 template <class B>
+__device__ __forceinline__ void od_est_push(const OdEstRecords& er, long long& cnt, long long tag, const OdInst& in, B& b,
+                                            const typename B::Filt& f, size_t i, size_t n) {
+    const long long k = cnt++;
+    if (k >= er.cap) return;
+    if (b.lead()) { er.epoch[(size_t)k * n + i] = in.epoch_ns; er.tag[(size_t)k * n + i] = tag; }
+    for (int r = b.first(); r < 9; r += B::stride) {
+        er.nominal[((size_t)k * 9 + r) * n + i] = in.y[r];
+        er.dev[((size_t)k * 9 + r) * n + i] = f.xdev[r];
+    }
+    for (int e = b.first(); e < 81; e += B::stride) {
+        const int r = e / 9, c = e - 9 * r;
+        er.covar[((size_t)k * 81 + c * 9 + r) * n + i] = f.P[e];
+        er.stm[((size_t)k * 81 + e) * n + i] = b.phi[e];        // phi is column-major: e = c*9 + r
+    }
+}
+
+// Loads filter i, runs the whole arc and stores the final covariance, deviation, state, details and status.  REC: also write one
+// estimate record per entry of the reference's ODSolution.estimates into *er (null when REC is false); the filter's arithmetic and
+// outputs are the same either way.
+template <class B, bool REC = false>
 __device__ void od_process_arc(const DevOd& od, B& b, size_t i, size_t n, const double* state, const double* consts, const long long* epoch0,
-                               double* out_state, long long* out_epoch, nyxb_details* out_details, int* out_status) {
+                               double* out_state, long long* out_epoch, nyxb_details* out_details, int* out_status,
+                               const OdEstRecords* er = nullptr) {
     const DevSetup& S = b.S;
     OdInst in;
     od_load(S, in, i, n, state, consts, epoch0, nullptr);
@@ -283,6 +305,7 @@ __device__ void od_process_arc(const DevOd& od, B& b, size_t i, size_t n, const 
     int rc = 0;
     const bool ekf = od.variant == NYXB_KF_REFERENCE_UPDATE;
     const int M = od.msr_size;
+    long long nrec = 0;
     for (long long k = 0; k < od.n_msr && rc == 0; ++k) {
         const long long t_k = od.msr_epoch[k];
         const double o[2] = { od.obs[((size_t)k * 2 + 0) * n + i], od.obs[((size_t)k * 2 + 1) * n + i] };
@@ -303,6 +326,7 @@ __device__ void od_process_arc(const DevOd& od, B& b, size_t i, size_t n, const 
             if (gap < 0) gap = -gap;
             if (!(gap < od.eps_ns)) {                                           // :250
                 od_time_update(od, in, prev_epoch, b, f);                       // :417-421
+                if (REC) od_est_push(*er, nrec, -1, in, b, f, i, n);            // push_time_update
                 od_reset_stm(b);
                 continue;
             }
@@ -349,6 +373,7 @@ __device__ void od_process_arc(const DevOd& od, B& b, size_t i, size_t n, const 
                 if (od.reject >= 0.0 && ratio > od.reject) {                    // :169-184
                     od_time_update(od, in, prev_epoch, b, f);
                     flags |= NYXB_MSRF_REJECTED;
+                    if (REC) od_est_push(*er, nrec, ((k * 2 + wno) * 2 + 1) * 2 + (M - 1), in, b, f, i, n);   // push_measurement_update
                 } else {
                     // gain K = PHt S^-1 (Cholesky solve; plain inverse when S is not positive definite)
                     double Si[2][2];
@@ -406,6 +431,7 @@ __device__ void od_process_arc(const DevOd& od, B& b, size_t i, size_t n, const 
                     b.sync();
                     prev_epoch = in.epoch_ns;
                     if (od.postfit && b.lead()) for (int q = 0; q < w.ncur; ++q) od.postfit[((size_t)k * 2 + wno * M + q) * n + i] = post[q];
+                    if (REC) od_est_push(*er, nrec, ((k * 2 + wno) * 2 + 0) * 2 + (M - 1), in, b, f, i, n);   // pre-update nominal, x-hat
                     if (ekf) {                                                  // :364-369 `Spacecraft + OVector<9>`
                         for (int r = 0; r < 9; ++r) in.y[r] = in.y[r] + xhat[r];
                         in.y[6] = in.y[6] < 0.0 ? 0.0 : (in.y[6] > 2.0 ? 2.0 : in.y[6]);
@@ -427,6 +453,7 @@ __device__ void od_process_arc(const DevOd& od, B& b, size_t i, size_t n, const 
         od.covar[(size_t)(c * 9 + r) * n + i] = f.P[e];
     }
     if (od.state_dev) for (int r = b.first(); r < 9; r += B::stride) od.state_dev[(size_t)r * n + i] = f.xdev[r];
+    if (REC && b.lead()) er->count[i] = nrec;
     od_store(b, in, rc, i, n, out_state, out_epoch, out_details, out_status);
 }
 

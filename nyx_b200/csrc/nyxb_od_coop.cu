@@ -252,6 +252,26 @@ nyxb_k_od_coop(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd
     od_process_arc(od, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
 }
 
+// the filter with every estimate recorded (ODSolution.estimates, for ODSolution::smooth), one warp per filter
+__global__ void __launch_bounds__(32 * ODC_WPB)
+nyxb_k_od_rec_coop(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od, const OdEstRecords er, const int* __restrict__ cols,
+                   size_t n, const double* __restrict__ state, const double* __restrict__ consts, const long long* __restrict__ epoch0,
+                   double* __restrict__ out_state, long long* __restrict__ out_epoch, nyxb_details* __restrict__ out_details,
+                   int* __restrict__ out_status) {
+    extern __shared__ __align__(16) unsigned char smem[];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    const size_t i = (size_t)blockIdx.x * ODC_WPB + wib;
+    if (i >= n) return;   // whole warps leave together
+    const int npw = S.has_grav ? 3 * (S.grav.N + 2) : 0;
+    const size_t slab = (sizeof(WarpS) + sizeof(D3) * (size_t)npw + 15) & ~(size_t)15;
+    WarpS& W = *reinterpret_cast<WarpS*>(smem + slab * wib);
+    Ctx cx;
+    cx.S = &S; cx.mycols = cols + lane * ODC_KMAX; cx.W = &W; cx.lane = lane;
+    cx.pw = reinterpret_cast<D3*>(smem + slab * wib + sizeof(WarpS));
+    WarpB b(cx);
+    od_process_arc<WarpB, true>(od, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status, &er);
+}
+
 // covariance prediction (KalmanODProcess::predict_until), one warp per run: same slab and column deal as the filter kernel
 __global__ void __launch_bounds__(32 * ODC_WPB)
 nyxb_k_pred_coop(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od, const int* __restrict__ cols, size_t n,
@@ -311,6 +331,19 @@ extern "C" cudaError_t nyxb_launch_od_coop(const DevSetup* S, const DevOd* od, c
     unsigned grid = (unsigned)((n + ODC_WPB - 1) / ODC_WPB);
     nyxb_k_od_coop<<<grid, 32 * ODC_WPB, smem, stream>>>(*S, *od, cols, n, state, consts, epoch0, out_state, out_epoch, out_details,
                                                          out_status);
+    return cudaGetLastError();
+}
+
+extern "C" cudaError_t nyxb_launch_od_rec_coop(const DevSetup* S, const DevOd* od, const OdEstRecords* er, const int* cols, size_t n,
+                                               const double* state, const double* consts, const long long* epoch0, double* out_state,
+                                               long long* out_epoch, nyxb_details* out_details, int* out_status, cudaStream_t stream) {
+    if (n == 0) return cudaSuccess;
+    const size_t smem = nyxb_od_coop_smem_bytes(S->has_grav ? S->grav.N : 0);
+    cudaError_t e = cudaFuncSetAttribute(nyxb_k_od_rec_coop, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    unsigned grid = (unsigned)((n + ODC_WPB - 1) / ODC_WPB);
+    nyxb_k_od_rec_coop<<<grid, 32 * ODC_WPB, smem, stream>>>(*S, *od, *er, cols, n, state, consts, epoch0, out_state, out_epoch,
+                                                             out_details, out_status);
     return cudaGetLastError();
 }
 

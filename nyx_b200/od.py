@@ -24,7 +24,7 @@ from __future__ import annotations
 
 import enum
 import math
-from dataclasses import dataclass, field
+from dataclasses import dataclass, field, replace
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
@@ -400,6 +400,40 @@ def _cov_units():
     return units
 
 
+def _estimate_columns(epochs, est, cov, tmpl: Spacecraft, fields=None):
+    """The per-estimate columns the OD exports share (export.rs:159-246, 385-446): "Epoch (UTC)", the state parameters of
+    estimate.state() est [9][k], the 45 "Covariance <a>*<b> (<frame>) (<unit>)" entries of cov [k][9][9], "Sigma <item> (<frame>)
+    (<unit>)" and "Sigma <item> (RIC) (<unit>)".  The RIC sigmas follow the as-coded product D C D^T with D = the RIC->inertial state
+    DCM of estimate.state(), its rate block taken as zero (as SpacecraftUncertainty)."""
+    import pyarrow as pa
+
+    from .cosmic import epochs_to_utc_iso
+
+    k = est.shape[1]
+    frame = tmpl.orbit.frame
+    cols = [pa.array(epochs_to_utc_iso(np.asarray(epochs, dtype=np.int64)), type=pa.string())]
+    schema = [pa.field("Epoch (UTC)", pa.string(), nullable=False)]
+    _state_columns(cols, schema, est, tmpl, fields)
+    units = _cov_units()
+    q = 0
+    for a in range(9):
+        for b in range(a, 9):
+            cols.append(pa.array(cov[:, a, b], type=pa.float64()))
+            schema.append(pa.field(f"Covariance {_STATE_ITEMS[a]}*{_STATE_ITEMS[b]} ({frame.name}) ({units[q]})", pa.float64(),
+                                   nullable=False))
+            q += 1
+    _sigma_columns(cols, schema, np.diagonal(cov, axis1=1, axis2=2), frame.name)
+    ric = np.empty((k, 6))
+    for j in range(k):
+        d3 = dcm_ric_to_inertial(Orbit(*[float(v) for v in est[:6, j]], 0, frame))
+        d6 = np.zeros((6, 6))
+        d6[:3, :3] = d3
+        d6[3:, 3:] = d3
+        ric[j] = np.diag(d6 @ cov[j, :6, :6] @ d6.T)
+    _sigma_columns(cols, schema, ric, "RIC")
+    return cols, schema
+
+
 @dataclass
 class ODSolution:
     """Results of n filters: final estimates and the per-measurement residual records (od/process/solution)."""
@@ -419,6 +453,14 @@ class ODSolution:
     templates: Sequence[Spacecraft] = ()
     arc: Optional["TrackingDataArc"] = None
     devices: Optional[Dict[str, GroundStation]] = None
+    # every estimate (ODSolution.estimates) when run with an estimates capacity K: epoch / tag [K][n], nominal / deviation [K][9][n],
+    # covar / stm [K][81][n] ((r, c) at [k][c*9 + r][i]), count [n] (see nyxb_od_records in include/nyxb.h)
+    records: Optional[dict] = None
+    process: Optional["KalmanODProcess"] = None
+    initial_estimates: Optional[Sequence[KfEstimate]] = None
+    # set on the solution smooth() returns: state / deviation / fs_ratio [K][9][n], covar [K][81][n], postfit [K][2][n] by estimate
+    # position, status [n], and the filter's own postfit [m][2][n]
+    smoother: Optional[dict] = None
 
     def accepted(self) -> np.ndarray:
         return ((self.msr_flags & abi.MSRF_PROCESSED) != 0) & ((self.msr_flags & abi.MSRF_REJECTED) == 0)
@@ -430,17 +472,203 @@ class ODSolution:
         sc = self.templates[i].with_vector(int(self.final_epoch_ns[i]), self.final_state_soa[:, i])
         return KfEstimate(sc, self.covar[i].copy(), self.state_deviation[:, i].copy())
 
+    def _to_parquet_estimates(self, path, index, fields, metadata):
+        import pyarrow as pa
+        import pyarrow.parquet as pq
+
+        L = self.n_estimates(index)
+        if L == 0:
+            raise ODError("EmptyDataset: no estimate recorded")
+        tmpl = self.templates[index]
+        ests = [self.estimate(k, index) for k in range(L)]
+        est = np.stack([e.state().to_vector() for e in ests], axis=1)          # [9][L]
+        cov = np.stack([e.covar for e in ests])                                # [L][9][9]
+        cols, schema = _estimate_columns(self.records["epoch"][:L, index], est, cov, tmpl, fields)
+        res = self.residuals(index)
+        M = self.process.msr_size if self.process is not None else 2
+        rec = self.records
+        tracker = [None] * L
+        types = [None] * L
+        for p in range(L):
+            src = p + 1 if (self.smoother is not None and p < L - 1) else p
+            if res[p] is None:
+                continue
+            mk, w, _, _ = abi.od_tag_fields(int(rec["tag"][src, index]))
+            tracker[p] = self.arc.tracker[mk] if self.arc is not None else None
+            dev = (self.devices or {}).get(tracker[p])
+            tl = list(dev.measurement_types) if dev is not None else [MeasurementType.Range, MeasurementType.Doppler]
+            types[p] = [int(t) for t in tl[w * M:(w + 1) * M]]
+        for label, j in (("Prefit residual", 0), ("Postfit residual", 1)):
+            for mt, un in ((MeasurementType.Range, "km"), (MeasurementType.Doppler, "km/s")):
+                v = np.full(L, np.nan)
+                for p in range(L):
+                    if res[p] is not None and int(mt) in types[p]:
+                        v[p] = res[p][j][types[p].index(int(mt))]
+                cols.append(pa.array(v, type=pa.float64(), mask=np.isnan(v)))
+                schema.append(pa.field(f"{label}: {mt.name} ({un})", pa.float64(), nullable=True))
+        ratio = np.array([r[2] if r is not None else np.nan for r in res])
+        cols.append(pa.array(ratio, type=pa.float64(), mask=np.isnan(ratio)))
+        schema.append(pa.field("Residual ratio", pa.float64(), nullable=True))
+        cols.append(pa.array([r[3] if r is not None else None for r in res], type=pa.bool_()))
+        schema.append(pa.field("Residual Rejected", pa.bool_(), nullable=True))
+        cols.append(pa.array(tracker, type=pa.string()))
+        schema.append(pa.field("Tracker", pa.string(), nullable=True))
+        for it in _STATE_ITEMS:                          # the gains are not kept (None on a smoother run, as the reference)
+            for j in range(M):
+                cols.append(pa.nulls(L, type=pa.float64()))
+                schema.append(pa.field(f"Gain {it}*[{j}]", pa.float64(), nullable=True))
+        units = _cov_units()
+        fs = self.filter_smoother_ratios(index)
+        for a in range(9):                               # as coded: the first nine covariance units (export.rs:333-343)
+            v = fs[:, a] if fs is not None else np.full(L, np.nan)
+            mask = np.arange(L) == L - 1 if fs is not None else np.ones(L, dtype=bool)   # a NaN ratio itself is Some(NaN)
+            cols.append(pa.array(v, type=pa.float64(), mask=mask))
+            schema.append(pa.field(f"Filter-smoother ratio {_STATE_ITEMS[a]} ({units[a]})", pa.float64(), nullable=True))
+        meta = {"Purpose": "Orbit determination results"}
+        meta.update(metadata or {})
+        pq.write_table(pa.Table.from_arrays(cols, schema=pa.schema(schema, metadata=meta)), str(path))
+        return path
+
+    # ---- estimates, smoothing and statistics (od/process/solution/{mod,smooth,stats}.rs)
+    def _need_records(self):
+        if self.records is None:
+            raise ODError("no estimate records: run process_arcs(.., estimates_capacity=K)")
+        return self.records
+
+    def n_estimates(self, i: int) -> int:
+        """Number of stored estimates of filter i (the reference's `estimates.len()` when nothing was truncated)."""
+        rec = self._need_records()
+        return int(min(rec["count"][i], rec["epoch"].shape[0]))
+
+    def is_smoother_run(self) -> bool:
+        return self.smoother is not None
+
+    def error(self, i: int) -> Optional[str]:
+        """None, or why filter i (or its smoothing) failed."""
+        st = int(self.smoother["status"][i]) if self.smoother is not None else int(self.status[i])
+        if st == 0:
+            return None
+        names = {abi.ERR_TOO_FEW_MEASUREMENTS: "TooFewMeasurements: fewer than two estimates",
+                 abi.ERR_SINGULAR_STM: "SingularStateTransitionMatrix", abi.ERR_RECORDS_TRUNCATED: "estimate records truncated",
+                 abi.ERR_EPHEMERIS: "epoch outside ephemeris coverage"}
+        return names.get(st, f"status {st}")
+
+    def estimate(self, k: int, i: int) -> KfEstimate:
+        """Estimate k of filter i (smoothed on a smoother run): nominal state, covariance and state deviation."""
+        rec = self._need_records()
+        if not 0 <= k < self.n_estimates(i):
+            raise IndexError(k)
+        src = self.smoother if self.smoother is not None else rec
+        sc = self.templates[i].with_vector(int(rec["epoch"][k, i]), rec["nominal"][k, :, i])
+        return KfEstimate(sc, src["covar"][k, :, i].reshape(9, 9).T.copy(), src["deviation"][k, :, i].copy())
+
+    def filter_smoother_ratios(self, i: int) -> Optional[np.ndarray]:
+        """[k][9] filter-smoother ratios of filter i on a smoother run (the last row, None in the reference, is NaN)."""
+        if self.smoother is None:
+            return None
+        return self.smoother["fs_ratio"][: self.n_estimates(i), :, i].copy()
+
+    def residuals(self, i: int) -> List[Optional[tuple]]:
+        """`self.residuals` of filter i, one entry per estimate: None for a time update (and, smoothed, a successor without residual
+        or an invisible smoothed state), else (prefit[M], postfit[M], ratio, rejected).  On a smoother run position k holds the
+        residual of estimate k+1 with its postfit recomputed at estimate k, and the last position the filter's own (as coded)."""
+        rec = self._need_records()
+        M = self.process.msr_size if self.process is not None else 2
+        L = self.n_estimates(i)
+        filt_post = self.smoother["filter_postfit"] if self.smoother is not None else self.postfit
+        out = []
+        for p in range(L):
+            src = p + 1 if (self.smoother is not None and p < L - 1) else p
+            tag = int(rec["tag"][src, i])
+            if tag < 0:
+                out.append(None)
+                continue
+            mk, w, rej, _ = abi.od_tag_fields(tag)
+            slots = [w * M + q for q in range(M)]
+            if src != p:
+                post = self.smoother["postfit"][p, slots, i]
+                if np.isnan(post).all():
+                    out.append(None)
+                    continue
+            else:
+                post = filt_post[mk, slots, i]
+            out.append((self.prefit[mk, slots, i].copy(), np.array(post), float(self.resid_ratio[mk, w if M == 1 else 0, i]), bool(rej)))
+        return out
+
+    def _rms(self, i, f):
+        res = self.residuals(i)
+        if not res:
+            return float("nan")
+        return float(np.sqrt(sum(f(r) for r in res if r is not None) / len(res)))
+
+    def rms_prefit_residuals(self, i: int = 0) -> float:
+        """stats.rs:148-155: the denominator counts every estimate (time updates too)."""
+        return self._rms(i, lambda r: float(r[0] @ r[0]))
+
+    def rms_postfit_residuals(self, i: int = 0) -> float:
+        """stats.rs:157-164 (a sigma-rejected filter residual has a NaN postfit, as in the reference)."""
+        return self._rms(i, lambda r: float(r[1] @ r[1]))
+
+    def rms_residual_ratios(self, i: int = 0) -> float:
+        """stats.rs:166-173."""
+        return self._rms(i, lambda r: r[2] ** 2)
+
+    def smooth(self) -> "ODSolution":
+        """`ODSolution::smooth` (od/process/solution/smooth.rs:104-249) of all n filters in ONE launch; returns a new solution (the
+        reference consumes `self`) whose estimates are the smoothed ones, with filter-smoother ratios, the smoothed postfit residuals
+        (`residuals(i)`; in the per-measurement `postfit` array, measurement of estimate p >= 1 gets the value of position p - 1, the
+        first estimate's measurement NaN), prefit and ratios kept, no gains.  Needs complete records: when a filter produced more
+        estimates than the capacity, the filters are run once more with a capacity of max(count) first.  Per-filter failures (filter
+        status, fewer than two estimates, singular STM) are in `error(i)`; they never abort the batch."""
+        rec = self._need_records()
+        if self.process is None or self.arc is None:
+            raise ODError("smooth() needs the solution of KalmanODProcess.process_arcs")
+        if self.smoother is not None:
+            raise ODError("already smoothed")
+        cap = rec["epoch"].shape[0]
+        if int(rec["count"].max(initial=0)) > cap:
+            again = self.process.process_arcs(self.initial_estimates, self.arc, record_estimates=self.est_state is not None,
+                                              estimates_capacity=int(rec["count"].max()))
+            return again.smooth()
+        odp = self.process
+        frame = self.templates[0].orbit.frame
+        names, st_c = odp.stations_c(frame)
+        tracker = np.array([names.index(t) if t in names else -1 for t in self.arc.tracker], dtype=np.int32)
+        eng = odp.prop.engine(frame, odp.almanac)
+        sm = eng.od_smooth_batch(odp.config_c(), len(names), st_c, tracker, self.arc.obs, rec, self.status)
+        sm["filter_postfit"] = self.postfit
+        post = np.full(self.postfit.shape, np.nan)
+        M = odp.msr_size
+        for i in range(len(self.status)):
+            if sm["status"][i] != 0:
+                continue
+            for p in range(self.n_estimates(i) - 1):
+                tag = int(rec["tag"][p + 1, i])
+                if tag >= 0:
+                    mk, w, _, _ = abi.od_tag_fields(tag)
+                    post[mk, w * M:(w + 1) * M, i] = sm["postfit"][p, w * M:(w + 1) * M, i]
+        return replace(self, postfit=post, smoother=sm)
+
     def to_parquet(self, path, index: int = 0, fields=None, metadata: Optional[dict] = None):
-        """`ODSolution::to_parquet` (od/process/solution/export.rs:60-688) for filter `index`, one row per processed measurement
-        epoch, with the columns this path records: "Epoch (UTC)", the state parameters of the estimate (default
-        `Spacecraft::export_params`), "Sigma <item> (<frame>) (<unit>)" from the covariance diagonal, prefit / postfit residuals
-        per measurement type, "Residual ratio", "Residual Rejected", "Tracker".  The full covariance, RIC sigmas, gains and
-        filter-smoother ratios of the reference's file need the off-diagonal terms per epoch, which the kernel does not write
-        back.  Needs `process_arcs(.., record_estimates=True)`."""
+        """`ODSolution::to_parquet` (od/process/solution/export.rs:60-688) for filter `index`.
+
+        With estimate records (`process_arcs(.., estimates_capacity=K)`), one row per estimate as export.rs writes it: "Epoch (UTC)",
+        the state parameters of estimate.state(), the 45 covariance entries, the sigmas in the state frame and in RIC (the column code
+        of PredictionSolution.to_parquet), prefit / postfit residuals per measurement type, "Residual ratio", "Residual Rejected",
+        "Tracker" (null for an estimate without residual), the gains (null: not kept) and the filter-smoother ratios (set on a
+        smoother run, null otherwise and on the last estimate).  A smoother run exports the smoothed estimates with their
+        (off-by-one, as coded) residuals.
+
+        Without records, one row per processed measurement epoch from the per-measurement outputs: "Epoch (UTC)", the state
+        parameters of the estimate, "Sigma <item> (<frame>) (<unit>)" from the covariance diagonal, the residuals, ratio, rejection and
+        tracker; that needs `process_arcs(.., record_estimates=True)` and carries no off-diagonal covariance terms."""
         import pyarrow as pa
         import pyarrow.parquet as pq
 
         from .cosmic import epochs_to_utc_iso
+
+        if self.records is not None:
+            return self._to_parquet_estimates(path, index, fields, metadata)
 
         if self.est_state is None or self.est_covar_diag is None or self.arc is None:
             raise ODError("no per-measurement estimates recorded: run process_arcs(.., record_estimates=True)")
@@ -532,37 +760,16 @@ class PredictionSolution:
         import pyarrow as pa
         import pyarrow.parquet as pq
 
-        from .cosmic import epochs_to_utc_iso
-
         if self.rec_state is None or self.rec_covar is None:
             raise ODError("records of both states and covariances are needed: predict with a record capacity")
         k = self.stored(index)
         if k == 0:
             raise ODError("TooFewMeasurements: need 1 estimate to export")
         tmpl = self.templates[index]
-        frame = tmpl.orbit.frame
         est = self.rec_state[:k, :, index].T                                   # [9][k]
         cov = self.rec_covar[:k, :, index].reshape(k, 9, 9).transpose(0, 2, 1)   # [k][r][c]
-        cols = [pa.array(epochs_to_utc_iso(self.record_epochs(index)), type=pa.string())]
-        schema = [pa.field("Epoch (UTC)", pa.string(), nullable=False)]
-        _state_columns(cols, schema, est, tmpl, fields)
+        cols, schema = _estimate_columns(self.record_epochs(index), est, cov, tmpl, fields)
         units = _cov_units()
-        q = 0
-        for a in range(9):
-            for b in range(a, 9):
-                cols.append(pa.array(cov[:, a, b], type=pa.float64()))
-                schema.append(pa.field(f"Covariance {_STATE_ITEMS[a]}*{_STATE_ITEMS[b]} ({frame.name}) ({units[q]})", pa.float64(),
-                                       nullable=False))
-                q += 1
-        _sigma_columns(cols, schema, np.diagonal(cov, axis1=1, axis2=2), frame.name)
-        ric = np.empty((k, 6))
-        for j in range(k):
-            d3 = dcm_ric_to_inertial(Orbit(*[float(v) for v in est[:6, j]], 0, frame))
-            d6 = np.zeros((6, 6))
-            d6[:3, :3] = d3
-            d6[3:, 3:] = d3
-            ric[j] = np.diag(d6 @ cov[j, :6, :6] @ d6.T)
-        _sigma_columns(cols, schema, ric, "RIC")
 
         def nulls(name, typ):
             cols.append(pa.nulls(k, type=typ))
@@ -633,8 +840,12 @@ class KalmanODProcess:
             arr[i] = self.devices[nme].to_c(frame, self.almanac)
         return names, arr
 
-    def process_arcs(self, initial_estimates: Sequence[KfEstimate], arc: TrackingDataArc, record_estimates: bool = False) -> ODSolution:
-        """n independent `process_arc(initial_estimate_i, arc_i)` runs (od/process/mod.rs:128-497) in one launch."""
+    def process_arcs(self, initial_estimates: Sequence[KfEstimate], arc: TrackingDataArc, record_estimates: bool = False,
+                     estimates_capacity: Optional[int] = None) -> ODSolution:
+        """n independent `process_arc(initial_estimate_i, arc_i)` runs (od/process/mod.rs:128-497) in one launch.  With
+        `estimates_capacity` K, the first K entries of each filter's ODSolution.estimates are recorded (1 456 bytes each), which
+        `ODSolution.smooth()`, `residuals`, the RMS statistics and the per-estimate parquet export need; the filter's results do not
+        change."""
         n = len(initial_estimates)
         if arc.n != n:
             raise ODError(f"arc carries {arc.n} observation sets for {n} filters")
@@ -650,11 +861,14 @@ class KalmanODProcess:
         eng = self.prop.engine(frame, self.almanac)
         names, st_c = self.stations_c(frame)
         tracker = np.array([names.index(t) if t in names else -1 for t in arc.tracker], dtype=np.int32)
+        rec_kw = {} if estimates_capacity is None else {"estimates_capacity": estimates_capacity}
         res = eng.od_ekf_batch(self.config_c(), len(names), st_c, arc.epoch_ns, tracker, arc.obs, st, cs, ep, cov0,
-                               record_estimates=record_estimates)
+                               record_estimates=record_estimates, **rec_kw)
         res.templates = [e.nominal_state for e in initial_estimates]
         res.arc = arc
         res.devices = self.devices
+        res.process = self
+        res.initial_estimates = list(initial_estimates)
         return res
 
     def process_arc(self, initial_estimate: KfEstimate, arc: TrackingDataArc) -> ODSolution:

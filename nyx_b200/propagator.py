@@ -340,8 +340,10 @@ class Engine:
         return out_state, out_epoch, out_stm, details, status
 
     def od_ekf_batch(self, cfg_c, n_stations, stations_c, msr_epoch_ns, msr_tracker, obs, state_soa, consts_soa, epoch0_ns,
-                     covar0_soa, record_estimates: bool = False):
-        """`nyxb_od_ekf_batch`: n sequential Kalman filters over one tracking schedule in ONE launch (od/process/mod.rs:128-497)."""
+                     covar0_soa, record_estimates: bool = False, estimates_capacity: Optional[int] = None):
+        """`nyxb_od_ekf_batch`: n sequential Kalman filters over one tracking schedule in ONE launch (od/process/mod.rs:128-497).
+        With `estimates_capacity` K, `nyxb_od_ekf_record_batch` also keeps the first K entries of each filter's ODSolution.estimates
+        (ODSolution.records); the filter's results are the same bits."""
         from .od import ODSolution
 
         state_soa = np.ascontiguousarray(state_soa, dtype=np.float64)
@@ -369,13 +371,46 @@ class Engine:
                              ratio.ctypes.data, prefit.ctypes.data, postfit.ctypes.data, flags.ctypes.data,
                              est_state.ctypes.data if record_estimates else None, est_cov.ctypes.data if record_estimates else None,
                              details.ctypes.data, status.ctypes.data)
-        rc = self._lib.nyxb_od_ekf_batch(self._h, C.byref(cfg_c), int(n_stations), stations_c, C.byref(arc), n,
-                                         state_soa.ctypes.data, consts_soa.ctypes.data, epoch0_ns.ctypes.data,
-                                         covar0_soa.ctypes.data, C.byref(out))
+        records = None
+        if estimates_capacity is None:
+            rc = self._lib.nyxb_od_ekf_batch(self._h, C.byref(cfg_c), int(n_stations), stations_c, C.byref(arc), n,
+                                             state_soa.ctypes.data, consts_soa.ctypes.data, epoch0_ns.ctypes.data,
+                                             covar0_soa.ctypes.data, C.byref(out))
+        else:
+            records, rec_c = _od_records(int(estimates_capacity), n)
+            rc = self._lib.nyxb_od_ekf_record_batch(self._h, C.byref(cfg_c), int(n_stations), stations_c, C.byref(arc), n,
+                                                    state_soa.ctypes.data, consts_soa.ctypes.data, epoch0_ns.ctypes.data,
+                                                    covar0_soa.ctypes.data, C.byref(out), C.byref(rec_c))
         if rc != 0:
             raise PropagationError(f"nyxb_od_ekf_batch rc={rc}: {abi.last_error()}")
         covar = np.ascontiguousarray(out_cov.T.reshape(n, 9, 9).transpose(0, 2, 1))  # (c*9+r) -> [i][r][c]
-        return ODSolution(out_state, out_epoch, covar, out_dev, ratio, prefit, postfit, flags, est_state, est_cov, details, status)
+        return ODSolution(out_state, out_epoch, covar, out_dev, ratio, prefit, postfit, flags, est_state, est_cov, details, status,
+                          records=records)
+
+    def od_smooth_batch(self, cfg_c, n_stations, stations_c, msr_tracker, obs, records: dict, filter_status, outputs=None):
+        """`nyxb_od_smooth_batch`: ODSolution::smooth (od/process/solution/smooth.rs:104-249) of n filters in ONE launch, from their
+        estimate records (dict as ODSolution.records).  `outputs`: the names among state, deviation, covar, fs_ratio, postfit to
+        compute (default all).  Returns a dict of them ([K][..][n], NaN where the reference has None) and status [n]."""
+        msr_tracker = np.ascontiguousarray(msr_tracker, dtype=np.int32)
+        obs = np.ascontiguousarray(obs, dtype=np.float64)
+        filter_status = np.ascontiguousarray(filter_status, dtype=np.int32)
+        cap, n = records["epoch"].shape
+        m = msr_tracker.shape[0]
+        if obs.shape != (m, 2, n) or filter_status.shape != (n,):
+            raise ValueError("expected obs[m][2][n], filter_status[n]")
+        rec_c = abi.OdRecordsC(cap, *(np.ascontiguousarray(records[k]).ctypes.data for k in _REC_KEYS))
+        shapes = {"state": 9, "deviation": 9, "covar": 81, "fs_ratio": 9, "postfit": 2}
+        want = shapes if outputs is None else {k: shapes[k] for k in outputs}
+        r = {k: np.empty((cap, rows, n)) for k, rows in want.items()}
+        r["status"] = np.zeros(n, dtype=np.int32)
+        out = abi.SmoothOutputsC(*(r[k].ctypes.data if k in r else None for k in ("state", "deviation", "covar", "fs_ratio", "postfit")),
+                                 r["status"].ctypes.data)
+        arc = abi.TrackingArcC(m, None, msr_tracker.ctypes.data, obs.ctypes.data)
+        rc = self._lib.nyxb_od_smooth_batch(self._h, C.byref(cfg_c), int(n_stations), stations_c, C.byref(arc), n, C.byref(rec_c),
+                                            filter_status.ctypes.data, C.byref(out))
+        if rc != 0:
+            raise PropagationError(f"nyxb_od_smooth_batch rc={rc}: {abi.last_error()}")
+        return r
 
     def _bls_args(self, msr_epoch_ns, msr_tracker, obs, state_soa, consts_soa, epoch0_ns):
         state_soa = np.ascontiguousarray(state_soa, dtype=np.float64)
@@ -467,6 +502,19 @@ class Engine:
                                                 out_state_ptr, out_epoch_ptr, details_ptr, status_ptr, stream_ptr)
         if rc != 0:
             raise PropagationError(f"nyxb_propagate_batch_dev rc={rc}: {abi.last_error()}")
+
+
+_REC_KEYS = ("epoch", "tag", "nominal", "deviation", "covar", "stm", "count")
+
+
+def _od_records(cap: int, n: int):
+    """Host arrays of nyxb_od_records for `cap` records of n filters, and the struct pointing at them."""
+    if cap < 0:
+        raise ValueError("negative estimates capacity")
+    rec = {"epoch": np.empty((cap, n), dtype=np.int64), "tag": np.empty((cap, n), dtype=np.int64), "nominal": np.empty((cap, 9, n)),
+           "deviation": np.empty((cap, 9, n)), "covar": np.empty((cap, 81, n)), "stm": np.empty((cap, 81, n)),
+           "count": np.zeros(n, dtype=np.int64)}
+    return rec, abi.OdRecordsC(cap, *(rec[k].ctypes.data for k in _REC_KEYS))
 
 
 @dataclass
