@@ -37,7 +37,8 @@ extern "C" {
 #define NYXB_ABI_VERSION 4 /* 4: nyxb_engine_set_kernel / nyxb_engine_last_kernel / nyxb_engine_set_tx_tuning, nyxb_tx_table_dump, nyxb_propagate_batch_multi, nyxb_reference_normals;
                               nyxb_integ_opts.state_center, nyxb_gravity_field.body, nyxb_dynamics.n_gravity / n_point_masses / point_mass_order; nyxb_od_predict_batch
                               and nyxb_predict_outputs, then nyxb_od_bls_batch, nyxb_od_bls_evaluate_batch, nyxb_bls_config, nyxb_bls_outputs and
-                              the status codes 6-8, then nyxb_od_records, nyxb_od_ekf_record_batch, nyxb_smooth_outputs, nyxb_od_smooth_batch
+                              the status codes 6-8, then nyxb_od_records, nyxb_od_ekf_record_batch, nyxb_smooth_outputs, nyxb_od_smooth_batch,
+                              then NYXB_MSR_X/Y/Z, nyxb_position_device, nyxb_position_arc, nyxb_od_position_batch, nyxb_od_position_smooth_batch
                               and the status codes 9-10 were added later without a bump (a pure addition: no existing type or entry point changed).  Earlier: 2: nyxb_srp gained `estimate`; STM, filter and dispersion entry points.  3: nyxb_traj_resample[_dev], nyxb_event_locate[_dev] */
 
 /* ---- IntegratorMethod — propagators/rk_methods/mod.rs:65-79 (same order) ---- */
@@ -400,7 +401,8 @@ int32_t nyxb_propagate_batch_stm(nyxb_engine* eng, size_t n,
  * n independent `KalmanODProcess::process_arc` runs (od/process/mod.rs:128-497) — propagate the nominal state + STM
  * to each measurement, `KalmanFilter::time_update` / `measurement_update` (od/kalman/filtering.rs:59-316), state
  * replacement (EKF) and STM reset — in ONE kernel launch, one filter per trajectory. */
-enum nyxb_msr_type { NYXB_MSR_RANGE = 0, NYXB_MSR_DOPPLER = 1 };  /* od/msr/types.rs:31-45 (the two-way capable ones) */
+enum nyxb_msr_type { NYXB_MSR_RANGE = 0, NYXB_MSR_DOPPLER = 1,   /* od/msr/types.rs:31-45 (the two-way capable ones) */
+                     NYXB_MSR_X = 6, NYXB_MSR_Y = 7, NYXB_MSR_Z = 8 }; /* position fixes (nyxb_position_device) */
 
 /* GroundStation (od/ground_station/mod.rs:47-75) reduced to what the filter needs.  The host converts latitude /
  * longitude / height into the body-fixed position and the local zenith (anise `Orbit::try_latlongalt`); the tracker's
@@ -550,6 +552,62 @@ typedef struct {
 int32_t nyxb_od_smooth_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations, const nyxb_ground_station* stations,
                              const nyxb_tracking_arc* arc, size_t n, const nyxb_od_records* rec, const int32_t* filter_status,
                              nyxb_smooth_outputs* out);
+
+/* ---- Position-fix orbit determination (od/position: PositionDevice, GNSS-style X, Y, Z fixes of the spacecraft position in the
+ * INTEGRATION frame of the estimate): the filter of nyxb_od_ekf_batch with a position device in place of the ground station.  As coded
+ * in the reference:
+ *   - the computed observation of the type at list position ii is component ii of the nominal position (trk_device.rs:76-83), the
+ *     bias added by measure() and subtracted again (process/mod.rs:324-333): the bias cancels, so a bias in the data stays in the
+ *     prefit;
+ *   - H puts the type's unit row at its OWN component, X -> 0, Y -> 1, Z -> 2 (position/sensitivity.rs:55-75): a device listed
+ *     [Y, X, Z] has an H that disagrees with its computed observation;
+ *   - H starts from zeros: a window slot without a type, or with a type absent from the fix, keeps a zero row, its real observation
+ *     is 0 and R keeps the type's variance (so its prefit is minus the computed observation);
+ *   - windows follow process/mod.rs:270-296: msr_size 3 one window, msr_size 1 one per type (the 2nd and 3rd with Phi = I), msr_size 2
+ *     with three types [t0, t1] then [t2] with a zero row and a zero R entry: S is singular and so is R, SingularNoiseRk
+ *     (NYXB_ERR_PROP_MATH) at the first fix;
+ *   - a zero variance gives SingularNoiseRk; there is no visibility test.
+ * msr_size 3: the residual ratio from the Cholesky factor of S (falling back to that of R), the gain from the Cholesky solve
+ * S K^T = (P H^T)^T (falling back to the closed-form 3x3 inverse); msr_size 1 and 2 take the ground station's arithmetic. */
+typedef struct {
+    int32_t n_types;             /* 1 to 3 */
+    int32_t types[3];            /* NYXB_MSR_X / _Y / _Z, distinct, in the device's list order */
+    double noise_var[3];         /* km^2, per list position */
+    double bias[3];              /* km, per list position (cancels in the computed observation) */
+} nyxb_position_device;
+
+/* obs[(k*3 + t - NYXB_MSR_X)*n + i]: the fix component of type t of filter i at measurement k; NaN = the type is not in `msr.data`
+ * (all three NaN: the measurement is not in filter i's arc). */
+typedef struct {
+    int64_t n_msr;
+    const int64_t* epoch_ns;     /* [n_msr] ascending */
+    const int32_t* tracker;      /* [n_msr] index into devices; < 0: unknown tracker */
+    const double* obs;           /* [n_msr][3][n] */
+} nyxb_position_arc;
+
+/* Record tags of the position filter: window 0..2 and msr_size 1..3 (NYXB_OD_TAG has one bit for each) */
+#define NYXB_OD_POS_TAG(k, w, rejected, msr_size) ((((int64_t)(k) * 4 + (w)) * 2 + (rejected)) * 4 + ((msr_size) - 1))
+#define NYXB_OD_POS_TAG_MSR(tag) ((tag) >> 5)
+#define NYXB_OD_POS_TAG_WINDOW(tag) (((tag) >> 3) & 3)
+#define NYXB_OD_POS_TAG_REJECTED(tag) (((tag) >> 2) & 1)
+#define NYXB_OD_POS_TAG_MSR_SIZE(tag) (((tag) & 3) + 1)
+
+/* n filters over one schedule of fixes.  cfg as nyxb_od_ekf_batch with msr_size 1, 2 or 3.  out: nyxb_od_outputs whose per-measurement
+ * arrays resid_ratio, prefit and postfit are [n_msr][3][n] (slot = position of the type in the device's list; the ratio of msr_size 1
+ * in slot w, else slot 0).  rec: NULL, or the estimate records of nyxb_od_ekf_record_batch tagged by NYXB_OD_POS_TAG; `out` is
+ * bit-identical either way.  NYXB_RC_BAD_ARG: a type other than X, Y, Z, a duplicate type, n_types outside 1..3, msr_size outside 1..3,
+ * a NULL required pointer; NYXB_RC_UNSUPPORTED: the setups nyxb_propagate_batch_stm rejects.  Per-filter failures are statuses.
+ * Kernel family as nyxb_od_ekf_batch.  HOST pointers everywhere. */
+int32_t nyxb_od_position_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_devices, const nyxb_position_device* devices,
+                               const nyxb_position_arc* arc, size_t n, const double* state_soa, const double* consts_soa,
+                               const int64_t* epoch0_ns, const double* covar0_soa, const nyxb_od_outputs* out,
+                               const nyxb_od_records* rec);
+
+/* ODSolution::smooth of position filters: the contract of nyxb_od_smooth_batch, with the records of nyxb_od_position_batch, and
+ * out->postfit [capacity][3][n] recomputed through the position device (bias cancelling as in the filter). */
+int32_t nyxb_od_position_smooth_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_devices, const nyxb_position_device* devices,
+                                      const nyxb_position_arc* arc, size_t n, const nyxb_od_records* rec, const int32_t* filter_status,
+                                      nyxb_smooth_outputs* out);
 
 /* ---- Covariance mapping over an ensemble: n independent `KalmanODProcess::predict_until` runs (od/process/mod.rs:440-486) in ONE
  * kernel launch.  Record 0 is the initial estimate; then chunks of cfg->max_step_ns (`for_duration(max_step)`: adaptive steps, the

@@ -434,7 +434,8 @@ class MonteCarlo {
 // ---------------------------------------------------------------------------------------------------------------------
 // Orbit determination (SURVEY.md §8 (f)-2): n sequential Kalman filters over one tracking schedule in ONE launch.
 // ---------------------------------------------------------------------------------------------------------------------
-enum class MeasurementType : int32_t { Range = NYXB_MSR_RANGE, Doppler = NYXB_MSR_DOPPLER };          // od/msr/types.rs:31-45
+enum class MeasurementType : int32_t { Range = NYXB_MSR_RANGE, Doppler = NYXB_MSR_DOPPLER,           // od/msr/types.rs:31-45
+                                       X = NYXB_MSR_X, Y = NYXB_MSR_Y, Z = NYXB_MSR_Z };              // position fixes
 enum class KalmanVariant : int32_t { ReferenceUpdate = NYXB_KF_REFERENCE_UPDATE, DeviationTracking = NYXB_KF_DEVIATION_TRACKING };
 struct StochasticNoise { double sigma = 0.0, bias_constant = 0.0; double covariance() const { return sigma * sigma; } };
 struct SigmaRejection { double num_sigmas = 3.0; };                                                        // process/rejectcrit.rs:35-46
@@ -488,14 +489,35 @@ struct KfEstimate {   // od/estimate/kfestimate.rs: nominal state + 9x9 covarian
     static KfEstimate from_diag(const Spacecraft& s, const double (&d)[9]) { KfEstimate e; e.nominal_state = s; for (int i = 0; i < 9; ++i) e.covar[i * 9 + i] = d[i]; return e; }
 };
 
-// one tracking schedule, n observation sets: obs[(k*2 + type)*n + i], NaN = type not in the measurement's data
-struct TrackingDataArc { std::vector<int64_t> epoch_ns; std::vector<std::string> tracker; std::vector<double> obs; size_t n = 0; };
+// one tracking schedule, n observation sets: obs[(k*ns + slot)*n + i], NaN = type not in the measurement's data; ns = 2 (slot =
+// Range / Doppler) for ground stations, 3 (slot = type - X) for position fixes
+struct TrackingDataArc { std::vector<int64_t> epoch_ns; std::vector<std::string> tracker; std::vector<double> obs; size_t n = 0; size_t ns = 2; };
+
+// PositionDevice (od/position/mod.rs): X / Y / Z fixes of the position in the integration frame; with_noise appends the type to the
+// device's list, as the reference builds it (the filter measures the component at the LIST position, H follows the type: nyxb.h)
+struct PositionDevice {
+    std::string name;
+    std::vector<MeasurementType> measurement_types;
+    std::vector<StochasticNoise> noises;   // per list position
+    PositionDevice& with_noise(MeasurementType t, StochasticNoise nz) {
+        for (size_t q = 0; q < measurement_types.size(); ++q) if (measurement_types[q] == t) { noises[q] = nz; return *this; }
+        measurement_types.push_back(t); noises.push_back(nz); return *this;
+    }
+    nyxb_position_device to_c() const {
+        if (measurement_types.empty() || measurement_types.size() > 3) throw std::runtime_error("a position device carries one to three types");
+        nyxb_position_device d{};
+        d.n_types = (int32_t)measurement_types.size();
+        for (int q = 0; q < d.n_types; ++q) { d.types[q] = (int32_t)measurement_types[q]; d.noise_var[q] = noises[q].covariance(); d.bias[q] = noises[q].bias_constant; }
+        return d;
+    }
+};
 
 class KalmanODProcess;
+class PositionKalmanODProcess;
 
 struct ODSolution {
-    size_t n = 0, m = 0;
-    std::vector<double> state, covar, state_dev, resid_ratio, prefit, postfit;   // [9][n], [81][n] (c*9+r), [9][n], [m][2][n] x3
+    size_t n = 0, m = 0, ns = 2;   // ns: observation slots, 2 (ground stations) or 3 (position fixes)
+    std::vector<double> state, covar, state_dev, resid_ratio, prefit, postfit;   // [9][n], [81][n] (c*9+r), [9][n], [m][ns][n] x3
     std::vector<int64_t> epoch; std::vector<int32_t> msr_flags, status; std::vector<nyxb_details> details;
     // every estimate (ODSolution.estimates) when process_arcs ran with an estimates capacity (nyxb_od_records): epoch / tag
     // [cap][n], nominal / deviation [cap][9][n], covar / stm [cap][81][n] with (r, c) at [(k*81 + c*9 + r)*n + i], count [n]
@@ -513,6 +535,8 @@ struct ODSolution {
     bool is_smoother_run() const { return smoother_run; }
     // ODSolution::smooth (od/process/solution/smooth.rs:104-249) of all n filters in one launch; `odp` and `arc` are those of the run
     inline ODSolution smooth(const KalmanODProcess& odp, const TrackingDataArc& arc) const;
+    // the same for position fixes (nyxb_od_position_smooth_batch; sm_postfit [cap][3][n])
+    inline ODSolution smooth(const PositionKalmanODProcess& odp, const TrackingDataArc& arc) const;
 };
 
 // Covariance mapping of one estimate (KalmanODProcess::predict_until): record k at epoch0 + k * max_step, k < count
@@ -526,6 +550,14 @@ struct PredictionSolution {
 };
 
 namespace detail {
+inline nyxb_od_config od_config(KalmanVariant variant, const std::optional<SigmaRejection>& rej, const std::optional<ProcessNoise3D>& snc,
+                                int64_t max_step, int64_t epoch_precision, int32_t msr_size) {
+    nyxb_od_config cfg{};
+    cfg.variant = (int32_t)variant; cfg.msr_size = msr_size; cfg.reject_num_sigmas = rej ? rej->num_sigmas : -1.0;
+    cfg.max_step_ns = max_step; cfg.epoch_precision_ns = epoch_precision;
+    if (snc) { cfg.snc_enabled = 1; cfg.snc_frame = snc->ric ? 1 : 0; for (int i = 0; i < 3; ++i) cfg.snc_diag[i] = snc->diag[i]; cfg.snc_disable_time_ns = snc->disable_time; }
+    return cfg;
+}
 // the devices as nyxb_ground_station, in order; a station on another body than the integration centre needs its ephemeris
 inline std::vector<nyxb_ground_station> pack_stations(const std::vector<GroundStation>& devices, const Frame& frame, const Almanac* almanac) {
     std::vector<nyxb_ground_station> st;
@@ -559,13 +591,7 @@ class KalmanODProcess {
         : prop(std::move(p)), variant(v), sigma_reject(rej), devices(std::move(dev)), almanac(alm), msr_size(msr) {}
     KalmanODProcess& with_process_noise(ProcessNoise3D snc) { process_noise = snc; return *this; }
 
-    nyxb_od_config config() const {
-        nyxb_od_config cfg{};
-        cfg.variant = (int32_t)variant; cfg.msr_size = msr_size; cfg.reject_num_sigmas = sigma_reject ? sigma_reject->num_sigmas : -1.0;
-        cfg.max_step_ns = max_step; cfg.epoch_precision_ns = epoch_precision;
-        if (process_noise) { cfg.snc_enabled = 1; cfg.snc_frame = process_noise->ric ? 1 : 0; for (int i = 0; i < 3; ++i) cfg.snc_diag[i] = process_noise->diag[i]; cfg.snc_disable_time_ns = process_noise->disable_time; }
-        return cfg;
-    }
+    nyxb_od_config config() const { return detail::od_config(variant, sigma_reject, process_noise, max_step, epoch_precision, msr_size); }
 
     // KalmanODProcess::predict_until / predict_for (od/process/mod.rs:440-496): every record of the time updates
     PredictionSolution predict_until(const KfEstimate& initial, int64_t end_epoch) const {
@@ -651,6 +677,80 @@ inline ODSolution ODSolution::smooth(const KalmanODProcess& odp, const TrackingD
     nyxb_smooth_outputs out{s.sm_state.data(), s.sm_deviation.data(), s.sm_covar.data(), s.sm_fs_ratio.data(), s.sm_postfit.data(), s.sm_status.data()};
     if (nyxb_od_smooth_batch(eng.get(), &cfg, (int32_t)st.size(), st.data(), &carc, n, &rec, status.data(), &out) != NYXB_RC_OK)
         throw std::runtime_error(std::string("nyxb_od_smooth_batch: ") + nyxb_last_error());
+    return s;
+}
+
+// KalmanODProcess<.., PositionDevice> (od/process/mod.rs:128-497 with od/position): the filter over position fixes, msr_size 1 to 3
+class PositionKalmanODProcess {
+  public:
+    Propagator prop; KalmanVariant variant; std::optional<SigmaRejection> sigma_reject; std::vector<PositionDevice> devices;
+    const Almanac* almanac = nullptr; std::optional<ProcessNoise3D> process_noise;
+    int64_t max_step = 60 * NS_PER_S, epoch_precision = 1000; int32_t msr_size = 3;
+    PositionKalmanODProcess(Propagator p, KalmanVariant v, std::optional<SigmaRejection> rej, std::vector<PositionDevice> dev, int32_t msr = 3)
+        : prop(std::move(p)), variant(v), sigma_reject(rej), devices(std::move(dev)), msr_size(msr) {}
+    PositionKalmanODProcess& with_process_noise(ProcessNoise3D snc) { process_noise = snc; return *this; }
+    nyxb_od_config config() const { return detail::od_config(variant, sigma_reject, process_noise, max_step, epoch_precision, msr_size); }
+    std::vector<nyxb_position_device> devices_c() const { std::vector<nyxb_position_device> d; for (auto& x : devices) d.push_back(x.to_c()); return d; }
+    std::vector<int32_t> tracker_index(const TrackingDataArc& arc) const {
+        std::vector<int32_t> trk(arc.epoch_ns.size());
+        for (size_t k = 0; k < trk.size(); ++k) { trk[k] = -1; for (size_t j = 0; j < devices.size(); ++j) if (devices[j].name == arc.tracker[k]) trk[k] = (int32_t)j; }
+        return trk;
+    }
+
+    // arc.ns must be 3; estimates_capacity >= 0 also records the estimates (tags NYXB_OD_POS_TAG), with the same filter outputs
+    ODSolution process_arcs(const std::vector<KfEstimate>& initial, const TrackingDataArc& arc, int64_t estimates_capacity = -1) const {
+        const size_t n = initial.size(), m = arc.epoch_ns.size();
+        if (arc.ns != 3 || arc.n != n || arc.obs.size() != m * 3 * n || arc.tracker.size() != m) throw std::runtime_error("arc shape does not match the filters");
+        std::vector<Spacecraft> noms; for (auto& e : initial) noms.push_back(e.nominal_state);
+        const Frame& frame = noms.at(0).frame;
+        auto eng = detail::make_engine(prop.dynamics, frame, almanac, prop.method, prop.opts, prop.mode, prop.device);
+        detail::Soa soa(noms);
+        std::vector<double> cov0(81 * n);
+        for (size_t i = 0; i < n; ++i) for (int r = 0; r < 9; ++r) for (int c = 0; c < 9; ++c) cov0[(size_t)(c * 9 + r) * n + i] = initial[i].covar[r * 9 + c];
+        const std::vector<nyxb_position_device> dev = devices_c();
+        std::vector<int32_t> trk = tracker_index(arc);
+        const nyxb_od_config cfg = config();
+        nyxb_position_arc carc{(int64_t)m, arc.epoch_ns.data(), trk.data(), arc.obs.data()};
+        ODSolution s; s.n = n; s.m = m; s.ns = 3; s.frame = frame;
+        s.state.resize(9 * n); s.epoch.resize(n); s.covar.resize(81 * n); s.state_dev.resize(9 * n); s.resid_ratio.resize(m * 3 * n); s.prefit.resize(m * 3 * n);
+        s.postfit.resize(m * 3 * n); s.msr_flags.resize(m * n); s.details.resize(n); s.status.resize(n);
+        nyxb_od_outputs out{s.state.data(), s.epoch.data(), s.covar.data(), s.state_dev.data(), s.resid_ratio.data(), s.prefit.data(), s.postfit.data(),
+                            s.msr_flags.data(), nullptr, nullptr, s.details.data(), s.status.data()};
+        nyxb_od_records rec{};
+        if (estimates_capacity >= 0) {
+            const size_t cap = (size_t)estimates_capacity;
+            s.rec_capacity = estimates_capacity;
+            s.rec_epoch.resize(cap * n); s.rec_tag.resize(cap * n); s.rec_count.resize(n);
+            s.rec_nominal.resize(cap * 9 * n); s.rec_deviation.resize(cap * 9 * n); s.rec_covar.resize(cap * 81 * n); s.rec_stm.resize(cap * 81 * n);
+            rec = nyxb_od_records{estimates_capacity, s.rec_epoch.data(), s.rec_tag.data(), s.rec_nominal.data(), s.rec_deviation.data(), s.rec_covar.data(),
+                                  s.rec_stm.data(), s.rec_count.data()};
+        }
+        if (nyxb_od_position_batch(eng.get(), &cfg, (int32_t)dev.size(), dev.data(), &carc, n, soa.state.data(), soa.consts.data(), soa.epoch.data(),
+                                   cov0.data(), &out, estimates_capacity >= 0 ? &rec : nullptr) != NYXB_RC_OK)
+            throw std::runtime_error(std::string("nyxb_od_position_batch: ") + nyxb_last_error());
+        return s;
+    }
+};
+
+inline ODSolution ODSolution::smooth(const PositionKalmanODProcess& odp, const TrackingDataArc& arc) const {
+    if (rec_count.empty()) throw std::runtime_error("no estimate records: run process_arcs(.., estimates_capacity)");
+    if (smoother_run) throw std::runtime_error("already smoothed");
+    auto eng = detail::make_engine(odp.prop.dynamics, frame, odp.almanac, odp.prop.method, odp.prop.opts, odp.prop.mode, odp.prop.device);
+    const std::vector<nyxb_position_device> dev = odp.devices_c();
+    std::vector<int32_t> trk = odp.tracker_index(arc);
+    const nyxb_od_config cfg = odp.config();
+    nyxb_position_arc carc{(int64_t)m, arc.epoch_ns.data(), trk.data(), arc.obs.data()};
+    nyxb_od_records rec{rec_capacity, const_cast<int64_t*>(rec_epoch.data()), const_cast<int64_t*>(rec_tag.data()), const_cast<double*>(rec_nominal.data()),
+                        const_cast<double*>(rec_deviation.data()), const_cast<double*>(rec_covar.data()), const_cast<double*>(rec_stm.data()),
+                        const_cast<int64_t*>(rec_count.data())};
+    ODSolution s = *this;
+    const size_t cap = (size_t)rec_capacity;
+    s.smoother_run = true;
+    s.sm_state.resize(cap * 9 * n); s.sm_deviation.resize(cap * 9 * n); s.sm_covar.resize(cap * 81 * n); s.sm_fs_ratio.resize(cap * 9 * n);
+    s.sm_postfit.resize(cap * 3 * n); s.sm_status.resize(n);
+    nyxb_smooth_outputs out{s.sm_state.data(), s.sm_deviation.data(), s.sm_covar.data(), s.sm_fs_ratio.data(), s.sm_postfit.data(), s.sm_status.data()};
+    if (nyxb_od_position_smooth_batch(eng.get(), &cfg, (int32_t)dev.size(), dev.data(), &carc, n, &rec, status.data(), &out) != NYXB_RC_OK)
+        throw std::runtime_error(std::string("nyxb_od_position_smooth_batch: ") + nyxb_last_error());
     return s;
 }
 

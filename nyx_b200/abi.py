@@ -162,6 +162,7 @@ class EventC(C.Structure):
 # ---- orbit determination (SURVEY.md §8 (f)-2): mirrors of nyxb_ground_station / nyxb_od_config / nyxb_tracking_arc / nyxb_od_outputs /
 # nyxb_od_records / nyxb_smooth_outputs / nyxb_predict_outputs / nyxb_bls_config / nyxb_bls_outputs
 MSR_RANGE, MSR_DOPPLER = 0, 1
+MSR_X, MSR_Y, MSR_Z = 6, 7, 8      # position fixes (nyxb_position_device)
 KF_REFERENCE_UPDATE, KF_DEVIATION_TRACKING = 0, 1
 MSRF_PROCESSED, MSRF_REJECTED, MSRF_NOT_VISIBLE, MSRF_ABSENT = 1, 2, 4, 8
 BLS_NORMAL_EQUATIONS, BLS_LEVENBERG_MARQUARDT = 0, 1
@@ -172,6 +173,15 @@ OD_TAG_TIME_UPDATE = -1   # estimate-record tags: NYXB_OD_TAG(k, w, rejected, ms
 
 def od_tag(k, window, rejected, msr_size):
     return ((int(k) * 2 + int(window)) * 2 + int(rejected)) * 2 + int(msr_size) - 1
+
+
+def od_pos_tag(k, window, rejected, msr_size):
+    """NYXB_OD_POS_TAG: the record tag of the position-fix filter (window 0..2, msr_size 1..3)."""
+    return ((int(k) * 4 + int(window)) * 2 + int(rejected)) * 4 + int(msr_size) - 1
+
+
+def od_pos_tag_fields(tag):
+    return tag >> 5, (tag >> 3) & 3, (tag >> 2) & 1, (tag & 3) + 1
 
 
 def od_tag_fields(tag):
@@ -192,6 +202,24 @@ class GroundStationC(C.Structure):
         ("noise_var", C.c_double * 2),
         ("bias", C.c_double * 2),
         ("body_radius_km", C.c_double),
+    ]
+
+
+class PositionDeviceC(C.Structure):
+    _fields_ = [
+        ("n_types", C.c_int32),
+        ("types", C.c_int32 * 3),
+        ("noise_var", C.c_double * 3),
+        ("bias", C.c_double * 3),
+    ]
+
+
+class PositionArcC(C.Structure):
+    _fields_ = [
+        ("n_msr", C.c_int64),
+        ("epoch_ns", C.c_void_p),
+        ("tracker", C.c_void_p),
+        ("obs", C.c_void_p),
     ]
 
 
@@ -382,6 +410,12 @@ def _declare(lib):
     lib.nyxb_od_smooth_batch.restype = C.c_int32
     lib.nyxb_od_smooth_batch.argtypes = [vp, C.POINTER(OdConfigC), C.c_int32, C.POINTER(GroundStationC), C.POINTER(TrackingArcC),
                                          C.c_size_t, C.POINTER(OdRecordsC), vp, C.POINTER(SmoothOutputsC)]
+    lib.nyxb_od_position_batch.restype = C.c_int32
+    lib.nyxb_od_position_batch.argtypes = [vp, C.POINTER(OdConfigC), C.c_int32, C.POINTER(PositionDeviceC), C.POINTER(PositionArcC),
+                                           C.c_size_t, vp, vp, vp, vp, C.POINTER(OdOutputsC), C.POINTER(OdRecordsC)]
+    lib.nyxb_od_position_smooth_batch.restype = C.c_int32
+    lib.nyxb_od_position_smooth_batch.argtypes = [vp, C.POINTER(OdConfigC), C.c_int32, C.POINTER(PositionDeviceC), C.POINTER(PositionArcC),
+                                                  C.c_size_t, C.POINTER(OdRecordsC), vp, C.POINTER(SmoothOutputsC)]
     lib.nyxb_od_predict_batch.restype = C.c_int32
     lib.nyxb_od_predict_batch.argtypes = [vp, C.POINTER(OdConfigC), C.c_size_t, vp, vp, vp, vp, vp, vp, C.POINTER(PredictOutputsC)]
     lib.nyxb_od_bls_batch.restype = C.c_int32
@@ -446,6 +480,8 @@ EXPORTED_SYMBOLS = [
     "nyxb_od_ekf_batch",
     "nyxb_od_ekf_record_batch",
     "nyxb_od_smooth_batch",
+    "nyxb_od_position_batch",
+    "nyxb_od_position_smooth_batch",
     "nyxb_od_predict_batch",
     "nyxb_od_bls_batch",
     "nyxb_od_bls_evaluate_batch",

@@ -25,6 +25,8 @@ extern "C" cudaError_t nyxb_launch_thread_fast(const DevSetup*, size_t, const do
                                                const DevSink*, cudaStream_t);
 extern "C" double nyxb_fp64_probe(int device, int iters);
 extern "C" cudaError_t nyxb_launch_frame_shift(const DevBody*, double, size_t, double*, const long long*, int*, cudaStream_t);
+extern "C" cudaError_t nyxb_launch_odpos_coop(const DevSetup*, const DevOdPos*, const OdEstRecords*, const int*, size_t, const double*,
+                                              const double*, const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
 extern "C" cudaError_t nyxb_launch_od_coop(const DevSetup*, const DevOd*, const int*, size_t, const double*, const double*, const long long*,
                                            double*, long long*, nyxb_details*, int*, cudaStream_t);
 extern "C" cudaError_t nyxb_launch_od_rec_coop(const DevSetup*, const DevOd*, const OdEstRecords*, const int*, size_t, const double*,
@@ -47,6 +49,7 @@ static_assert(sizeof(nyxb_integ_opts) == 56 && sizeof(nyxb_gravity_field) == 104
 static_assert(sizeof(nyxb_ground_station) == 176 && sizeof(nyxb_od_config) == 72 && sizeof(nyxb_tracking_arc) == 32 && sizeof(nyxb_od_outputs) == 96, "ABI layout");
 static_assert(sizeof(nyxb_bls_config) == 80 && sizeof(nyxb_bls_outputs) == 72, "ABI layout");
 static_assert(sizeof(nyxb_od_records) == 64 && sizeof(nyxb_smooth_outputs) == 48, "ABI layout");
+static_assert(sizeof(nyxb_position_device) == 64 && sizeof(nyxb_position_arc) == 32, "ABI layout");
 
 static thread_local std::string g_err;
 static void set_err(const std::string& s) { g_err = s; }
@@ -892,6 +895,36 @@ extern "C" int32_t nyxb_propagate_batch_stm(nyxb_engine* eng, size_t n, const do
 }
 
 namespace {
+// the filter kernel of the engine's family: warp-cooperative when d_cols is set, else per-thread STRICT or FAST; er: null, or the records
+cudaError_t od_launch(const nyxb_engine* eng, const DevOd* od, const OdEstRecords* er, const int* d_cols, size_t n, const double* d_state,
+                      const double* d_consts, const long long* d_ep, double* d_out, long long* d_oep, nyxb_details* d_det, int* d_status,
+                      cudaStream_t st) {
+    const bool coop = d_cols != nullptr;
+    return er
+        ? (coop ? nyxb_launch_od_rec_coop(&eng->S, od, er, d_cols, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
+                : (eng->mode == NYXB_MODE_STRICT)
+                    ? nyxb_launch_od_rec_strict(&eng->S, od, er, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
+                    : nyxb_launch_od_rec_fast(&eng->S, od, er, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st))
+        : coop
+        ? nyxb_launch_od_coop(&eng->S, od, d_cols, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
+        : (eng->mode == NYXB_MODE_STRICT)
+            ? nyxb_launch_od_strict(&eng->S, od, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
+            : nyxb_launch_od_fast(&eng->S, od, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st);
+}
+cudaError_t od_launch(const nyxb_engine* eng, const DevOdPos* od, const OdEstRecords* er, const int* d_cols, size_t n,
+                      const double* d_state, const double* d_consts, const long long* d_ep, double* d_out, long long* d_oep,
+                      nyxb_details* d_det, int* d_status, cudaStream_t st) {
+    if (d_cols) return nyxb_launch_odpos_coop(&eng->S, od, er, d_cols, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st);
+    return (eng->mode == NYXB_MODE_STRICT)
+        ? nyxb_launch_odpos_strict(&eng->S, od, er, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
+        : nyxb_launch_odpos_fast(&eng->S, od, er, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st);
+}
+
+template <class OD, int NS, class Dev>
+int32_t od_filter_run(nyxb_engine* eng, const nyxb_od_config* cfg, const std::vector<Dev>& hs, int64_t n_msr, const int64_t* arc_epoch,
+                      const int32_t* arc_tracker, const double* arc_obs, size_t n, const double* state_soa, const double* consts_soa,
+                      const int64_t* epoch0_ns, const double* covar0_soa, const nyxb_od_outputs* out, const nyxb_od_records* rec);
+
 // nyxb_od_ekf_batch and nyxb_od_ekf_record_batch: argument checks, packing, one launch, read-back.  rec: null, or the estimate records.
 int32_t od_ekf_run(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations, const nyxb_ground_station* stations,
                    const nyxb_tracking_arc* arc, size_t n, const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
@@ -923,11 +956,6 @@ int32_t od_ekf_run(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_statio
         if (g.n_types % cfg->msr_size != 0) { set_err("filter misconfigured: measurement types per device must be a multiple of msr_size"); return NYXB_RC_UNSUPPORTED; }
     }
     if (n == 0) return NYXB_RC_OK;
-    CUDA_TRY(cudaSetDevice(eng->device));
-    if (!eng->stream) CUDA_TRY(cudaStreamCreateWithFlags(&eng->stream, cudaStreamNonBlocking));
-    cudaStream_t st = eng->stream;
-    const size_t m = (size_t)arc->n_msr;
-    DevBufs B;
     std::vector<DevStation> hs((size_t)n_stations);
     for (int32_t s = 0; s < n_stations; ++s) {
         const nyxb_ground_station& g = stations[s];
@@ -937,7 +965,23 @@ int32_t od_ekf_run(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_statio
         for (int q = 0; q < 2; ++q) { d.types[q] = g.types[q]; d.noise_var[q] = g.noise_var[q]; d.bias[q] = g.bias[q]; }
         d.body_radius = g.body_radius_km;
     }
-    DevOd od{};
+    return od_filter_run<DevOd, 2>(eng, cfg, hs, arc->n_msr, arc->epoch_ns, arc->tracker, arc->obs, n, state_soa, consts_soa, epoch0_ns,
+                                   covar0_soa, out, rec);
+}
+
+// The common part of the ground-station and position-fix filter calls: upload, one launch, read-back.  OD: DevOd or DevOdPos, NS its
+// observation slots; hs: the packed devices.
+template <class OD, int NS, class Dev>
+int32_t od_filter_run(nyxb_engine* eng, const nyxb_od_config* cfg, const std::vector<Dev>& hs, int64_t n_msr, const int64_t* arc_epoch,
+                      const int32_t* arc_tracker, const double* arc_obs, size_t n, const double* state_soa, const double* consts_soa,
+                      const int64_t* epoch0_ns, const double* covar0_soa, const nyxb_od_outputs* out, const nyxb_od_records* rec) {
+    CUDA_TRY(cudaSetDevice(eng->device));
+    if (!eng->stream) CUDA_TRY(cudaStreamCreateWithFlags(&eng->stream, cudaStreamNonBlocking));
+    cudaStream_t st = eng->stream;
+    const size_t m = (size_t)n_msr;
+    const int32_t n_stations = (int32_t)hs.size();
+    DevBufs B;
+    OD od{};
     od.variant = cfg->variant; od.msr_size = cfg->msr_size; od.reject = cfg->reject_num_sigmas;
     od.max_step_ns = cfg->max_step_ns; od.eps_ns = cfg->epoch_precision_ns;
     od.snc_enabled = cfg->snc_enabled; od.snc_frame = cfg->snc_frame;
@@ -945,10 +989,10 @@ int32_t od_ekf_run(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_statio
     od.snc_disable_ns = cfg->snc_disable_time_ns;
     od.n_stations = n_stations;
     od.stations = B.put(hs.data(), hs.size(), st);
-    od.n_msr = arc->n_msr;
-    od.msr_epoch = B.put((const long long*)arc->epoch_ns, m, st);
-    od.msr_tracker = B.put((const int*)arc->tracker, m, st);
-    od.obs = B.put(arc->obs, m * 2 * n, st);
+    od.n_msr = n_msr;
+    od.msr_epoch = B.put((const long long*)arc_epoch, m, st);
+    od.msr_tracker = B.put((const int*)arc_tracker, m, st);
+    od.obs = B.put(arc_obs, m * NS * n, st);
     od.covar0 = B.put(covar0_soa, 81 * n, st);
     double* d_state = B.put(state_soa, 9 * n, st);
     double* d_consts = B.put(consts_soa, 4 * n, st);
@@ -959,9 +1003,9 @@ int32_t od_ekf_run(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_statio
     int* d_status = B.alloc<int>(n);
     od.covar = B.alloc<double>(81 * n);
     od.state_dev = out->state_dev_soa ? B.alloc<double>(9 * n) : nullptr;
-    od.ratio = out->resid_ratio ? B.alloc<double>(m * 2 * n) : nullptr;
-    od.prefit = out->prefit ? B.alloc<double>(m * 2 * n) : nullptr;
-    od.postfit = out->postfit ? B.alloc<double>(m * 2 * n) : nullptr;
+    od.ratio = out->resid_ratio ? B.alloc<double>(m * NS * n) : nullptr;
+    od.prefit = out->prefit ? B.alloc<double>(m * NS * n) : nullptr;
+    od.postfit = out->postfit ? B.alloc<double>(m * NS * n) : nullptr;
     od.flags = out->msr_flags ? B.alloc<int>(m * n) : nullptr;
     od.est_state = out->est_state ? B.alloc<double>(m * 9 * n) : nullptr;
     od.est_cov = out->est_covar_diag ? B.alloc<double>(m * 9 * n) : nullptr;
@@ -973,9 +1017,9 @@ int32_t od_ekf_run(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_statio
         return NYXB_RC_CUDA;
     }
     // per-measurement records default to NaN (0xFF bytes) / 0 flags where nothing is written
-    if (od.ratio) CUDA_TRY(cudaMemsetAsync(od.ratio, 0xFF, sizeof(double) * m * 2 * n, st));
-    if (od.prefit) CUDA_TRY(cudaMemsetAsync(od.prefit, 0xFF, sizeof(double) * m * 2 * n, st));
-    if (od.postfit) CUDA_TRY(cudaMemsetAsync(od.postfit, 0xFF, sizeof(double) * m * 2 * n, st));
+    if (od.ratio) CUDA_TRY(cudaMemsetAsync(od.ratio, 0xFF, sizeof(double) * m * NS * n, st));
+    if (od.prefit) CUDA_TRY(cudaMemsetAsync(od.prefit, 0xFF, sizeof(double) * m * NS * n, st));
+    if (od.postfit) CUDA_TRY(cudaMemsetAsync(od.postfit, 0xFF, sizeof(double) * m * NS * n, st));
     if (od.flags) CUDA_TRY(cudaMemsetAsync(od.flags, 0, sizeof(int) * m * n, st));
     if (od.est_state) CUDA_TRY(cudaMemsetAsync(od.est_state, 0xFF, sizeof(double) * m * 9 * n, st));
     if (od.est_cov) CUDA_TRY(cudaMemsetAsync(od.est_cov, 0xFF, sizeof(double) * m * 9 * n, st));
@@ -1010,16 +1054,7 @@ int32_t od_ekf_run(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_statio
     if (int32_t rc = od_coop_cols(eng, B, st, d_cols)) return rc;
     const bool coop = d_cols != nullptr;
     CUDA_TRY(cudaEventRecord(eng->ev0, st));
-    cudaError_t err = rec
-        ? (coop ? nyxb_launch_od_rec_coop(&eng->S, &od, &er, d_cols, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
-                : (eng->mode == NYXB_MODE_STRICT)
-                    ? nyxb_launch_od_rec_strict(&eng->S, &od, &er, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
-                    : nyxb_launch_od_rec_fast(&eng->S, &od, &er, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st))
-        : coop
-        ? nyxb_launch_od_coop(&eng->S, &od, d_cols, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
-        : (eng->mode == NYXB_MODE_STRICT)
-            ? nyxb_launch_od_strict(&eng->S, &od, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
-            : nyxb_launch_od_fast(&eng->S, &od, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st);
+    cudaError_t err = od_launch(eng, &od, rec ? &er : nullptr, d_cols, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st);
     if (err != cudaSuccess) { set_err(std::string("kernel launch: ") + cudaGetErrorString(err)); return NYXB_RC_CUDA; }
     eng->launches += 1;
     eng->last_kernel = coop ? NYXB_KERNEL_COOP : NYXB_KERNEL_THREAD;
@@ -1028,9 +1063,9 @@ int32_t od_ekf_run(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_statio
     CUDA_TRY(cudaMemcpyAsync(out->epoch_ns, d_oep, sizeof(long long) * n, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(out->covar_soa, od.covar, sizeof(double) * 81 * n, cudaMemcpyDeviceToHost, st));
     if (od.state_dev) CUDA_TRY(cudaMemcpyAsync(out->state_dev_soa, od.state_dev, sizeof(double) * 9 * n, cudaMemcpyDeviceToHost, st));
-    if (od.ratio) CUDA_TRY(cudaMemcpyAsync(out->resid_ratio, od.ratio, sizeof(double) * m * 2 * n, cudaMemcpyDeviceToHost, st));
-    if (od.prefit) CUDA_TRY(cudaMemcpyAsync(out->prefit, od.prefit, sizeof(double) * m * 2 * n, cudaMemcpyDeviceToHost, st));
-    if (od.postfit) CUDA_TRY(cudaMemcpyAsync(out->postfit, od.postfit, sizeof(double) * m * 2 * n, cudaMemcpyDeviceToHost, st));
+    if (od.ratio) CUDA_TRY(cudaMemcpyAsync(out->resid_ratio, od.ratio, sizeof(double) * m * NS * n, cudaMemcpyDeviceToHost, st));
+    if (od.prefit) CUDA_TRY(cudaMemcpyAsync(out->prefit, od.prefit, sizeof(double) * m * NS * n, cudaMemcpyDeviceToHost, st));
+    if (od.postfit) CUDA_TRY(cudaMemcpyAsync(out->postfit, od.postfit, sizeof(double) * m * NS * n, cudaMemcpyDeviceToHost, st));
     if (od.flags) CUDA_TRY(cudaMemcpyAsync(out->msr_flags, od.flags, sizeof(int) * m * n, cudaMemcpyDeviceToHost, st));
     if (od.est_state) CUDA_TRY(cudaMemcpyAsync(out->est_state, od.est_state, sizeof(double) * m * 9 * n, cudaMemcpyDeviceToHost, st));
     if (od.est_cov) CUDA_TRY(cudaMemcpyAsync(out->est_covar_diag, od.est_cov, sizeof(double) * m * 9 * n, cudaMemcpyDeviceToHost, st));
@@ -1068,6 +1103,12 @@ extern "C" int32_t nyxb_od_ekf_record_batch(nyxb_engine* eng, const nyxb_od_conf
     if (!rec) { set_err("null argument"); return NYXB_RC_BAD_ARG; }
     return od_ekf_run(eng, cfg, n_stations, stations, arc, n, state_soa, consts_soa, epoch0_ns, covar0_soa, out, rec);
 }
+
+namespace {
+template <class SM, int NS, class Dev>
+int32_t od_smooth_run(nyxb_engine* eng, int M, const std::vector<Dev>& hs, int64_t n_msr, const int32_t* arc_tracker, const double* arc_obs,
+                      size_t n, const nyxb_od_records* rec, const std::vector<int>& pre, nyxb_smooth_outputs* out);
+}  // namespace
 
 extern "C" int32_t nyxb_od_smooth_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations, const nyxb_ground_station* stations,
                                         const nyxb_tracking_arc* arc, size_t n, const nyxb_od_records* rec, const int32_t* filter_status,
@@ -1115,11 +1156,6 @@ extern "C" int32_t nyxb_od_smooth_batch(nyxb_engine* eng, const nyxb_od_config* 
     }
     for (size_t i = 0; i < n; ++i) out->status[i] = pre[i];
     if (n == 0 || cap == 0) return NYXB_RC_OK;
-    CUDA_TRY(cudaSetDevice(eng->device));
-    if (!eng->stream) CUDA_TRY(cudaStreamCreateWithFlags(&eng->stream, cudaStreamNonBlocking));
-    cudaStream_t st = eng->stream;
-    const size_t m = (size_t)arc->n_msr;
-    DevBufs B;
     std::vector<DevStation> hs((size_t)n_stations);
     for (int32_t s = 0; s < n_stations; ++s) {
         const nyxb_ground_station& g = stations[s];
@@ -1129,12 +1165,32 @@ extern "C" int32_t nyxb_od_smooth_batch(nyxb_engine* eng, const nyxb_od_config* 
         for (int q = 0; q < 2; ++q) { d.types[q] = g.types[q]; d.noise_var[q] = g.noise_var[q]; d.bias[q] = g.bias[q]; }
         d.body_radius = g.body_radius_km;
     }
-    DevSmooth sm{};
+    return od_smooth_run<DevSmooth, 2>(eng, M, hs, arc->n_msr, arc->tracker, arc->obs, n, rec, pre, out);
+}
+
+namespace {
+// The common part of the two smoothing calls: upload, the smoothing launch, read-back.  SM: DevSmooth or DevSmoothPos, NS its
+// observation slots; pre: the statuses decided on the host.
+cudaError_t smooth_launch(const nyxb_engine* eng, const DevSmooth* sm, size_t n, cudaStream_t st) { return nyxb_launch_smooth(&eng->S, sm, n, st); }
+cudaError_t smooth_launch(const nyxb_engine* eng, const DevSmoothPos* sm, size_t n, cudaStream_t st) {
+    return nyxb_launch_smooth_pos(&eng->S, sm, n, st);
+}
+
+template <class SM, int NS, class Dev>
+int32_t od_smooth_run(nyxb_engine* eng, int M, const std::vector<Dev>& hs, int64_t n_msr, const int32_t* arc_tracker, const double* arc_obs,
+                      size_t n, const nyxb_od_records* rec, const std::vector<int>& pre, nyxb_smooth_outputs* out) {
+    CUDA_TRY(cudaSetDevice(eng->device));
+    if (!eng->stream) CUDA_TRY(cudaStreamCreateWithFlags(&eng->stream, cudaStreamNonBlocking));
+    cudaStream_t st = eng->stream;
+    const size_t m = (size_t)n_msr, cap = (size_t)rec->capacity;
+    const int32_t n_stations = (int32_t)hs.size();
+    DevBufs B;
+    SM sm{};
     sm.msr_size = M;
     sm.n_stations = n_stations;
     sm.stations = n_stations ? B.put(hs.data(), hs.size(), st) : nullptr;
-    sm.msr_tracker = m ? B.put((const int*)arc->tracker, m, st) : nullptr;
-    sm.obs = m ? B.put(arc->obs, m * 2 * n, st) : nullptr;
+    sm.msr_tracker = m ? B.put((const int*)arc_tracker, m, st) : nullptr;
+    sm.obs = m ? B.put(arc_obs, m * NS * n, st) : nullptr;
     sm.cap = (long long)cap;
     sm.epoch = B.put((const long long*)rec->epoch_ns, cap * n, st);
     sm.tag = B.put((const long long*)rec->tag, cap * n, st);
@@ -1148,7 +1204,7 @@ extern "C" int32_t nyxb_od_smooth_batch(nyxb_engine* eng, const nyxb_od_config* 
     sm.sdev = out->deviation ? B.alloc<double>(cap * 9 * n) : nullptr;
     sm.scov = out->covar ? B.alloc<double>(cap * 81 * n) : nullptr;
     sm.ratio = out->fs_ratio ? B.alloc<double>(cap * 9 * n) : nullptr;
-    sm.postfit = out->postfit ? B.alloc<double>(cap * 2 * n) : nullptr;
+    sm.postfit = out->postfit ? B.alloc<double>(cap * NS * n) : nullptr;
     sm.err_key = B.alloc<long long>(n);
     if ((n_stations && !sm.stations) || (m && (!sm.msr_tracker || !sm.obs)) || !sm.epoch || !sm.tag || !sm.nominal || !sm.dev || !sm.covar ||
         !sm.stm || !sm.count || !sm.pre_status || (out->state && !sm.state) || (out->deviation && !sm.sdev) || (out->covar && !sm.scov) ||
@@ -1160,10 +1216,10 @@ extern "C" int32_t nyxb_od_smooth_batch(nyxb_engine* eng, const nyxb_od_config* 
     if (sm.sdev) CUDA_TRY(cudaMemsetAsync(sm.sdev, 0xFF, sizeof(double) * cap * 9 * n, st));
     if (sm.scov) CUDA_TRY(cudaMemsetAsync(sm.scov, 0xFF, sizeof(double) * cap * 81 * n, st));
     if (sm.ratio) CUDA_TRY(cudaMemsetAsync(sm.ratio, 0xFF, sizeof(double) * cap * 9 * n, st));
-    if (sm.postfit) CUDA_TRY(cudaMemsetAsync(sm.postfit, 0xFF, sizeof(double) * cap * 2 * n, st));
+    if (sm.postfit) CUDA_TRY(cudaMemsetAsync(sm.postfit, 0xFF, sizeof(double) * cap * NS * n, st));
     CUDA_TRY(cudaMemsetAsync(sm.err_key, 0xFF, sizeof(long long) * n, st));
     CUDA_TRY(cudaEventRecord(eng->ev0, st));
-    cudaError_t err = nyxb_launch_smooth(&eng->S, &sm, n, st);
+    cudaError_t err = smooth_launch(eng, &sm, n, st);
     if (err != cudaSuccess) { set_err(std::string("kernel launch: ") + cudaGetErrorString(err)); return NYXB_RC_CUDA; }
     eng->launches += 1;
     eng->last_kernel = NYXB_KERNEL_THREAD;
@@ -1174,7 +1230,7 @@ extern "C" int32_t nyxb_od_smooth_batch(nyxb_engine* eng, const nyxb_od_config* 
     if (sm.sdev) CUDA_TRY(cudaMemcpyAsync(out->deviation, sm.sdev, sizeof(double) * cap * 9 * n, cudaMemcpyDeviceToHost, st));
     if (sm.scov) CUDA_TRY(cudaMemcpyAsync(out->covar, sm.scov, sizeof(double) * cap * 81 * n, cudaMemcpyDeviceToHost, st));
     if (sm.ratio) CUDA_TRY(cudaMemcpyAsync(out->fs_ratio, sm.ratio, sizeof(double) * cap * 9 * n, cudaMemcpyDeviceToHost, st));
-    if (sm.postfit) CUDA_TRY(cudaMemcpyAsync(out->postfit, sm.postfit, sizeof(double) * cap * 2 * n, cudaMemcpyDeviceToHost, st));
+    if (sm.postfit) CUDA_TRY(cudaMemcpyAsync(out->postfit, sm.postfit, sizeof(double) * cap * NS * n, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     float ms = 0.f;
     if (cudaEventElapsedTime(&ms, eng->ev0, eng->ev1) == cudaSuccess) eng->last_ms = ms;
@@ -1183,6 +1239,97 @@ extern "C" int32_t nyxb_od_smooth_batch(nyxb_engine* eng, const nyxb_od_config* 
     for (size_t i = 0; i < n; ++i)
         if (key[i] >= 0) out->status[i] = (key[i] & 1) ? NYXB_ERR_SINGULAR_STM : NYXB_ERR_EPHEMERIS;
     return NYXB_RC_OK;
+}
+
+// the checks and packing of a position device list (nyxb_od_position_batch / _smooth_batch)
+int32_t pack_position_devices(int32_t n_devices, const nyxb_position_device* devices, std::vector<DevPosDevice>& hs) {
+    hs.assign((size_t)(n_devices > 0 ? n_devices : 0), DevPosDevice{});
+    for (int32_t s = 0; s < n_devices; ++s) {
+        const nyxb_position_device& g = devices[s];
+        if (g.n_types < 1 || g.n_types > 3) { set_err("bad position device: n_types must be 1 to 3"); return NYXB_RC_BAD_ARG; }
+        DevPosDevice& d = hs[s];
+        d.n_types = g.n_types;
+        for (int q = 0; q < 3; ++q) { d.types[q] = g.types[q]; d.noise_var[q] = g.noise_var[q]; d.bias[q] = g.bias[q]; }
+        for (int q = 0; q < g.n_types; ++q) {
+            if (g.types[q] != NYXB_MSR_X && g.types[q] != NYXB_MSR_Y && g.types[q] != NYXB_MSR_Z) {
+                set_err("bad position device: measurement types must be X, Y or Z");
+                return NYXB_RC_BAD_ARG;
+            }
+            for (int p = 0; p < q; ++p)
+                if (g.types[p] == g.types[q]) { set_err("bad position device: duplicate measurement type"); return NYXB_RC_BAD_ARG; }
+        }
+    }
+    return NYXB_RC_OK;
+}
+}  // namespace
+
+extern "C" int32_t nyxb_od_position_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_devices, const nyxb_position_device* devices,
+                                          const nyxb_position_arc* arc, size_t n, const double* state_soa, const double* consts_soa,
+                                          const int64_t* epoch0_ns, const double* covar0_soa, const nyxb_od_outputs* out,
+                                          const nyxb_od_records* rec) {
+    if (!eng || !cfg || !arc || !state_soa || !consts_soa || !epoch0_ns || !covar0_soa || !out || !out->state_soa || !out->epoch_ns ||
+        !out->covar_soa || !out->status || (n_devices > 0 && !devices) || n_devices < 0) {
+        set_err("null argument");
+        return NYXB_RC_BAD_ARG;
+    }
+    if (rec && (rec->capacity < 0 || !rec->count ||
+                (rec->capacity > 0 && (!rec->epoch_ns || !rec->tag || !rec->nominal || !rec->deviation || !rec->covar || !rec->stm)))) {
+        set_err("bad estimate records: count is required, and every record array when capacity > 0");
+        return NYXB_RC_BAD_ARG;
+    }
+    if (cfg->msr_size < 1 || cfg->msr_size > 3) { set_err("msr_size must be 1, 2 or 3"); return NYXB_RC_BAD_ARG; }
+    if (cfg->variant != NYXB_KF_REFERENCE_UPDATE && cfg->variant != NYXB_KF_DEVIATION_TRACKING) { set_err("bad filter variant"); return NYXB_RC_BAD_ARG; }
+    if (cfg->max_step_ns <= 0) { set_err("StepSize: max_step must be positive (process/mod.rs:147-150)"); return NYXB_RC_BAD_ARG; }
+    if (arc->n_msr < 2) { set_err("TooFewMeasurements: need 2 (process/mod.rs:139-145)"); return NYXB_RC_BAD_ARG; }
+    if (!arc->epoch_ns || !arc->tracker || !arc->obs) { set_err("null tracking arc arrays"); return NYXB_RC_BAD_ARG; }
+    std::vector<DevPosDevice> hs;
+    if (int32_t rc = pack_position_devices(n_devices, devices, hs)) return rc;
+    if (!stm_supported(eng)) return NYXB_RC_UNSUPPORTED;
+    if (n == 0) return NYXB_RC_OK;
+    return od_filter_run<DevOdPos, 3>(eng, cfg, hs, arc->n_msr, arc->epoch_ns, arc->tracker, arc->obs, n, state_soa, consts_soa, epoch0_ns,
+                                      covar0_soa, out, rec);
+}
+
+extern "C" int32_t nyxb_od_position_smooth_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_devices,
+                                                 const nyxb_position_device* devices, const nyxb_position_arc* arc, size_t n,
+                                                 const nyxb_od_records* rec, const int32_t* filter_status, nyxb_smooth_outputs* out) {
+    if (!eng || !cfg || !arc || !rec || !filter_status || !out || !out->status || (n_devices > 0 && !devices) || n_devices < 0) {
+        set_err("null argument");
+        return NYXB_RC_BAD_ARG;
+    }
+    if (cfg->msr_size < 1 || cfg->msr_size > 3) { set_err("msr_size must be 1, 2 or 3"); return NYXB_RC_BAD_ARG; }
+    if (rec->capacity < 0 || !rec->count ||
+        (rec->capacity > 0 && (!rec->epoch_ns || !rec->tag || !rec->nominal || !rec->deviation || !rec->covar || !rec->stm))) {
+        set_err("bad estimate records: count is required, and every record array when capacity > 0");
+        return NYXB_RC_BAD_ARG;
+    }
+    if (arc->n_msr < 0 || (arc->n_msr > 0 && (!arc->tracker || !arc->obs))) { set_err("null tracking arc arrays"); return NYXB_RC_BAD_ARG; }
+    std::vector<DevPosDevice> hs;
+    if (int32_t rc = pack_position_devices(n_devices, devices, hs)) return rc;
+    const size_t cap = (size_t)rec->capacity;
+    const int M = cfg->msr_size;
+    std::vector<int> pre(n);
+    for (size_t i = 0; i < n; ++i) {
+        const long long cnt = rec->count[i];
+        pre[i] = filter_status[i] ? filter_status[i]
+               : (cnt > (long long)cap) ? NYXB_ERR_RECORDS_TRUNCATED
+               : (cnt < 2) ? NYXB_ERR_TOO_FEW_MEASUREMENTS : 0;
+        if (pre[i]) continue;
+        for (long long k = 0; k < cnt; ++k) {
+            const int64_t tg = rec->tag[(size_t)k * n + i];
+            if (tg == NYXB_OD_TAG_TIME_UPDATE) continue;
+            const int64_t mk = NYXB_OD_POS_TAG_MSR(tg);
+            const int w = (int)NYXB_OD_POS_TAG_WINDOW(tg);
+            if (tg < 0 || NYXB_OD_POS_TAG_MSR_SIZE(tg) != M) { set_err("estimate records written with another msr_size"); return NYXB_RC_BAD_ARG; }
+            if (mk >= arc->n_msr || arc->tracker[mk] < 0 || arc->tracker[mk] >= n_devices || w * M >= hs[arc->tracker[mk]].n_types) {
+                set_err("estimate records do not match this tracking arc");
+                return NYXB_RC_BAD_ARG;
+            }
+        }
+    }
+    for (size_t i = 0; i < n; ++i) out->status[i] = pre[i];
+    if (n == 0 || cap == 0) return NYXB_RC_OK;
+    return od_smooth_run<DevSmoothPos, 3>(eng, M, hs, arc->n_msr, arc->tracker, arc->obs, n, rec, pre, out);
 }
 
 extern "C" int32_t nyxb_od_predict_batch(nyxb_engine* eng, const nyxb_od_config* cfg, size_t n, const double* state_soa,

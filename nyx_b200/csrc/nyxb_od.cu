@@ -37,6 +37,9 @@
 #define NYXB_LAUNCH_BLS nyxb_launch_bls_strict
 #define NYXB_KODREC nyxb_k_od_rec_strict
 #define NYXB_LAUNCH_ODREC nyxb_launch_od_rec_strict
+#define NYXB_KODPOS nyxb_k_odpos_strict
+#define NYXB_KODPOSREC nyxb_k_odpos_rec_strict
+#define NYXB_LAUNCH_ODPOS nyxb_launch_odpos_strict
 #else
 #define NYXB_KSTM nyxb_k_stm_fast
 #define NYXB_KOD nyxb_k_od_fast
@@ -48,6 +51,9 @@
 #define NYXB_LAUNCH_BLS nyxb_launch_bls_fast
 #define NYXB_KODREC nyxb_k_od_rec_fast
 #define NYXB_LAUNCH_ODREC nyxb_launch_od_rec_fast
+#define NYXB_KODPOS nyxb_k_odpos_fast
+#define NYXB_KODPOSREC nyxb_k_odpos_rec_fast
+#define NYXB_LAUNCH_ODPOS nyxb_launch_odpos_fast
 #endif
 
 // ------------------------------------------------------------------------- per-thread backend of nyxb_od_arc.cuh
@@ -69,20 +75,22 @@ __device__ static int eom_stm(const DevSetup& S, OdInst& in, double delta_t_s, c
     return 0;
 }
 
-// One thread runs the whole trajectory or filter: every loop is serial and its arrays are local.
-struct ThreadB {
+// One thread runs the whole trajectory or filter: every loop is serial and its arrays are local.  NS: the tracker kind's observation
+// slots (the gain scratch PHt and K is 9 x NS).
+template <int NS>
+struct ThreadBT {
     static constexpr int stride = 1;
     const DevSetup& S;
     double phi[81];
     struct Step {
         double nphi[81], k[NYXB_MAX_STAGES][6], Ai[NYXB_MAX_STAGES][12];
-        __device__ explicit Step(ThreadB&) {}
+        __device__ explicit Step(ThreadBT&) {}
     };
     struct Filt {
-        double P[81], xdev[9], Pb[81], T[81], F[81], PHt[18], K[18];
-        __device__ explicit Filt(ThreadB&) {}
+        double P[81], xdev[9], Pb[81], T[81], F[81], PHt[9 * NS], K[9 * NS];
+        __device__ explicit Filt(ThreadBT&) {}
     };
-    __device__ explicit ThreadB(const DevSetup& s) : S(s) {}
+    __device__ explicit ThreadBT(const DevSetup& s) : S(s) {}
     __device__ int first() const { return 0; }
     __device__ bool lead() const { return true; }
     __device__ void sync() const {}
@@ -91,6 +99,7 @@ struct ThreadB {
         return eom_stm(S, in, delta_t_s, ys, st.k[slot], st.Ai[slot], st.Ai[slot] + 9);
     }
 };
+using ThreadB = ThreadBT<2>;
 
 __global__ void __launch_bounds__(64)
 NYXB_KSTM(const __grid_constant__ DevSetup S, size_t n, const double* __restrict__ state, const double* __restrict__ consts,
@@ -154,6 +163,28 @@ NYXB_KBLS(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od, 
     od_bls(od, bl, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
 }
 
+// the filter over position fixes (PositionDevice), without and with the estimate records
+__global__ void __launch_bounds__(64)
+NYXB_KODPOS(const __grid_constant__ DevSetup S, const __grid_constant__ DevOdPos od, size_t n, const double* __restrict__ state,
+            const double* __restrict__ consts, const long long* __restrict__ epoch0, double* __restrict__ out_state,
+            long long* __restrict__ out_epoch, nyxb_details* __restrict__ out_details, int* __restrict__ out_status) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    ThreadBT<3> b(S);
+    od_process_arc<ThreadBT<3>, false, PosTrk>(od, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
+}
+
+__global__ void __launch_bounds__(64)
+NYXB_KODPOSREC(const __grid_constant__ DevSetup S, const __grid_constant__ DevOdPos od, const OdEstRecords er, size_t n,
+               const double* __restrict__ state, const double* __restrict__ consts, const long long* __restrict__ epoch0,
+               double* __restrict__ out_state, long long* __restrict__ out_epoch, nyxb_details* __restrict__ out_details,
+               int* __restrict__ out_status) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    ThreadBT<3> b(S);
+    od_process_arc<ThreadBT<3>, true, PosTrk>(od, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status, &er);
+}
+
 extern "C" cudaError_t NYXB_LAUNCH_STM(const DevSetup* S, size_t n, const double* state, const double* consts, const long long* epoch0,
                                        long long end_epoch, long long* step_io, const double* stm_in, double* out_state,
                                        long long* out_epoch, double* out_stm, nyxb_details* out_details, int* out_status,
@@ -205,5 +236,19 @@ extern "C" cudaError_t NYXB_LAUNCH_BLS(const DevSetup* S, const DevOd* od, const
     const int block = 32;  // as the filter kernel
     unsigned grid = (unsigned)((n + block - 1) / block);
     NYXB_KBLS<<<grid, block, 0, stream>>>(*S, *od, *bl, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
+    return cudaGetLastError();
+}
+
+// er: null for the filter alone
+extern "C" cudaError_t NYXB_LAUNCH_ODPOS(const DevSetup* S, const DevOdPos* od, const OdEstRecords* er, size_t n, const double* state,
+                                         const double* consts, const long long* epoch0, double* out_state, long long* out_epoch,
+                                         nyxb_details* out_details, int* out_status, cudaStream_t stream) {
+    if (n == 0) return cudaSuccess;
+    const int block = 32;  // as the filter kernel
+    unsigned grid = (unsigned)((n + block - 1) / block);
+    if (er)
+        NYXB_KODPOSREC<<<grid, block, 0, stream>>>(*S, *od, *er, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
+    else
+        NYXB_KODPOS<<<grid, block, 0, stream>>>(*S, *od, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
     return cudaGetLastError();
 }

@@ -13,7 +13,17 @@ struct DevStation {
     double body_radius;
 };
 
-struct DevOd {
+// GNSS-style position fixes (od/position): X, Y, Z of the spacecraft in the integration frame.  types[] in the device's list order,
+// as NYXB_MSR_X.. (the observation slot of a type is type - NYXB_MSR_X); noise_var / bias per list position.
+struct DevPosDevice {
+    int n_types;
+    int types[3];
+    double noise_var[3], bias[3];
+};
+
+// Dev: the tracker kind (DevStation, or DevPosDevice for position fixes, whose observations are [m][3][n])
+template <class Dev>
+struct DevOdT {
     int variant, msr_size;
     double reject;                 // < 0: no sigma rejection
     long long max_step_ns, eps_ns;
@@ -21,22 +31,23 @@ struct DevOd {
     double snc_diag[3];
     long long snc_disable_ns;
     int n_stations;
-    const DevStation* stations;
+    const Dev* stations;
     long long n_msr;
     const long long* msr_epoch;    // [m]
     const int* msr_tracker;        // [m]
-    const double* obs;             // [m][2][n]
+    const double* obs;             // [m][2][n] ([m][3][n] for position fixes)
     const double* covar0;          // [81][n]
     // outputs (any of the per-measurement ones may be null)
     double* covar;                 // [81][n]
     double* state_dev;             // [9][n] or null
-    double* ratio;                 // [m][2][n]
+    double* ratio;                 // [m][2][n] (slots: as obs)
     double* prefit;                // [m][2][n]
     double* postfit;               // [m][2][n]
     int* flags;                    // [m][n]
     double* est_state;             // [m][9][n]
     double* est_cov;               // [m][9][n]
 };
+struct DevOd : DevOdT<DevStation> {};
 
 // Records of a covariance prediction (KalmanODProcess::predict_until): record k holds estimate.state() (nominal + deviation, Cr
 // clamped to [0, 2]: `Spacecraft + OVector<9>`, cosmic/spacecraft.rs:713-728) at [(k*9 + r)*n + i] and the covariance, (r, c) at
@@ -63,11 +74,12 @@ struct OdEstRecords {
     long long* count;    // [n]
 };
 
-// ODSolution::smooth over the records of n filters (nyxb_smooth.cu)
-struct DevSmooth {
+// ODSolution::smooth over the records of n filters (nyxb_smooth.cu); Dev as DevOdT
+template <class Dev>
+struct DevSmoothT {
     int msr_size;
     int n_stations;
-    const DevStation* stations;
+    const Dev* stations;
     const int* msr_tracker;        // [m]
     const double* obs;             // [m][2][n]
     long long cap;
@@ -86,6 +98,7 @@ struct DevSmooth {
     double* postfit;               // [cap][2][n] or null
     long long* err_key;            // [n] -1, or the largest 2k + (1: singular Phi, 0: ephemeris) among the failing estimates k
 };
+struct DevSmooth : DevSmoothT<DevStation> {};
 
 // Batch least squares (BatchLeastSquares::estimate / evaluate, od/blse/mod.rs:146-541).  The schedule, stations, observations,
 // max_step and epoch precision come from DevOd; this holds the solver settings and the per-problem outputs ([n], covar [81][n]).
@@ -126,3 +139,12 @@ extern "C" cudaError_t nyxb_launch_bls_strict(const DevSetup*, const DevOd*, con
 extern "C" cudaError_t nyxb_launch_bls_fast(const DevSetup*, const DevOd*, const DevBls*, size_t, const double*, const double*,
                                             const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
 extern "C" cudaError_t nyxb_launch_smooth(const DevSetup*, const DevSmooth*, size_t, cudaStream_t);
+
+// position fixes (DevOdT<DevPosDevice>): the same filter and smoother, three observation slots
+struct DevOdPos : DevOdT<DevPosDevice> {};
+struct DevSmoothPos : DevSmoothT<DevPosDevice> {};
+extern "C" cudaError_t nyxb_launch_odpos_strict(const DevSetup*, const DevOdPos*, const OdEstRecords*, size_t, const double*, const double*,
+                                                const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
+extern "C" cudaError_t nyxb_launch_odpos_fast(const DevSetup*, const DevOdPos*, const OdEstRecords*, size_t, const double*, const double*,
+                                              const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
+extern "C" cudaError_t nyxb_launch_smooth_pos(const DevSetup*, const DevSmoothPos*, size_t, cudaStream_t);

@@ -198,8 +198,8 @@ __device__ int od_propagate(B& b, OdInst& in, long long duration_ns) {
 
 // ------------------------------------------------------------------------- time update, measurement update (filtering.rs:59-316)
 // f.Pb = Phi P Phi^T (+ SNC: ProcessNoise::propagate, snc.rs:211-286); filtering.rs:61-78 / 132-150
-template <class B>
-__device__ __forceinline__ void od_covar_bar(const DevOd& od, const OdInst& in, long long prev_epoch, B& b, typename B::Filt& f) {
+template <class B, class Dev>
+__device__ __forceinline__ void od_covar_bar(const DevOdT<Dev>& od, const OdInst& in, long long prev_epoch, B& b, typename B::Filt& f) {
     for (int e = b.first(); e < 81; e += B::stride) {   // T = Phi P
         const int r = e / 9, c = e - 9 * r;
         double s = 0.0;
@@ -245,8 +245,8 @@ __device__ __forceinline__ void od_covar_bar(const DevOd& od, const OdInst& in, 
 }
 
 // KalmanFilter::time_update, filtering.rs:59-102
-template <class B>
-__device__ __forceinline__ void od_time_update(const DevOd& od, const OdInst& in, long long& prev_epoch, B& b, typename B::Filt& f) {
+template <class B, class Dev>
+__device__ __forceinline__ void od_time_update(const DevOdT<Dev>& od, const OdInst& in, long long& prev_epoch, B& b, typename B::Filt& f) {
     od_covar_bar(od, in, prev_epoch, b, f);
     const bool tracking = od.variant == NYXB_KF_DEVIATION_TRACKING;
     for (int r = b.first(); r < 9; r += B::stride) {   // new deviation into T, free once Pb is formed
@@ -284,16 +284,19 @@ __device__ __forceinline__ void od_est_push(const OdEstRecords& er, long long& c
 
 // Loads filter i, runs the whole arc and stores the final covariance, deviation, state, details and status.  REC: also write one
 // estimate record per entry of the reference's ODSolution.estimates into *er (null when REC is false); the filter's arithmetic and
-// outputs are the same either way.
-template <class B, bool REC = false>
-__device__ void od_process_arc(const DevOd& od, B& b, size_t i, size_t n, const double* state, const double* consts, const long long* epoch0,
+// outputs are the same either way.  TRK: the tracker kind (GroundTrk, PosTrk in nyxb_od_device.cuh); B::Filt's PHt and K hold
+// 9 x TRK::NS entries.
+template <class B, bool REC = false, class TRK = GroundTrk>
+__device__ void od_process_arc(const DevOdT<typename TRK::Dev>& od, B& b, size_t i, size_t n, const double* state, const double* consts, const long long* epoch0,
                                double* out_state, long long* out_epoch, nyxb_details* out_details, int* out_status,
                                const OdEstRecords* er = nullptr) {
+    constexpr int NS = TRK::NS;
     const DevSetup& S = b.S;
     OdInst in;
     od_load(S, in, i, n, state, consts, epoch0, nullptr);
     if (!in.fixed) in.step_ns = od.max_step_ns;              // :170-172
     typename B::Filt f(b);
+    static_assert(sizeof(f.PHt) == sizeof(double) * 9 * NS && sizeof(f.K) == sizeof(double) * 9 * NS, "B::Filt of another tracker kind");
     for (int e = b.first(); e < 81; e += B::stride) {
         const int r = e / 9, c = e - 9 * r;
         f.P[e] = od.covar0[(size_t)(c * 9 + r) * n + i];
@@ -308,9 +311,11 @@ __device__ void od_process_arc(const DevOd& od, B& b, size_t i, size_t n, const 
     long long nrec = 0;
     for (long long k = 0; k < od.n_msr && rc == 0; ++k) {
         const long long t_k = od.msr_epoch[k];
-        const double o[2] = { od.obs[((size_t)k * 2 + 0) * n + i], od.obs[((size_t)k * 2 + 1) * n + i] };
+        double o[NS];
+#pragma unroll
+        for (int s = 0; s < NS; ++s) o[s] = od.obs[((size_t)k * NS + s) * n + i];
         int flags = 0;
-        if (o[0] != o[0] && o[1] != o[1]) {
+        if (TRK::absent(o)) {
             if (od.flags && b.lead()) od.flags[(size_t)k * n + i] = NYXB_MSRF_ABSENT;
             continue;
         }
@@ -333,75 +338,80 @@ __device__ void od_process_arc(const DevOd& od, B& b, size_t i, size_t n, const 
             in.epoch_ns = t_k;                                                  // :254
             const int trk = od.msr_tracker[k];
             if (trk < 0 || trk >= od.n_stations) break;                         // unknown tracker :400-410
-            const DevStation& gs = od.stations[trk];
+            const typename TRK::Dev& gs = od.stations[trk];
             const int windows = gs.n_types / M;
             for (int wno = 0; wno <= windows; ++wno) {                          // :270-398
-                OdWindow w;
-                const int wrc = od_window_setup(S, gs, M, wno, o, t_k, in.y, w);
+                typename TRK::Win w;
+                const int wrc = TRK::setup(S, gs, M, wno, o, t_k, in.y, w);
                 if (wrc == OD_WIN_EMPTY) break;
                 if (wrc == OD_WIN_UNAVAILABLE) continue;
                 if (wrc == OD_WIN_EPHEMERIS) { rc = NYXB_ERR_EPHEMERIS; break; }
                 if (wrc == OD_WIN_NOT_VISIBLE) { flags |= NYXB_MSRF_NOT_VISIBLE; continue; }
-                const double (&H)[2][9] = w.H;
+                const double (&H)[NS][9] = w.H;
                 const double* Rk = w.Rk;
                 // ---- measurement_update (filtering.rs:107-316)
                 od_covar_bar(od, in, prev_epoch, b, f);
-                for (int e = b.first(); e < 18; e += B::stride) {               // PHt[r][q], r = e / 2, q = e % 2
-                    const int r = e >> 1, q = e & 1;
+                for (int e = b.first(); e < 9 * NS; e += B::stride) {           // PHt[r][q], r = e / NS, q = e % NS
+                    const int r = (NS == 2) ? (e >> 1) : e / NS, q = (NS == 2) ? (e & 1) : e % NS;
                     double s = 0.0;
                     if (q < M)
                         for (int c = 0; c < 9; ++c) s += f.Pb[r * 9 + c] * H[q][c];
                     f.PHt[e] = s;
                 }
                 b.sync();
-                double Sk[2][2] = { {0.0, 0.0}, {0.0, 0.0} }, pre[2] = { 0.0, 0.0 };
+                double Sk[NS][NS], pre[NS];
+#pragma unroll
+                for (int a = 0; a < NS; ++a) {
+                    pre[a] = 0.0;
+#pragma unroll
+                    for (int bb = 0; bb < NS; ++bb) Sk[a][bb] = 0.0;
+                }
                 for (int a = 0; a < M; ++a)
                     for (int bb = 0; bb < M; ++bb) {
                         double s = 0.0;
-                        for (int c = 0; c < 9; ++c) s += H[a][c] * f.PHt[c * 2 + bb];
+                        for (int c = 0; c < 9; ++c) s += H[a][c] * f.PHt[c * NS + bb];
                         Sk[a][bb] = s + ((a == bb) ? Rk[a] : 0.0);
                     }
                 for (int q = 0; q < M; ++q) pre[q] = w.real_obs[q] - w.comp[q];
                 double ratio;
-                if (!od_ratio(M, Sk, Rk, pre, ratio)) { rc = NYXB_ERR_PROP_MATH; break; }   // SingularNoiseRk
+                if (!TRK::ratio(M, Sk, Rk, pre, ratio)) { rc = NYXB_ERR_PROP_MATH; break; }   // SingularNoiseRk
                 const int rslot = (M == 1) ? wno : 0;
                 if (b.lead()) {
-                    if (od.ratio) od.ratio[((size_t)k * 2 + rslot) * n + i] = ratio;
-                    if (od.prefit) for (int q = 0; q < w.ncur; ++q) od.prefit[((size_t)k * 2 + wno * M + q) * n + i] = pre[q];
+                    if (od.ratio) od.ratio[((size_t)k * NS + rslot) * n + i] = ratio;
+                    if (od.prefit) for (int q = 0; q < w.ncur; ++q) od.prefit[((size_t)k * NS + wno * M + q) * n + i] = pre[q];
                 }
                 flags |= NYXB_MSRF_PROCESSED;
                 if (od.reject >= 0.0 && ratio > od.reject) {                    // :169-184
                     od_time_update(od, in, prev_epoch, b, f);
                     flags |= NYXB_MSRF_REJECTED;
-                    if (REC) od_est_push(*er, nrec, ((k * 2 + wno) * 2 + 1) * 2 + (M - 1), in, b, f, i, n);   // push_measurement_update
+                    if (REC) od_est_push(*er, nrec, TRK::tag(k, wno, 1, M), in, b, f, i, n);   // push_measurement_update
                 } else {
                     // gain K = PHt S^-1 (Cholesky solve; plain inverse when S is not positive definite)
-                    double Si[2][2];
-                    if (!od_sinv(M, Sk, Si)) { rc = NYXB_ERR_PROP_MATH; break; }   // SingularKalmanGain
-                    for (int e = b.first(); e < 18; e += B::stride) {           // K[r][q]
-                        const int r = e >> 1, q = e & 1;
-                        double s = 0.0;
-                        if (q < M)
-                            for (int bb = 0; bb < M; ++bb) s += f.PHt[r * 2 + bb] * Si[bb][q];
-                        f.K[e] = s;
+                    typename TRK::Gain g;
+                    if (!TRK::gain_setup(M, Sk, g)) { rc = NYXB_ERR_PROP_MATH; break; }   // SingularKalmanGain
+                    for (int e = b.first(); e < 9 * NS; e += B::stride) {       // K[r][q]
+                        const int r = (NS == 2) ? (e >> 1) : e / NS, q = (NS == 2) ? (e & 1) : e % NS;
+                        f.K[e] = TRK::gain_entry(M, g, &f.PHt[r * NS], q);
                     }
                     b.sync();
                     // xhat and postfit in every lane, so that the state replacement stays in registers
-                    double xhat[9], post[2] = { 0.0, 0.0 };
+                    double xhat[9], post[NS];
+#pragma unroll
+                    for (int q = 0; q < NS; ++q) post[q] = 0.0;
                     if (ekf) {
-                        for (int r = 0; r < 9; ++r) { double s = 0.0; for (int q = 0; q < M; ++q) s += f.K[r * 2 + q] * pre[q]; xhat[r] = s; }
+                        for (int r = 0; r < 9; ++r) { double s = 0.0; for (int q = 0; q < M; ++q) s += f.K[r * NS + q] * pre[q]; xhat[r] = s; }
                         for (int q = 0; q < M; ++q) { double s = 0.0; for (int c = 0; c < 9; ++c) s += H[q][c] * xhat[c]; post[q] = pre[q] - s; }
                     } else {
                         double xbar[9];
                         for (int r = 0; r < 9; ++r) { double s = 0.0; for (int c = 0; c < 9; ++c) s += b.phi[c * 9 + r] * f.xdev[c]; xbar[r] = s; }
                         for (int q = 0; q < M; ++q) { double s = 0.0; for (int c = 0; c < 9; ++c) s += H[q][c] * xbar[c]; post[q] = pre[q] - s; }
-                        for (int r = 0; r < 9; ++r) { double s = 0.0; for (int q = 0; q < M; ++q) s += f.K[r * 2 + q] * post[q]; xhat[r] = xbar[r] + s; }
+                        for (int r = 0; r < 9; ++r) { double s = 0.0; for (int q = 0; q < M; ++q) s += f.K[r * NS + q] * post[q]; xhat[r] = xbar[r] + s; }
                     }
                     // Joseph update: (I - K H) Pbar (I - K H)^T + K R K^T, then symmetrise (filtering.rs:290-300)
                     for (int e = b.first(); e < 81; e += B::stride) {           // F = I - K H
                         const int r = e / 9, c = e - 9 * r;
                         double s = 0.0;
-                        for (int q = 0; q < M; ++q) s += f.K[r * 2 + q] * H[q][c];
+                        for (int q = 0; q < M; ++q) s += f.K[r * NS + q] * H[q][c];
                         f.F[e] = ((r == c) ? 1.0 : 0.0) - s;
                     }
                     b.sync();
@@ -419,7 +429,7 @@ __device__ void od_process_arc(const DevOd& od, B& b, size_t i, size_t n, const 
 #pragma unroll
                         for (int kk = 0; kk < 9; ++kk) s += f.T[r * 9 + kk] * f.F[c * 9 + kk];
                         double s2 = 0.0;
-                        for (int q = 0; q < M; ++q) s2 += (f.K[r * 2 + q] * Rk[q]) * f.K[c * 2 + q];
+                        for (int q = 0; q < M; ++q) s2 += (f.K[r * NS + q] * Rk[q]) * f.K[c * NS + q];
                         f.Pb[e] = s + s2;
                     }
                     b.sync();
@@ -430,8 +440,8 @@ __device__ void od_process_arc(const DevOd& od, B& b, size_t i, size_t n, const 
                     for (int r = b.first(); r < 9; r += B::stride) f.xdev[r] = xhat[r];
                     b.sync();
                     prev_epoch = in.epoch_ns;
-                    if (od.postfit && b.lead()) for (int q = 0; q < w.ncur; ++q) od.postfit[((size_t)k * 2 + wno * M + q) * n + i] = post[q];
-                    if (REC) od_est_push(*er, nrec, ((k * 2 + wno) * 2 + 0) * 2 + (M - 1), in, b, f, i, n);   // pre-update nominal, x-hat
+                    if (od.postfit && b.lead()) for (int q = 0; q < w.ncur; ++q) od.postfit[((size_t)k * NS + wno * M + q) * n + i] = post[q];
+                    if (REC) od_est_push(*er, nrec, TRK::tag(k, wno, 0, M), in, b, f, i, n);   // pre-update nominal, x-hat
                     if (ekf) {                                                  // :364-369 `Spacecraft + OVector<9>`
                         for (int r = 0; r < 9; ++r) in.y[r] = in.y[r] + xhat[r];
                         in.y[6] = in.y[6] < 0.0 ? 0.0 : (in.y[6] > 2.0 ? 2.0 : in.y[6]);

@@ -29,6 +29,12 @@ struct WarpS {
     double PHt[18], K[18], xdev[9];
 };
 
+// the slab of a position-fix filter: the gain scratch has 9 x 3 entries (WarpS's PHt and K stay unused)
+struct WarpSPos {
+    WarpS s;
+    double PHt[27], K[27];
+};
+
 __device__ __forceinline__ double wsum(double v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
@@ -233,6 +239,16 @@ struct WarpB {
     }
 };
 
+// the warp backend of a position-fix filter: WarpB with its gain scratch in WarpSPos
+struct WarpBPos : WarpB {
+    WarpSPos& X;
+    struct Filt {
+        double (&P)[81], (&xdev)[9], (&Pb)[81], (&T)[81], (&F)[81], (&PHt)[27], (&K)[27];
+        __device__ explicit Filt(WarpBPos& b) : P(b.W.P), xdev(b.W.xdev), Pb(b.W.Pb), T(b.W.T), F(b.W.F), PHt(b.X.PHt), K(b.X.K) {}
+    };
+    __device__ WarpBPos(const Ctx& c, WarpSPos& x) : WarpB(c), X(x) {}
+};
+
 __global__ void __launch_bounds__(32 * ODC_WPB)
 nyxb_k_od_coop(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od, const int* __restrict__ cols, size_t n,
                const double* __restrict__ state, const double* __restrict__ consts, const long long* __restrict__ epoch0,
@@ -313,6 +329,41 @@ nyxb_k_bls_coop(const __grid_constant__ DevSetup S, const __grid_constant__ DevO
     od_bls(od, bl, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
 }
 
+// the filter over position fixes, one warp per filter, without and with the estimate records
+template <bool REC>
+__device__ __forceinline__ void odpos_coop(const DevSetup& S, const DevOdPos& od, const OdEstRecords* er, const int* __restrict__ cols,
+                                           size_t n, const double* state, const double* consts, const long long* epoch0, double* out_state,
+                                           long long* out_epoch, nyxb_details* out_details, int* out_status) {
+    extern __shared__ __align__(16) unsigned char smem[];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    const size_t i = (size_t)blockIdx.x * ODC_WPB + wib;
+    if (i >= n) return;   // whole warps leave together
+    const int npw = S.has_grav ? 3 * (S.grav.N + 2) : 0;
+    const size_t slab = (sizeof(WarpSPos) + sizeof(D3) * (size_t)npw + 15) & ~(size_t)15;
+    WarpSPos& X = *reinterpret_cast<WarpSPos*>(smem + slab * wib);
+    Ctx cx;
+    cx.S = &S; cx.mycols = cols + lane * ODC_KMAX; cx.W = &X.s; cx.lane = lane;
+    cx.pw = reinterpret_cast<D3*>(smem + slab * wib + sizeof(WarpSPos));
+    WarpBPos b(cx, X);
+    od_process_arc<WarpBPos, REC, PosTrk>(od, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status, er);
+}
+
+__global__ void __launch_bounds__(32 * ODC_WPB)
+nyxb_k_odpos_coop(const __grid_constant__ DevSetup S, const __grid_constant__ DevOdPos od, const int* __restrict__ cols, size_t n,
+                  const double* __restrict__ state, const double* __restrict__ consts, const long long* __restrict__ epoch0,
+                  double* __restrict__ out_state, long long* __restrict__ out_epoch, nyxb_details* __restrict__ out_details,
+                  int* __restrict__ out_status) {
+    odpos_coop<false>(S, od, nullptr, cols, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
+}
+
+__global__ void __launch_bounds__(32 * ODC_WPB)
+nyxb_k_odpos_rec_coop(const __grid_constant__ DevSetup S, const __grid_constant__ DevOdPos od, const OdEstRecords er,
+                      const int* __restrict__ cols, size_t n, const double* __restrict__ state, const double* __restrict__ consts,
+                      const long long* __restrict__ epoch0, double* __restrict__ out_state, long long* __restrict__ out_epoch,
+                      nyxb_details* __restrict__ out_details, int* __restrict__ out_status) {
+    odpos_coop<true>(S, od, &er, cols, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
+}
+
 extern "C" size_t nyxb_od_coop_smem_bytes(int degree_or_zero) {
     const size_t npw = degree_or_zero > 0 ? 3 * (size_t)(degree_or_zero + 2) : 0;
     const size_t slab = (sizeof(WarpS) + sizeof(D3) * npw + 15) & ~(size_t)15;
@@ -371,5 +422,28 @@ extern "C" cudaError_t nyxb_launch_bls_coop(const DevSetup* S, const DevOd* od, 
     unsigned grid = (unsigned)((n + ODC_WPB - 1) / ODC_WPB);
     nyxb_k_bls_coop<<<grid, 32 * ODC_WPB, smem, stream>>>(*S, *od, *bl, cols, n, state, consts, epoch0, out_state, out_epoch, out_details,
                                                           out_status);
+    return cudaGetLastError();
+}
+
+// er: null for the filter alone
+extern "C" cudaError_t nyxb_launch_odpos_coop(const DevSetup* S, const DevOdPos* od, const OdEstRecords* er, const int* cols, size_t n,
+                                              const double* state, const double* consts, const long long* epoch0, double* out_state,
+                                              long long* out_epoch, nyxb_details* out_details, int* out_status, cudaStream_t stream) {
+    if (n == 0) return cudaSuccess;
+    const size_t npw = S->has_grav ? 3 * (size_t)(S->grav.N + 2) : 0;
+    const size_t smem = ((sizeof(WarpSPos) + sizeof(D3) * npw + 15) & ~(size_t)15) * ODC_WPB;
+    unsigned grid = (unsigned)((n + ODC_WPB - 1) / ODC_WPB);
+    cudaError_t e;
+    if (er) {
+        e = cudaFuncSetAttribute(nyxb_k_odpos_rec_coop, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        nyxb_k_odpos_rec_coop<<<grid, 32 * ODC_WPB, smem, stream>>>(*S, *od, *er, cols, n, state, consts, epoch0, out_state, out_epoch,
+                                                                    out_details, out_status);
+    } else {
+        e = cudaFuncSetAttribute(nyxb_k_odpos_coop, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        nyxb_k_odpos_coop<<<grid, 32 * ODC_WPB, smem, stream>>>(*S, *od, cols, n, state, consts, epoch0, out_state, out_epoch, out_details,
+                                                                out_status);
+    }
     return cudaGetLastError();
 }

@@ -235,13 +235,16 @@ __device__ static bool station_state(const DevSetup& S, const DevStation& st, lo
 // noise and the computed observation minus the device bias.  Shared by the per-thread and the warp-cooperative filter kernels.
 // SUB_BIAS = false leaves the bias in: the batch least-squares estimator compares with measure_instantaneous(state, None), which
 // has no noise and no bias (blse/mod.rs:248-249).
-struct OdWindow {
+// NS: observation slots of the tracker kind (2 for the ground station, 3 for position fixes)
+template <int NS>
+struct OdWindowT {
     int ncur;
-    int cur[2];
-    bool avail[2];
-    double real_obs[2], Rk[2], comp[2];
-    double H[2][9];
+    int cur[NS];
+    bool avail[NS];
+    double real_obs[NS], Rk[NS], comp[NS];
+    double H[NS][9];
 };
+using OdWindow = OdWindowT<2>;
 enum { OD_WIN_OK = 0, OD_WIN_EMPTY = 1, OD_WIN_UNAVAILABLE = 2, OD_WIN_NOT_VISIBLE = 3, OD_WIN_EPHEMERIS = 4 };
 
 template <bool SUB_BIAS = true>
@@ -328,3 +331,169 @@ __device__ static bool od_sinv(int M, const double Sk[2][2], double Si[2][2]) {
     Si[0][0] = Sk[1][1] / det; Si[0][1] = -Sk[0][1] / det; Si[1][0] = -Sk[1][0] / det; Si[1][1] = Sk[0][0] / det;
     return true;
 }
+
+// ------------------------------------------------------------------------- tracker kinds of the filter loop (od_process_arc's TRK)
+// TRK::NS      observation slots per measurement: obs, ratio, prefit and postfit are [m][NS][n], and slot wno*M + q is the position of
+//              the window's type in the device's list (the ratio takes slot wno when M == 1, else 0);
+// TRK::Dev     the device struct of DevOdT;
+// absent(o)    no type of the measurement is in this filter's arc;
+// setup(..)    the window (od_window_setup's contract);
+// ratio(..)    residual ratio of filtering.rs:152-167, false on SingularNoiseRk;
+// gain_setup / gain_entry   K = P H^T S^-1 (filtering.rs:206-231): gain_setup factors S (false on SingularKalmanGain), gain_entry gives
+//              entry q of row r of K from row r of P H^T;
+// tag(..)      the estimate record's tag, and tag_msr / tag_window its measurement index and window.
+struct GroundTrk {
+    static constexpr int NS = 2;
+    using Dev = DevStation;
+    using Win = OdWindow;
+    struct Gain { double Si[2][2]; };
+    __device__ __forceinline__ static bool absent(const double o[2]) { return o[0] != o[0] && o[1] != o[1]; }
+    __device__ __forceinline__ static int setup(const DevSetup& S, const Dev& gs, int M, int wno, const double o[2], long long t_k, const double y[9],
+                                Win& w) {
+        return od_window_setup(S, gs, M, wno, o, t_k, y, w);
+    }
+    __device__ __forceinline__ static bool ratio(int M, const double Sk[2][2], const double Rk[2], const double pre[2], double& r) {
+        return od_ratio(M, Sk, Rk, pre, r);
+    }
+    __device__ __forceinline__ static bool gain_setup(int M, const double Sk[2][2], Gain& g) { return od_sinv(M, Sk, g.Si); }
+    __device__ __forceinline__ static double gain_entry(int M, const Gain& g, const double* pht, int q) {
+        double s = 0.0;
+        if (q < M)
+            for (int bb = 0; bb < M; ++bb) s += pht[bb] * g.Si[bb][q];
+        return s;
+    }
+    __device__ __forceinline__ static long long tag(long long k, int wno, int rej, int M) { return ((k * 2 + wno) * 2 + rej) * 2 + (M - 1); }
+    __device__ __forceinline__ static long long tag_msr(long long tg) { return tg >> 3; }
+    __device__ __forceinline__ static int tag_window(long long tg) { return (int)((tg >> 2) & 1); }
+};
+
+// PositionDevice (od/position): the type at list position ii measures component ii of the nominal position (trk_device.rs:76-83, the
+// list position, not the type), while h_tilde puts its unit row at the TYPE's component X -> 0, Y -> 1, Z -> 2 (sensitivity.rs:55-75)
+// and starts from zeros (sensitivity.rs:32): a window slot without a type, or whose type is absent, keeps a zero row, R keeps the
+// type's variance (trackdata.rs:84-102) and the real observation is 0 (measurement.rs:84-96).  The computed observation is
+// measure()'s ((r_ii + 0) + bias) minus the bias vector (process/mod.rs:324-333): the bias cancels.  No visibility test.
+__device__ static int od_pos_window_setup(const DevPosDevice& d, int M, int wno, const double o[3], const double y[9], OdWindowT<3>& w) {
+    w.ncur = 0;
+    for (int q = wno * M; q < (wno + 1) * M && q < d.n_types; ++q) w.cur[w.ncur++] = d.types[q];
+    if (w.ncur == 0) return OD_WIN_EMPTY;
+    bool any = false;
+    for (int q = 0; q < 3; ++q) w.avail[q] = false;
+    for (int q = 0; q < w.ncur; ++q) { const double v = o[w.cur[q] - NYXB_MSR_X]; w.avail[q] = (v == v); any = any || w.avail[q]; }
+    if (!any) return OD_WIN_UNAVAILABLE;
+    for (int q = 0; q < 3; ++q) {
+        w.real_obs[q] = 0.0; w.Rk[q] = 0.0; w.comp[q] = 0.0;
+        for (int c = 0; c < 9; ++c) w.H[q][c] = 0.0;
+    }
+    for (int q = 0; q < w.ncur; ++q) {
+        const int slot = wno * M + q;
+        w.Rk[q] = d.noise_var[slot];
+        w.comp[q] = ((y[slot] + 0.0) + d.bias[slot]) - d.bias[slot];
+        if (!w.avail[q]) continue;
+        w.real_obs[q] = o[w.cur[q] - NYXB_MSR_X];
+        w.H[q][w.cur[q] - NYXB_MSR_X] = 1.0;
+    }
+    return OD_WIN_OK;
+}
+
+// Lower Cholesky factor of a symmetric 3x3 S, column by column; false when a pivot is not positive.
+__device__ static bool od_chol3(const double A[3][3], double L[3][3]) {
+    L[0][1] = L[0][2] = L[1][2] = 0.0;
+    if (!(A[0][0] > 0.0)) return false;
+    L[0][0] = sqrt(A[0][0]);
+    L[1][0] = A[1][0] / L[0][0];
+    L[2][0] = A[2][0] / L[0][0];
+    const double d1 = A[1][1] - L[1][0] * L[1][0];
+    if (!(d1 > 0.0)) return false;
+    L[1][1] = sqrt(d1);
+    L[2][1] = (A[2][1] - L[2][0] * L[1][0]) / L[1][1];
+    const double d2 = (A[2][2] - L[2][0] * L[2][0]) - L[2][1] * L[2][1];
+    if (!(d2 > 0.0)) return false;
+    L[2][2] = sqrt(d2);
+    return true;
+}
+
+// y = L^-1 b (forward substitution, column-oriented as nalgebra's solve_lower_triangular)
+__device__ __forceinline__ void od_fwd3(const double L[3][3], const double b[3], double y[3]) {
+    double t1 = b[1], t2 = b[2];
+    y[0] = b[0] / L[0][0];
+    t1 = t1 - y[0] * L[1][0]; t2 = t2 - y[0] * L[2][0];
+    y[1] = t1 / L[1][1];
+    t2 = t2 - y[1] * L[2][1];
+    y[2] = t2 / L[2][2];
+}
+
+struct PosTrk {
+    static constexpr int NS = 3;
+    using Dev = DevPosDevice;
+    using Win = OdWindowT<3>;
+    // chol: S = L L^T (M = 3), else Si: S^-1 (M <= 2: od_sinv, M = 3: the closed-form 3x3 inverse after a failed Cholesky)
+    struct Gain { bool chol; double L[3][3]; double Si[3][3]; };
+    __device__ __forceinline__ static bool absent(const double o[3]) { return o[0] != o[0] && o[1] != o[1] && o[2] != o[2]; }
+    __device__ __forceinline__ static int setup(const DevSetup&, const Dev& d, int M, int wno, const double o[3], long long, const double y[9], Win& w) {
+        return od_pos_window_setup(d, M, wno, o, y, w);
+    }
+    // M <= 2: od_ratio on the leading 2x2 block, the ground station's arithmetic
+    __device__ __forceinline__ static bool ratio(int M, const double Sk[3][3], const double Rk[3], const double pre[3], double& r) {
+        if (M < 3) {
+            const double S2[2][2] = { { Sk[0][0], Sk[0][1] }, { Sk[1][0], Sk[1][1] } };
+            const double R2[2] = { Rk[0], Rk[1] }, p2[2] = { pre[0], pre[1] };
+            return od_ratio(M, S2, R2, p2, r);
+        }
+        double L[3][3];
+        if (!od_chol3(Sk, L)) {                                   // fall back to the Cholesky factor of the diagonal R
+            if (!(Rk[0] > 0.0) || !(Rk[1] > 0.0) || !(Rk[2] > 0.0)) return false;
+            for (int a = 0; a < 3; ++a) for (int c = 0; c < 3; ++c) L[a][c] = 0.0;
+            L[0][0] = sqrt(Rk[0]); L[1][1] = sqrt(Rk[1]); L[2][2] = sqrt(Rk[2]);
+        }
+        double w[3];
+        od_fwd3(L, pre, w);
+        r = sqrt(((w[0] * w[0] + w[1] * w[1]) + w[2] * w[2]) / 3.0);
+        return true;
+    }
+    __device__ __forceinline__ static bool gain_setup(int M, const double Sk[3][3], Gain& g) {
+        g.chol = false;
+        if (M < 3) {
+            const double S2[2][2] = { { Sk[0][0], Sk[0][1] }, { Sk[1][0], Sk[1][1] } };
+            double Si[2][2];
+            if (!od_sinv(M, S2, Si)) return false;
+            for (int a = 0; a < 3; ++a) for (int c = 0; c < 3; ++c) g.Si[a][c] = (a < 2 && c < 2) ? Si[a][c] : 0.0;
+            return true;
+        }
+        if (od_chol3(Sk, g.L)) { g.chol = true; return true; }
+        // try_inverse: the closed-form inverse (cofactors over the determinant); not pinned to nalgebra's
+        const double m11 = Sk[0][0], m12 = Sk[0][1], m13 = Sk[0][2], m21 = Sk[1][0], m22 = Sk[1][1], m23 = Sk[1][2];
+        const double m31 = Sk[2][0], m32 = Sk[2][1], m33 = Sk[2][2];
+        const double c11 = m22 * m33 - m32 * m23, c12 = m21 * m33 - m31 * m23, c13 = m21 * m32 - m31 * m22;
+        const double det = (m11 * c11 - m12 * c12) + m13 * c13;
+        if (det == 0.0 || det != det) return false;
+        g.Si[0][0] = c11 / det;
+        g.Si[0][1] = (m13 * m32 - m33 * m12) / det;
+        g.Si[0][2] = (m12 * m23 - m22 * m13) / det;
+        g.Si[1][0] = -c12 / det;
+        g.Si[1][1] = (m11 * m33 - m31 * m13) / det;
+        g.Si[1][2] = (m13 * m21 - m23 * m11) / det;
+        g.Si[2][0] = c13 / det;
+        g.Si[2][1] = (m12 * m31 - m32 * m11) / det;
+        g.Si[2][2] = (m11 * m22 - m21 * m12) / det;
+        return true;
+    }
+    // Cholesky solve S k = (row r of P H^T): forward, then back substitution with L^T
+    __device__ __forceinline__ static double gain_entry(int M, const Gain& g, const double* pht, int q) {
+        if (g.chol) {
+            const double b[3] = { pht[0], pht[1], pht[2] };
+            double y[3], x[3];
+            od_fwd3(g.L, b, y);
+            x[2] = y[2] / g.L[2][2];
+            x[1] = (y[1] - g.L[2][1] * x[2]) / g.L[1][1];
+            x[0] = (y[0] - (g.L[1][0] * x[1] + g.L[2][0] * x[2])) / g.L[0][0];
+            return x[q];
+        }
+        double s = 0.0;
+        if (q < M)
+            for (int bb = 0; bb < M; ++bb) s += pht[bb] * g.Si[bb][q];
+        return s;
+    }
+    __device__ __forceinline__ static long long tag(long long k, int wno, int rej, int M) { return ((k * 4 + wno) * 2 + rej) * 4 + (M - 1); }
+    __device__ __forceinline__ static long long tag_msr(long long tg) { return tg >> 5; }
+    __device__ __forceinline__ static int tag_window(long long tg) { return (int)((tg >> 3) & 3); }
+};

@@ -7,12 +7,15 @@
 // is nyxb_smooth.h, shared with a host build.  The postfit is recomputed through the filter's own window geometry (od_window_setup,
 // bias subtracted) at estimate k's epoch with the measurement of record k+1.
 //
-// Built once, STRICT and without FMA contraction, like the host API: the 9x9 part is then bit-identical to its host build.
+// Built once, STRICT and without FMA contraction, like the host API: the 9x9 part is then bit-identical to its host build.  The same
+// body serves the ground station's records (nyxb_k_smooth) and those of position fixes (nyxb_k_smooth_pos).
 #include "nyxb_od_device.cuh"
 #include "nyxb_smooth.h"
 
-__global__ void __launch_bounds__(128)
-nyxb_k_smooth(const __grid_constant__ DevSetup S, const __grid_constant__ DevSmooth sm, size_t n) {
+// TRK: the tracker kind of the filter that wrote the records (GroundTrk, PosTrk; nyxb_od_device.cuh)
+template <class TRK>
+__device__ __forceinline__ void smooth_one(const DevSetup& S, const DevSmoothT<typename TRK::Dev>& sm, size_t n) {
+    constexpr int NS = TRK::NS;
     const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (size_t)sm.cap * n) return;
     const size_t i = t % n;
@@ -57,15 +60,17 @@ nyxb_k_smooth(const __grid_constant__ DevSetup S, const __grid_constant__ DevSmo
     // residual k+1 recomputed at estimate k (smooth.rs:171-210): measure_instantaneous(smoothed state k) minus the bias
     const long long tg = sm.tag[k1 * n + i];
     if (tg >= 0 && sm.postfit) {
-        const long long mk = tg >> 3;
-        const int wno = (int)((tg >> 2) & 1);
-        const DevStation& gs = sm.stations[sm.msr_tracker[mk]];
-        const double o[2] = { sm.obs[((size_t)mk * 2 + 0) * n + i], sm.obs[((size_t)mk * 2 + 1) * n + i] };
-        OdWindow w;
-        const int wrc = od_window_setup<true>(S, gs, sm.msr_size, wno, o, sm.epoch[(size_t)k * n + i], ys, w);
+        const long long mk = TRK::tag_msr(tg);
+        const int wno = TRK::tag_window(tg);
+        const typename TRK::Dev& gs = sm.stations[sm.msr_tracker[mk]];
+        double o[NS];
+#pragma unroll
+        for (int s = 0; s < NS; ++s) o[s] = sm.obs[((size_t)mk * NS + s) * n + i];
+        typename TRK::Win w;
+        const int wrc = TRK::setup(S, gs, sm.msr_size, wno, o, sm.epoch[(size_t)k * n + i], ys, w);
         if (wrc == OD_WIN_EPHEMERIS) { atomicMax(&sm.err_key[i], 2 * k); return; }
         if (wrc == OD_WIN_OK)
-            for (int q = 0; q < w.ncur; ++q) sm.postfit[((size_t)k * 2 + wno * sm.msr_size + q) * n + i] = w.real_obs[q] - w.comp[q];
+            for (int q = 0; q < w.ncur; ++q) sm.postfit[((size_t)k * NS + wno * sm.msr_size + q) * n + i] = w.real_obs[q] - w.comp[q];
     }
     for (int r = 0; r < 9; ++r) {
         if (sm.state) sm.state[((size_t)k * 9 + r) * n + i] = ys[r];
@@ -79,10 +84,20 @@ nyxb_k_smooth(const __grid_constant__ DevSetup S, const __grid_constant__ DevSmo
         }
 }
 
+__global__ void __launch_bounds__(128)
+nyxb_k_smooth(const __grid_constant__ DevSetup S, const __grid_constant__ DevSmooth sm, size_t n) {
+    smooth_one<GroundTrk>(S, sm, n);
+}
+
+__global__ void __launch_bounds__(128)
+nyxb_k_smooth_pos(const __grid_constant__ DevSetup S, const __grid_constant__ DevSmoothPos sm, size_t n) {
+    smooth_one<PosTrk>(S, sm, n);
+}
+
 // A filter whose smoothing failed (err_key >= 0) has no solution in the reference: every output of it becomes NaN, also those that
 // threads of its other estimates wrote.  Runs after nyxb_k_smooth on the same grid.
-__global__ void __launch_bounds__(128)
-nyxb_k_smooth_fail(const __grid_constant__ DevSmooth sm, size_t n) {
+template <class Dev, int NS>
+__device__ __forceinline__ void smooth_fail(const DevSmoothT<Dev>& sm, size_t n) {
     const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (size_t)sm.cap * n) return;
     const size_t i = t % n, k = t / n;
@@ -94,7 +109,17 @@ nyxb_k_smooth_fail(const __grid_constant__ DevSmooth sm, size_t n) {
         if (sm.ratio) sm.ratio[(k * 9 + r) * n + i] = nan;
     }
     if (sm.scov) for (int e = 0; e < 81; ++e) sm.scov[(k * 81 + e) * n + i] = nan;
-    if (sm.postfit) for (int q = 0; q < 2; ++q) sm.postfit[(k * 2 + q) * n + i] = nan;
+    if (sm.postfit) for (int q = 0; q < NS; ++q) sm.postfit[(k * NS + q) * n + i] = nan;
+}
+
+__global__ void __launch_bounds__(128)
+nyxb_k_smooth_fail(const __grid_constant__ DevSmooth sm, size_t n) {
+    smooth_fail<DevStation, 2>(sm, n);
+}
+
+__global__ void __launch_bounds__(128)
+nyxb_k_smooth_fail_pos(const __grid_constant__ DevSmoothPos sm, size_t n) {
+    smooth_fail<DevPosDevice, 3>(sm, n);
 }
 
 extern "C" cudaError_t nyxb_launch_smooth(const DevSetup* S, const DevSmooth* sm, size_t n, cudaStream_t stream) {
@@ -106,5 +131,17 @@ extern "C" cudaError_t nyxb_launch_smooth(const DevSetup* S, const DevSmooth* sm
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     nyxb_k_smooth_fail<<<grid, block, 0, stream>>>(*sm, n);
+    return cudaGetLastError();
+}
+
+extern "C" cudaError_t nyxb_launch_smooth_pos(const DevSetup* S, const DevSmoothPos* sm, size_t n, cudaStream_t stream) {
+    const size_t total = (size_t)sm->cap * n;
+    if (total == 0) return cudaSuccess;
+    const int block = 128;
+    const unsigned grid = (unsigned)((total + block - 1) / block);
+    nyxb_k_smooth_pos<<<grid, block, 0, stream>>>(*S, *sm, n);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    nyxb_k_smooth_fail_pos<<<grid, block, 0, stream>>>(*sm, n);
     return cudaGetLastError();
 }

@@ -38,6 +38,12 @@ from .frames import IAU_EARTH_FRAME, NS_PER_S, Almanac, Frame
 class MeasurementType(enum.IntEnum):
     Range = abi.MSR_RANGE
     Doppler = abi.MSR_DOPPLER
+    X = abi.MSR_X          # position fixes (PositionDevice), km in the integration frame
+    Y = abi.MSR_Y
+    Z = abi.MSR_Z
+
+
+_POSITION_TYPES = (MeasurementType.X, MeasurementType.Y, MeasurementType.Z)
 
 
 class KalmanVariant(enum.IntEnum):
@@ -150,21 +156,64 @@ class GroundStation:
 
 
 @dataclass
+class PositionDevice:
+    """`PositionDevice` (od/position/mod.rs): GNSS-style position fixes, X, Y and Z of the spacecraft in the integration frame of the
+    estimate.  `with_noise(type, noise)` adds the type to the device's list (in call order) with its noise, as the reference builds it.
+    The filter measures the component at the type's LIST position and differentiates the type's own component (see
+    nyxb_position_device in include/nyxb.h); a bias cancels in the computed observation."""
+
+    name: str
+    measurement_types: List[MeasurementType] = field(default_factory=list)
+    stochastic_noises: Dict[MeasurementType, StochasticNoise] = field(default_factory=dict)
+
+    def with_noise(self, msr_type: MeasurementType, noise: StochasticNoise) -> "PositionDevice":
+        msr_type = MeasurementType(msr_type)
+        self.stochastic_noises[msr_type] = noise
+        if msr_type not in self.measurement_types:
+            self.measurement_types.append(msr_type)
+        return self
+
+    def to_c(self) -> abi.PositionDeviceC:
+        types = list(self.measurement_types)
+        if not 1 <= len(types) <= 3 or len(set(types)) != len(types) or any(t not in _POSITION_TYPES for t in types):
+            raise ODError("a position device carries one to three distinct types of {X, Y, Z}")
+        d = abi.PositionDeviceC()
+        d.n_types = len(types)
+        for i, t in enumerate(types):
+            d.types[i] = int(t)
+            d.noise_var[i] = self.stochastic_noises[t].covariance()
+            d.bias[i] = self.stochastic_noises[t].bias_constant
+        return d
+
+
+@dataclass
 class TrackingDataArc:
     """One tracking schedule (epochs + tracker names) with `n` observation sets: obs[k][type][i], NaN = type not in
-    the measurement's data (both NaN: measurement k absent from arc i)."""
+    the measurement's data (both NaN: measurement k absent from arc i).  `types` names the observation slots: (Range, Doppler), or
+    (X, Y, Z) for position fixes, whose obs is [m][3][n] (all three NaN: absent)."""
 
     epoch_ns: np.ndarray            # [m] int64 ascending
     tracker: List[str]              # [m]
-    obs: np.ndarray                 # [m][2][n] float64
+    obs: np.ndarray                 # [m][len(types)][n] float64
+    types: Sequence[MeasurementType] = (MeasurementType.Range, MeasurementType.Doppler)
+
+    @property
+    def is_position(self) -> bool:
+        return tuple(self.types) == _POSITION_TYPES
 
     def __post_init__(self):
         self.epoch_ns = np.ascontiguousarray(self.epoch_ns, dtype=np.int64)
         self.obs = np.ascontiguousarray(self.obs, dtype=np.float64)
+        self.types = tuple(MeasurementType(t) for t in self.types)
         m = self.epoch_ns.shape[0]
         if self.obs.ndim == 2:
             self.obs = np.ascontiguousarray(self.obs[:, :, None])
-        if len(self.tracker) != m or self.obs.shape[0] != m or self.obs.shape[1] != 2:
+        if self.types not in ((MeasurementType.Range, MeasurementType.Doppler), _POSITION_TYPES):
+            raise ODError("types must be (Range, Doppler) or (X, Y, Z)")
+        if self.is_position:
+            if len(self.tracker) != m or self.obs.shape[0] != m or self.obs.shape[1] != 3:
+                raise ODError("expected epoch_ns[m], tracker[m], obs[m][3][n]")
+        elif len(self.tracker) != m or self.obs.shape[0] != m or self.obs.shape[1] != 2:
             raise ODError("expected epoch_ns[m], tracker[m], obs[m][2][n]")
         if m and np.any(np.diff(self.epoch_ns) < 0):
             raise ODError("measurement epochs must be ascending")
@@ -178,6 +227,7 @@ class TrackingDataArc:
 
     # ---- parquet I/O in the reference's layout (od/msr/trackingdata/io_parquet.rs:43-354): one arc per file
     _COLUMNS = ("Range (km)", "Doppler (km/s)")   # MeasurementType::to_field names (od/msr/types.rs)
+    _POS_COLUMNS = ("X (km)", "Y (km)", "Z (km)")
 
     def to_parquet(self, path, index: int = 0, metadata: Optional[dict] = None):
         """`TrackingDataArc::to_parquet` for the observation set `index`: "Epoch (UTC)", "Tracking device" and one nullable
@@ -194,7 +244,7 @@ class TrackingDataArc:
         cols = [pa.array(epochs_to_utc_iso(self.epoch_ns[present]), type=pa.string()),
                 pa.array([t for t, p in zip(self.tracker, present) if p], type=pa.string())]
         fields = [pa.field("Epoch (UTC)", pa.string(), nullable=False), pa.field("Tracking device", pa.string(), nullable=False)]
-        for c, name in enumerate(self._COLUMNS):
+        for c, name in enumerate(self._POS_COLUMNS if self.is_position else self._COLUMNS):
             v = o[present, c]
             if np.isnan(v).all():
                 continue   # unique_types(): a type no measurement carries has no column
@@ -208,7 +258,8 @@ class TrackingDataArc:
     @classmethod
     def from_parquet(cls, path) -> "TrackingDataArc":
         """`TrackingDataArc::from_parquet` (io_parquet.rs:43-213): needs "Epoch (UTC)", "Tracking device" and at least one of
-        the measurement columns this path knows (range, Doppler); rows are sorted by epoch."""
+        the measurement columns this path knows: range / Doppler, or X / Y / Z (an arc of types (X, Y, Z)), not both kinds; rows are
+        sorted by epoch."""
         import pyarrow.parquet as pq
 
         from .cosmic import utc_iso_to_epochs
@@ -218,16 +269,21 @@ class TrackingDataArc:
         for need in ("Epoch (UTC)", "Tracking device"):
             if need not in names:
                 raise ODError(f"MissingData: {need}")
-        if not names & set(cls._COLUMNS):
-            raise ODError("MissingData: `Range (km)` or `Doppler (km/s)`")
+        ground, pos = bool(names & set(cls._COLUMNS)), bool(names & set(cls._POS_COLUMNS))
+        if ground and pos:
+            raise ODError("range / Doppler and X / Y / Z columns in one arc: one tracker kind per arc")
+        if not ground and not pos:
+            raise ODError("MissingData: `Range (km)`, `Doppler (km/s)` or `X (km)`, `Y (km)`, `Z (km)`")
+        columns = cls._POS_COLUMNS if pos else cls._COLUMNS
         ep = utc_iso_to_epochs(tab["Epoch (UTC)"].to_pylist())
-        obs = np.full((len(ep), 2), np.nan)
-        for c, name in enumerate(cls._COLUMNS):
+        obs = np.full((len(ep), len(columns)), np.nan)
+        for c, name in enumerate(columns):
             if name in names:
                 obs[:, c] = [np.nan if v is None else v for v in tab[name].to_pylist()]
         order = np.argsort(ep, kind="stable")
         trk = tab["Tracking device"].to_pylist()
-        return cls(ep[order], [trk[i] for i in order], obs[order][:, :, None])
+        types = _POSITION_TYPES if pos else (MeasurementType.Range, MeasurementType.Doppler)
+        return cls(ep[order], [trk[i] for i in order], obs[order][:, :, None], types)
 
     def filter_by_offset(self, start_ns: Optional[int] = None, end_ns: Optional[int] = None) -> "TrackingDataArc":
         """`TrackingDataArc::filter_by_offset` (od/msr/trackingdata/mod.rs:394-410) as coded: the measurements in
@@ -239,7 +295,7 @@ class TrackingDataArc:
         lo = first if start_ns is None else first + int(start_ns)
         hi = last if end_ns is None else first + int(end_ns)
         keep = (self.epoch_ns >= lo) & (self.epoch_ns < hi)
-        return TrackingDataArc(self.epoch_ns[keep], [t for t, k in zip(self.tracker, keep) if k], self.obs[keep])
+        return TrackingDataArc(self.epoch_ns[keep], [t for t, k in zip(self.tracker, keep) if k], self.obs[keep], self.types)
 
     @classmethod
     def stack(cls, arcs: Sequence["TrackingDataArc"]) -> "TrackingDataArc":
@@ -248,13 +304,16 @@ class TrackingDataArc:
         keys = sorted({(int(e), t) for a in arcs for e, t in zip(a.epoch_ns, a.tracker)})
         pos = {k: i for i, k in enumerate(keys)}
         n = sum(a.n for a in arcs)
-        obs = np.full((len(keys), 2, n), np.nan)
+        types = arcs[0].types if arcs else (MeasurementType.Range, MeasurementType.Doppler)
+        if any(a.types != types for a in arcs):
+            raise ODError("arcs of different measurement types")
+        obs = np.full((len(keys), len(types), n), np.nan)
         col = 0
         for a in arcs:
             rows = [pos[(int(e), t)] for e, t in zip(a.epoch_ns, a.tracker)]
             obs[rows, :, col:col + a.n] = a.obs
             col += a.n
-        return cls(np.array([k[0] for k in keys], dtype=np.int64), [k[1] for k in keys], obs)
+        return cls(np.array([k[0] for k in keys], dtype=np.int64), [k[1] for k in keys], obs, types)
 
 
 @dataclass(frozen=True)
@@ -493,13 +552,13 @@ class ODSolution:
             src = p + 1 if (self.smoother is not None and p < L - 1) else p
             if res[p] is None:
                 continue
-            mk, w, _, _ = abi.od_tag_fields(int(rec["tag"][src, index]))
+            mk, w, _, _ = self._tag_fields(int(rec["tag"][src, index]))
             tracker[p] = self.arc.tracker[mk] if self.arc is not None else None
             dev = (self.devices or {}).get(tracker[p])
             tl = list(dev.measurement_types) if dev is not None else [MeasurementType.Range, MeasurementType.Doppler]
             types[p] = [int(t) for t in tl[w * M:(w + 1) * M]]
         for label, j in (("Prefit residual", 0), ("Postfit residual", 1)):
-            for mt, un in ((MeasurementType.Range, "km"), (MeasurementType.Doppler, "km/s")):
+            for mt, un in self._residual_types():
                 v = np.full(L, np.nan)
                 for p in range(L):
                     if res[p] is not None and int(mt) in types[p]:
@@ -530,6 +589,20 @@ class ODSolution:
         return path
 
     # ---- estimates, smoothing and statistics (od/process/solution/{mod,smooth,stats}.rs)
+    def _is_position(self) -> bool:
+        return self.arc is not None and self.arc.is_position
+
+    def _tag_fields(self, tag):
+        """(measurement, window, rejected, msr_size) of a record tag, in the layout of the run's tracker kind (NYXB_OD_TAG or
+        NYXB_OD_POS_TAG)."""
+        return abi.od_pos_tag_fields(tag) if self._is_position() else abi.od_tag_fields(tag)
+
+    def _residual_types(self):
+        """(type, unit) of the residual columns: Range / Doppler, or X / Y / Z for position fixes."""
+        if self._is_position():
+            return [(t, "km") for t in _POSITION_TYPES]
+        return [(MeasurementType.Range, "km"), (MeasurementType.Doppler, "km/s")]
+
     def _need_records(self):
         if self.records is None:
             raise ODError("no estimate records: run process_arcs(.., estimates_capacity=K)")
@@ -583,7 +656,7 @@ class ODSolution:
             if tag < 0:
                 out.append(None)
                 continue
-            mk, w, rej, _ = abi.od_tag_fields(tag)
+            mk, w, rej, _ = self._tag_fields(tag)
             slots = [w * M + q for q in range(M)]
             if src != p:
                 post = self.smoother["postfit"][p, slots, i]
@@ -632,10 +705,16 @@ class ODSolution:
             return again.smooth()
         odp = self.process
         frame = self.templates[0].orbit.frame
-        names, st_c = odp.stations_c(frame)
-        tracker = np.array([names.index(t) if t in names else -1 for t in self.arc.tracker], dtype=np.int32)
         eng = odp.prop.engine(frame, odp.almanac)
-        sm = eng.od_smooth_batch(odp.config_c(), len(names), st_c, tracker, self.arc.obs, rec, self.status)
+        pos = odp.is_position
+        if pos:
+            names, dev_c = odp.position_devices_c()
+            tracker = np.array([names.index(t) if t in names else -1 for t in self.arc.tracker], dtype=np.int32)
+            sm = eng.od_position_smooth_batch(odp.config_c(), len(names), dev_c, tracker, self.arc.obs, rec, self.status)
+        else:
+            names, st_c = odp.stations_c(frame)
+            tracker = np.array([names.index(t) if t in names else -1 for t in self.arc.tracker], dtype=np.int32)
+            sm = eng.od_smooth_batch(odp.config_c(), len(names), st_c, tracker, self.arc.obs, rec, self.status)
         sm["filter_postfit"] = self.postfit
         post = np.full(self.postfit.shape, np.nan)
         M = odp.msr_size
@@ -645,7 +724,7 @@ class ODSolution:
             for p in range(self.n_estimates(i) - 1):
                 tag = int(rec["tag"][p + 1, i])
                 if tag >= 0:
-                    mk, w, _, _ = abi.od_tag_fields(tag)
+                    mk, w, _, _ = self._tag_fields(tag)
                     post[mk, w * M:(w + 1) * M, i] = sm["postfit"][p, w * M:(w + 1) * M, i]
         return replace(self, postfit=post, smoother=sm)
 
@@ -683,21 +762,23 @@ class ODSolution:
         _state_columns(cols, schema, est, tmpl, fields)
         _sigma_columns(cols, schema, self.est_covar_diag[rows, :, index], frame.name)
         # residual slots follow the order of the tracker's measurement types (include/nyxb.h: nyxb_od_outputs)
-        slot_type = np.full((len(rows), 2), -1)
+        ns = self.prefit.shape[1]
+        slot_type = np.full((len(rows), ns), -1)
         for a, r in enumerate(rows):
             dev = (self.devices or {}).get(self.arc.tracker[r])
             types = list(dev.measurement_types) if dev is not None else [MeasurementType.Range, MeasurementType.Doppler]
             slot_type[a, :len(types)] = [int(t) for t in types]
         for label, arr in (("Prefit residual", self.prefit), ("Postfit residual", self.postfit)):
-            for mt, un in ((MeasurementType.Range, "km"), (MeasurementType.Doppler, "km/s")):
+            for mt, un in self._residual_types():
                 v = np.full(len(rows), np.nan)
-                for q in range(2):
+                for q in range(ns):
                     hit = slot_type[:, q] == int(mt)
                     v[hit] = arr[rows[hit], q, index]
                 cols.append(pa.array(v, type=pa.float64(), mask=np.isnan(v)))
                 schema.append(pa.field(f"{label}: {mt.name} ({un})", pa.float64(), nullable=True))
         ratio = self.resid_ratio[rows, 0, index]
-        ratio = np.where(np.isnan(ratio), self.resid_ratio[rows, 1, index], ratio)
+        for q in range(1, ns):
+            ratio = np.where(np.isnan(ratio), self.resid_ratio[rows, q, index], ratio)
         cols.append(pa.array(ratio, type=pa.float64(), mask=np.isnan(ratio)))
         schema.append(pa.field("Residual ratio", pa.float64(), nullable=True))
         cols.append(pa.array((self.msr_flags[rows, index] & abi.MSRF_REJECTED) != 0, type=pa.bool_()))
@@ -833,6 +914,21 @@ class KalmanODProcess:
             c.snc_disable_time_ns = int(snc.disable_time)
         return c
 
+    @property
+    def is_position(self) -> bool:
+        """True for a filter over PositionDevices; the reference's `Trk` is one type, so the kinds are never mixed."""
+        kinds = {type(d) for d in self.devices.values()}
+        if len(kinds) > 1:
+            raise ODError("mixed tracker kinds: all devices must be GroundStations or all PositionDevices")
+        return kinds == {PositionDevice}
+
+    def position_devices_c(self):
+        names = list(self.devices)
+        arr = (abi.PositionDeviceC * max(len(names), 1))()
+        for i, nme in enumerate(names):
+            arr[i] = self.devices[nme].to_c()
+        return names, arr
+
     def stations_c(self, frame: Frame):
         names = list(self.devices)
         arr = (abi.GroundStationC * max(len(names), 1))()
@@ -859,11 +955,23 @@ class KalmanODProcess:
         for i, e in enumerate(initial_estimates):
             cov0[:, i] = np.asarray(e.covar, dtype=np.float64).reshape(9, 9).T.reshape(81)  # (c*9 + r)
         eng = self.prop.engine(frame, self.almanac)
-        names, st_c = self.stations_c(frame)
-        tracker = np.array([names.index(t) if t in names else -1 for t in arc.tracker], dtype=np.int32)
-        rec_kw = {} if estimates_capacity is None else {"estimates_capacity": estimates_capacity}
-        res = eng.od_ekf_batch(self.config_c(), len(names), st_c, arc.epoch_ns, tracker, arc.obs, st, cs, ep, cov0,
-                               record_estimates=record_estimates, **rec_kw)
+        if self.is_position:
+            if not arc.is_position:
+                raise ODError("position devices need a tracking arc of types (X, Y, Z)")
+            names, dev_c = self.position_devices_c()
+            tracker = np.array([names.index(t) if t in names else -1 for t in arc.tracker], dtype=np.int32)
+            res = eng.od_position_batch(self.config_c(), len(names), dev_c, arc.epoch_ns, tracker, arc.obs, st, cs, ep, cov0,
+                                        record_estimates=record_estimates, estimates_capacity=estimates_capacity)
+        else:
+            if self.msr_size == 3:
+                raise ODError("msr_size 3 needs position devices")
+            if arc.is_position:
+                raise ODError("ground stations need a tracking arc of types (Range, Doppler)")
+            names, st_c = self.stations_c(frame)
+            tracker = np.array([names.index(t) if t in names else -1 for t in arc.tracker], dtype=np.int32)
+            rec_kw = {} if estimates_capacity is None else {"estimates_capacity": estimates_capacity}
+            res = eng.od_ekf_batch(self.config_c(), len(names), st_c, arc.epoch_ns, tracker, arc.obs, st, cs, ep, cov0,
+                                   record_estimates=record_estimates, **rec_kw)
         res.templates = [e.nominal_state for e in initial_estimates]
         res.arc = arc
         res.devices = self.devices
@@ -1002,6 +1110,8 @@ class BatchLeastSquares:
                  tolerance_pos_km: float = 1e-4, max_iterations: int = 10, max_step: int = 30 * NS_PER_S, epoch_precision: int = 1_000,
                  lm_lambda_init: float = 10.0, lm_lambda_decrease: float = 10.0, lm_lambda_increase: float = 10.0,
                  lm_lambda_min: float = 1e-12, lm_lambda_max: float = 1e12, lm_use_diag_scaling: bool = True):
+        if any(isinstance(d, PositionDevice) for d in devices.values()):
+            raise ODError("batch least squares takes ground stations only")
         self.prop = prop
         self.devices = dict(devices)
         self.almanac = almanac
@@ -1133,3 +1243,21 @@ def simulate_tracking(truth_epochs_ns, truth_states, devices: Dict[str, GroundSt
             noise = rng.normal(0.0, gs.stochastic_noises[t].sigma, n) if rng is not None else 0.0
             obs[k, int(t), :] = np.where(vis, val + noise, np.nan)
     return TrackingDataArc(np.asarray(truth_epochs_ns, dtype=np.int64), list(schedule), obs)
+
+
+def simulate_position_fixes(truth_epochs_ns, truth_states, devices: Dict[str, PositionDevice], schedule: Sequence[str],
+                            rng: Optional[np.random.Generator] = None) -> TrackingDataArc:
+    """Synthetic position fixes of `truth_states[k]` ([m][>=3][n], integration frame) at `truth_epochs_ns[k]` from device
+    `schedule[k]`, as `measure_instantaneous` with an RNG (position/trk_device.rs:76-83): the value of the type at list position ii is
+    position component ii, plus white noise of the type's sigma when `rng` is given, plus the type's constant bias.  Returns an arc of
+    types (X, Y, Z); the types a device does not carry are NaN."""
+    truth_states = np.asarray(truth_states, dtype=np.float64)
+    m, _, n = truth_states.shape
+    obs = np.full((m, 3, n), np.nan)
+    for k in range(m):
+        dev = devices[schedule[k]]
+        for ii, t in enumerate(dev.measurement_types):
+            nz = dev.stochastic_noises[t]
+            noise = rng.normal(0.0, nz.sigma, n) if rng is not None else 0.0
+            obs[k, int(t) - abi.MSR_X, :] = (truth_states[k, ii, :] + noise) + nz.bias_constant
+    return TrackingDataArc(np.asarray(truth_epochs_ns, dtype=np.int64), list(schedule), obs, _POSITION_TYPES)

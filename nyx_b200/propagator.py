@@ -412,6 +412,75 @@ class Engine:
             raise PropagationError(f"nyxb_od_smooth_batch rc={rc}: {abi.last_error()}")
         return r
 
+    def od_position_batch(self, cfg_c, n_devices, devices_c, msr_epoch_ns, msr_tracker, obs, state_soa, consts_soa, epoch0_ns,
+                          covar0_soa, record_estimates: bool = False, estimates_capacity: Optional[int] = None):
+        """`nyxb_od_position_batch`: n sequential Kalman filters over one schedule of position fixes (obs [m][3][n], slot = type - X)
+        in ONE launch; per-measurement outputs [m][3][n].  `record_estimates`: the estimated state and covariance diagonal after each
+        measurement, as od_ekf_batch.  With `estimates_capacity` K the first K estimates of each filter are recorded (tags
+        NYXB_OD_POS_TAG); the filter's results are the same bits."""
+        from .od import ODSolution
+
+        state_soa = np.ascontiguousarray(state_soa, dtype=np.float64)
+        consts_soa = np.ascontiguousarray(consts_soa, dtype=np.float64)
+        epoch0_ns = np.ascontiguousarray(epoch0_ns, dtype=np.int64)
+        covar0_soa = np.ascontiguousarray(covar0_soa, dtype=np.float64)
+        msr_epoch_ns = np.ascontiguousarray(msr_epoch_ns, dtype=np.int64)
+        msr_tracker = np.ascontiguousarray(msr_tracker, dtype=np.int32)
+        obs = np.ascontiguousarray(obs, dtype=np.float64)
+        n = state_soa.shape[1]
+        m = msr_epoch_ns.shape[0]
+        if state_soa.shape != (9, n) or consts_soa.shape != (4, n) or epoch0_ns.shape != (n,) or covar0_soa.shape != (81, n):
+            raise ValueError("expected state[9][n], consts[4][n], epoch0[n], covar0[81][n]")
+        if obs.shape != (m, 3, n) or msr_tracker.shape != (m,):
+            raise ValueError("expected obs[m][3][n], tracker[m]")
+        arc = abi.PositionArcC(m, msr_epoch_ns.ctypes.data, msr_tracker.ctypes.data, obs.ctypes.data)
+        out_state = np.empty((9, n)); out_epoch = np.empty(n, dtype=np.int64); out_cov = np.empty((81, n)); out_dev = np.empty((9, n))
+        ratio = np.full((m, 3, n), np.nan); prefit = np.full((m, 3, n), np.nan); postfit = np.full((m, 3, n), np.nan)
+        flags = np.zeros((m, n), dtype=np.int32)
+        est_state = np.full((m, 9, n), np.nan) if record_estimates else None
+        est_cov = np.full((m, 9, n), np.nan) if record_estimates else None
+        details = np.zeros(n, dtype=abi.DETAILS_DTYPE)
+        status = np.zeros(n, dtype=np.int32)
+        out = abi.OdOutputsC(out_state.ctypes.data, out_epoch.ctypes.data, out_cov.ctypes.data, out_dev.ctypes.data,
+                             ratio.ctypes.data, prefit.ctypes.data, postfit.ctypes.data, flags.ctypes.data,
+                             est_state.ctypes.data if record_estimates else None, est_cov.ctypes.data if record_estimates else None,
+                             details.ctypes.data, status.ctypes.data)
+        records, rec_p = None, None
+        if estimates_capacity is not None:
+            records, rec_c = _od_records(int(estimates_capacity), n)
+            rec_p = C.byref(rec_c)
+        rc = self._lib.nyxb_od_position_batch(self._h, C.byref(cfg_c), int(n_devices), devices_c, C.byref(arc), n,
+                                              state_soa.ctypes.data, consts_soa.ctypes.data, epoch0_ns.ctypes.data,
+                                              covar0_soa.ctypes.data, C.byref(out), rec_p)
+        if rc != 0:
+            raise PropagationError(f"nyxb_od_position_batch rc={rc}: {abi.last_error()}")
+        covar = np.ascontiguousarray(out_cov.T.reshape(n, 9, 9).transpose(0, 2, 1))
+        return ODSolution(out_state, out_epoch, covar, out_dev, ratio, prefit, postfit, flags, est_state, est_cov, details, status,
+                          records=records)
+
+    def od_position_smooth_batch(self, cfg_c, n_devices, devices_c, msr_tracker, obs, records: dict, filter_status, outputs=None):
+        """`nyxb_od_position_smooth_batch`: od_smooth_batch for the records of od_position_batch; postfit is [K][3][n]."""
+        msr_tracker = np.ascontiguousarray(msr_tracker, dtype=np.int32)
+        obs = np.ascontiguousarray(obs, dtype=np.float64)
+        filter_status = np.ascontiguousarray(filter_status, dtype=np.int32)
+        cap, n = records["epoch"].shape
+        m = msr_tracker.shape[0]
+        if obs.shape != (m, 3, n) or filter_status.shape != (n,):
+            raise ValueError("expected obs[m][3][n], filter_status[n]")
+        rec_c = abi.OdRecordsC(cap, *(np.ascontiguousarray(records[k]).ctypes.data for k in _REC_KEYS))
+        shapes = {"state": 9, "deviation": 9, "covar": 81, "fs_ratio": 9, "postfit": 3}
+        want = shapes if outputs is None else {k: shapes[k] for k in outputs}
+        r = {k: np.empty((cap, rows, n)) for k, rows in want.items()}
+        r["status"] = np.zeros(n, dtype=np.int32)
+        out = abi.SmoothOutputsC(*(r[k].ctypes.data if k in r else None for k in ("state", "deviation", "covar", "fs_ratio", "postfit")),
+                                 r["status"].ctypes.data)
+        arc = abi.PositionArcC(m, None, msr_tracker.ctypes.data, obs.ctypes.data)
+        rc = self._lib.nyxb_od_position_smooth_batch(self._h, C.byref(cfg_c), int(n_devices), devices_c, C.byref(arc), n, C.byref(rec_c),
+                                                     filter_status.ctypes.data, C.byref(out))
+        if rc != 0:
+            raise PropagationError(f"nyxb_od_position_smooth_batch rc={rc}: {abi.last_error()}")
+        return r
+
     def _bls_args(self, msr_epoch_ns, msr_tracker, obs, state_soa, consts_soa, epoch0_ns):
         state_soa = np.ascontiguousarray(state_soa, dtype=np.float64)
         consts_soa = np.ascontiguousarray(consts_soa, dtype=np.float64)
