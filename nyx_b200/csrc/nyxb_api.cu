@@ -6,6 +6,7 @@
 #include <cstring>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include <map>
@@ -25,18 +26,6 @@ extern "C" cudaError_t nyxb_launch_thread_fast(const DevSetup*, size_t, const do
                                                const DevSink*, cudaStream_t);
 extern "C" double nyxb_fp64_probe(int device, int iters);
 extern "C" cudaError_t nyxb_launch_frame_shift(const DevBody*, double, size_t, double*, const long long*, int*, cudaStream_t);
-extern "C" cudaError_t nyxb_launch_odpos_coop(const DevSetup*, const DevOdPos*, const OdEstRecords*, const int*, size_t, const double*,
-                                              const double*, const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
-extern "C" cudaError_t nyxb_launch_od_coop(const DevSetup*, const DevOd*, const int*, size_t, const double*, const double*, const long long*,
-                                           double*, long long*, nyxb_details*, int*, cudaStream_t);
-extern "C" cudaError_t nyxb_launch_od_rec_coop(const DevSetup*, const DevOd*, const OdEstRecords*, const int*, size_t, const double*,
-                                               const double*, const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
-extern "C" cudaError_t nyxb_launch_pred_coop(const DevSetup*, const DevOd*, const int*, size_t, const double*, const double*,
-                                             const long long*, const long long*, const double*, const OdRecords*, long long*, double*,
-                                             long long*, nyxb_details*, int*, cudaStream_t);
-extern "C" cudaError_t nyxb_launch_bls_coop(const DevSetup*, const DevOd*, const DevBls*, const int*, size_t, const double*, const double*,
-                                            const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
-extern "C" int nyxb_od_coop_kmax(void);
 extern "C" cudaError_t nyxb_launch_traj_resample(long long, const long long*, const double*, const long long*, size_t, size_t,
                                                  const long long*, double*, int*, cudaStream_t);
 extern "C" cudaError_t nyxb_launch_event_locate(long long, const long long*, const double*, const long long*, size_t, int, double, long long,
@@ -794,21 +783,73 @@ extern "C" int32_t nyxb_propagate_batch_multi(nyxb_engine* const* engines, int32
 // per-call device buffers (these calls run for seconds; allocation cost is irrelevant).
 // ---------------------------------------------------------------------------------------------------------------------
 namespace {
+// The device buffers of one call.  A failed allocation or upload sets `failed`; the call checks it before its launch.
 struct DevBufs {
     std::vector<void*> p;
+    bool failed = false;
     ~DevBufs() { for (void* q : p) cudaFree(q); }
     template <typename T> T* alloc(size_t count) {
         T* d = nullptr;
-        if (cudaMalloc(&d, sizeof(T) * (count ? count : 1)) != cudaSuccess) return nullptr;
+        if (cudaMalloc(&d, sizeof(T) * (count ? count : 1)) != cudaSuccess) { failed = true; return nullptr; }
         p.push_back(d);
         return d;
     }
     template <typename T> T* put(const T* host, size_t count, cudaStream_t st) {
         T* d = alloc<T>(count);
-        if (d && count && cudaMemcpyAsync(d, host, sizeof(T) * count, cudaMemcpyHostToDevice, st) != cudaSuccess) return nullptr;
+        if (d && count && cudaMemcpyAsync(d, host, sizeof(T) * count, cudaMemcpyHostToDevice, st) != cudaSuccess) { failed = true; return nullptr; }
         return d;
     }
+    int32_t check(const char* what = "device allocation / upload failed") const {
+        if (!failed) return NYXB_RC_OK;
+        set_err(what);
+        return NYXB_RC_CUDA;
+    }
 };
+// copies count entries of dev back to host, unless host is null
+template <typename H, typename D>
+cudaError_t get(H* host, const D* dev, size_t count, cudaStream_t st) {
+    static_assert(sizeof(H) == sizeof(D), "host and device entries differ");
+    return host ? cudaMemcpyAsync(host, dev, sizeof(D) * count, cudaMemcpyDeviceToHost, st) : cudaSuccess;
+}
+
+// uploads the per-filter inputs and allocates the per-filter outputs every OD kernel has
+OdIo od_io(DevBufs& B, cudaStream_t st, size_t n, const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns) {
+    return OdIo{B.put(state_soa, 9 * n, st), B.put(consts_soa, 4 * n, st), B.put((const long long*)epoch0_ns, n, st), B.alloc<double>(9 * n),
+                B.alloc<long long>(n), B.alloc<nyxb_details>(n), B.alloc<int>(n)};
+}
+int32_t od_io_get(const OdIo& io, size_t n, cudaStream_t st, double* out_state, int64_t* out_epoch, nyxb_details* out_details, int32_t* out_status) {
+    CUDA_TRY(get(out_state, io.out_state, 9 * n, st));
+    CUDA_TRY(get(out_epoch, io.out_epoch, n, st));
+    CUDA_TRY(get(out_details, io.out_details, n, st));
+    CUDA_TRY(get(out_status, io.out_status, n, st));
+    return NYXB_RC_OK;
+}
+
+// The start and finish of every call below: od_stream selects the engine's device and stream; timed_launch runs one launch between
+// the events ev0 and ev1 and counts it; od_finish waits for the copies back and keeps the kernel time.
+int32_t od_stream(nyxb_engine* eng, cudaStream_t& st) {
+    CUDA_TRY(cudaSetDevice(eng->device));
+    if (!eng->stream) CUDA_TRY(cudaStreamCreateWithFlags(&eng->stream, cudaStreamNonBlocking));
+    st = eng->stream;
+    return NYXB_RC_OK;
+}
+template <class F>
+int32_t timed_launch(nyxb_engine* eng, int family, F launch) {
+    CUDA_TRY(cudaEventRecord(eng->ev0, eng->stream));
+    cudaError_t err = launch();
+    if (err != cudaSuccess) { set_err(std::string("kernel launch: ") + cudaGetErrorString(err)); return NYXB_RC_CUDA; }
+    eng->launches += 1;
+    eng->last_kernel = family;
+    CUDA_TRY(cudaEventRecord(eng->ev1, eng->stream));
+    return NYXB_RC_OK;
+}
+int32_t od_finish(nyxb_engine* eng) {
+    CUDA_TRY(cudaStreamSynchronize(eng->stream));
+    float ms = 0.f;
+    if (cudaEventElapsedTime(&ms, eng->ev0, eng->ev1) == cudaSuccess) eng->last_ms = ms;
+    return NYXB_RC_OK;
+}
+
 bool stm_supported(const nyxb_engine* e) {
     if (e->S.grav_body >= 0 || e->S.n_xgrav > 0 || e->S.state_center >= 0) {
         set_err("the STM / filter kernels take one harmonic field, of the integration centre, and states in the integration frame");
@@ -821,28 +862,42 @@ bool stm_supported(const nyxb_engine* e) {
     }
     return true;
 }
-// Kernel family of the filter and prediction calls.  FAST mode with a gravity field of degree >= 8: one WARP per filter, the harmonic
-// gradient split by columns over the lanes (nyxb_od_coop.cu); columns -> lanes by longest-processing-time, uploaded to d_cols.
-// nyxb_engine_set_kernel(NYXB_KERNEL_THREAD) forces the per-thread kernel, and so does a deal that needs more than
-// nyxb_od_coop_kmax() columns on one lane.  d_cols stays null for the per-thread kernel.
-int32_t od_coop_cols(const nyxb_engine* eng, DevBufs& B, cudaStream_t st, const int*& d_cols) {
-    d_cols = nullptr;
+
+// The column deal of the warp kernels (nyxb_od_coop.cu), used in FAST mode with a gravity field of degree >= 8: one WARP per filter,
+// the harmonic gradient split by columns over the lanes, columns -> lanes by longest-processing-time.  Empty for the per-thread kernel:
+// nyxb_engine_set_kernel(NYXB_KERNEL_THREAD) forces it, and so does a deal that needs more than ODC_KMAX columns on one lane.
+std::vector<int> coop_cols(const nyxb_engine* eng) {
     bool coop = eng->mode == NYXB_MODE_FAST && eng->S.has_grav && eng->S.grav.N >= 8 && eng->kernel != NYXB_KERNEL_THREAD;
-    if (!coop) return NYXB_RC_OK;
-    const int N = eng->S.grav.N, mtop = eng->S.grav.M < N ? eng->S.grav.M : N, kmax = nyxb_od_coop_kmax();
-    std::vector<int> cols(32 * (size_t)kmax, -1), cnt(32, 0);
+    if (!coop) return {};
+    const int N = eng->S.grav.N, mtop = eng->S.grav.M < N ? eng->S.grav.M : N;
+    std::vector<int> cols(32 * (size_t)ODC_KMAX, -1), cnt(32, 0);
     std::vector<long long> load(32, 0);
     for (int m = 0; m <= mtop; ++m) {   // columns in decreasing length order: m = 0, 1 (same length), 2, ...
         int best = 0;
         for (int l = 1; l < 32; ++l)
             if (load[l] < load[best] || (load[l] == load[best] && cnt[l] < cnt[best])) best = l;
-        if (cnt[best] >= kmax) return NYXB_RC_OK;
-        cols[(size_t)best * kmax + cnt[best]++] = m;
+        if (cnt[best] >= ODC_KMAX) return {};
+        cols[(size_t)best * ODC_KMAX + cnt[best]++] = m;
         load[best] += N - (m > 0 ? m : 1) + 1 + 6;   // entries + per-column overhead
     }
-    d_cols = B.put(cols.data(), cols.size(), st);
-    if (!d_cols) { set_err("device allocation / upload failed"); return NYXB_RC_CUDA; }
-    return NYXB_RC_OK;
+    return cols;
+}
+
+template <class Job>
+cudaError_t thread_launch(const nyxb_engine* eng, const Job& job, size_t n, const OdIo& io) {
+    return eng->mode == NYXB_MODE_STRICT ? nyxb_od_strict::launch(eng->S, job, n, io, eng->stream)
+                                         : nyxb_od_fast::launch(eng->S, job, n, io, eng->stream);
+}
+
+// One timed launch of an OD job in the engine's kernel family: warp-cooperative when coop_cols deals the columns (uploaded into B),
+// else per-thread STRICT or FAST.
+template <class Job>
+int32_t od_launch(nyxb_engine* eng, const Job& job, DevBufs& B, size_t n, const OdIo& io) {
+    const std::vector<int> cols = coop_cols(eng);
+    if (cols.empty()) return timed_launch(eng, NYXB_KERNEL_THREAD, [&] { return thread_launch(eng, job, n, io); });
+    const int* d_cols = B.put(cols.data(), cols.size(), eng->stream);
+    if (int32_t rc = B.check()) return rc;
+    return timed_launch(eng, NYXB_KERNEL_COOP, [&] { return nyxb_od_coop_launch(eng->S, job, d_cols, n, io, eng->stream); });
 }
 }  // namespace
 
@@ -856,391 +911,36 @@ extern "C" int32_t nyxb_propagate_batch_stm(nyxb_engine* eng, size_t n, const do
     }
     if (!stm_supported(eng)) return NYXB_RC_UNSUPPORTED;
     if (n == 0) return NYXB_RC_OK;
-    CUDA_TRY(cudaSetDevice(eng->device));
-    if (!eng->stream) CUDA_TRY(cudaStreamCreateWithFlags(&eng->stream, cudaStreamNonBlocking));
-    cudaStream_t st = eng->stream;
+    cudaStream_t st;
+    if (int32_t rc = od_stream(eng, st)) return rc;
     DevBufs B;
-    double* d_state = B.put(state_soa, 9 * n, st);
-    double* d_consts = B.put(consts_soa, 4 * n, st);
-    long long* d_ep = B.put((const long long*)epoch0_ns, n, st);
-    long long* d_step = step_ns ? B.put((const long long*)step_ns, n, st) : nullptr;
-    double* d_stm_in = stm_in_soa ? B.put(stm_in_soa, 81 * n, st) : nullptr;
-    double* d_out = B.alloc<double>(9 * n);
-    double* d_stm = B.alloc<double>(81 * n);
-    long long* d_oep = B.alloc<long long>(n);
-    nyxb_details* d_det = B.alloc<nyxb_details>(n);
-    int* d_status = B.alloc<int>(n);
-    if (!d_state || !d_consts || !d_ep || (step_ns && !d_step) || (stm_in_soa && !d_stm_in) || !d_out || !d_stm || !d_oep || !d_det || !d_status) {
-        set_err("device allocation / upload failed");
-        return NYXB_RC_CUDA;
-    }
-    CUDA_TRY(cudaEventRecord(eng->ev0, st));
-    cudaError_t err = (eng->mode == NYXB_MODE_STRICT)
-        ? nyxb_launch_stm_strict(&eng->S, n, d_state, d_consts, d_ep, end_epoch_ns, d_step, d_stm_in, d_out, d_oep, d_stm, d_det, d_status, st)
-        : nyxb_launch_stm_fast(&eng->S, n, d_state, d_consts, d_ep, end_epoch_ns, d_step, d_stm_in, d_out, d_oep, d_stm, d_det, d_status, st);
-    if (err != cudaSuccess) { set_err(std::string("kernel launch: ") + cudaGetErrorString(err)); return NYXB_RC_CUDA; }
-    eng->launches += 1;
-    eng->last_kernel = NYXB_KERNEL_THREAD;
-    CUDA_TRY(cudaEventRecord(eng->ev1, st));
-    CUDA_TRY(cudaMemcpyAsync(out_state_soa, d_out, sizeof(double) * 9 * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(out_stm_soa, d_stm, sizeof(double) * 81 * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(out_epoch_ns, d_oep, sizeof(long long) * n, cudaMemcpyDeviceToHost, st));
-    if (step_ns) CUDA_TRY(cudaMemcpyAsync(step_ns, d_step, sizeof(long long) * n, cudaMemcpyDeviceToHost, st));
-    if (out_details) CUDA_TRY(cudaMemcpyAsync(out_details, d_det, sizeof(nyxb_details) * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(out_status, d_status, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, eng->ev0, eng->ev1) == cudaSuccess) eng->last_ms = ms;
-    return NYXB_RC_OK;
+    const OdIo io = od_io(B, st, n, state_soa, consts_soa, epoch0_ns);
+    OdStmJob job{end_epoch_ns, step_ns ? B.put((const long long*)step_ns, n, st) : nullptr, stm_in_soa ? B.put(stm_in_soa, 81 * n, st) : nullptr,
+                 B.alloc<double>(81 * n)};
+    if (int32_t rc = B.check()) return rc;
+    if (int32_t rc = timed_launch(eng, NYXB_KERNEL_THREAD, [&] { return thread_launch(eng, job, n, io); })) return rc;
+    if (int32_t rc = od_io_get(io, n, st, out_state_soa, out_epoch_ns, out_details, out_status)) return rc;
+    CUDA_TRY(get(out_stm_soa, job.out_stm, 81 * n, st));
+    CUDA_TRY(get(step_ns, job.step_io, n, st));
+    return od_finish(eng);
 }
 
 namespace {
-// the filter kernel of the engine's family: warp-cooperative when d_cols is set, else per-thread STRICT or FAST; er: null, or the records
-cudaError_t od_launch(const nyxb_engine* eng, const DevOd* od, const OdEstRecords* er, const int* d_cols, size_t n, const double* d_state,
-                      const double* d_consts, const long long* d_ep, double* d_out, long long* d_oep, nyxb_details* d_det, int* d_status,
-                      cudaStream_t st) {
-    const bool coop = d_cols != nullptr;
-    return er
-        ? (coop ? nyxb_launch_od_rec_coop(&eng->S, od, er, d_cols, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
-                : (eng->mode == NYXB_MODE_STRICT)
-                    ? nyxb_launch_od_rec_strict(&eng->S, od, er, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
-                    : nyxb_launch_od_rec_fast(&eng->S, od, er, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st))
-        : coop
-        ? nyxb_launch_od_coop(&eng->S, od, d_cols, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
-        : (eng->mode == NYXB_MODE_STRICT)
-            ? nyxb_launch_od_strict(&eng->S, od, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
-            : nyxb_launch_od_fast(&eng->S, od, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st);
+bool station_ok(const nyxb_engine* eng, const nyxb_ground_station& g) {
+    if (g.n_types < 1 || g.n_types > 2 || (g.body != NYXB_CENTRAL_BODY && (g.body < 0 || g.body >= eng->S.n_bodies))) {
+        set_err("bad ground station descriptor");
+        return false;
+    }
+    return true;
 }
-cudaError_t od_launch(const nyxb_engine* eng, const DevOdPos* od, const OdEstRecords* er, const int* d_cols, size_t n,
-                      const double* d_state, const double* d_consts, const long long* d_ep, double* d_out, long long* d_oep,
-                      nyxb_details* d_det, int* d_status, cudaStream_t st) {
-    if (d_cols) return nyxb_launch_odpos_coop(&eng->S, od, er, d_cols, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st);
-    return (eng->mode == NYXB_MODE_STRICT)
-        ? nyxb_launch_odpos_strict(&eng->S, od, er, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
-        : nyxb_launch_odpos_fast(&eng->S, od, er, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st);
+DevStation pack_station(const nyxb_ground_station& g) {
+    DevStation d{};
+    for (int q = 0; q < 3; ++q) { d.pos[q] = g.pos_fixed_km[q]; d.up[q] = g.up_fixed[q]; }
+    d.mask_deg = g.elevation_mask_deg; d.rot = pack_rot(g.rot); d.body = g.body; d.n_types = g.n_types;
+    for (int q = 0; q < 2; ++q) { d.types[q] = g.types[q]; d.noise_var[q] = g.noise_var[q]; d.bias[q] = g.bias[q]; }
+    d.body_radius = g.body_radius_km;
+    return d;
 }
-
-template <class OD, int NS, class Dev>
-int32_t od_filter_run(nyxb_engine* eng, const nyxb_od_config* cfg, const std::vector<Dev>& hs, int64_t n_msr, const int64_t* arc_epoch,
-                      const int32_t* arc_tracker, const double* arc_obs, size_t n, const double* state_soa, const double* consts_soa,
-                      const int64_t* epoch0_ns, const double* covar0_soa, const nyxb_od_outputs* out, const nyxb_od_records* rec);
-
-// nyxb_od_ekf_batch and nyxb_od_ekf_record_batch: argument checks, packing, one launch, read-back.  rec: null, or the estimate records.
-int32_t od_ekf_run(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations, const nyxb_ground_station* stations,
-                   const nyxb_tracking_arc* arc, size_t n, const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
-                   const double* covar0_soa, const nyxb_od_outputs* out, const nyxb_od_records* rec) {
-    if (!eng || !cfg || !arc || !state_soa || !consts_soa || !epoch0_ns || !covar0_soa || !out || !out->state_soa || !out->epoch_ns ||
-        !out->covar_soa || !out->status || (n_stations > 0 && !stations) || n_stations < 0) {
-        set_err("null argument");
-        return NYXB_RC_BAD_ARG;
-    }
-    if (rec && (rec->capacity < 0 || !rec->count ||
-                (rec->capacity > 0 && (!rec->epoch_ns || !rec->tag || !rec->nominal || !rec->deviation || !rec->covar || !rec->stm)))) {
-        set_err("bad estimate records: count is required, and every record array when capacity > 0");
-        return NYXB_RC_BAD_ARG;
-    }
-    if (!stm_supported(eng)) return NYXB_RC_UNSUPPORTED;
-    if (cfg->msr_size != 1 && cfg->msr_size != 2) { set_err("msr_size must be 1 or 2"); return NYXB_RC_BAD_ARG; }
-    if (cfg->variant != NYXB_KF_REFERENCE_UPDATE && cfg->variant != NYXB_KF_DEVIATION_TRACKING) { set_err("bad filter variant"); return NYXB_RC_BAD_ARG; }
-    if (cfg->max_step_ns <= 0) { set_err("StepSize: max_step must be positive (process/mod.rs:147-150)"); return NYXB_RC_BAD_ARG; }
-    if (arc->n_msr < 2) { set_err("TooFewMeasurements: need 2 (process/mod.rs:139-145)"); return NYXB_RC_BAD_ARG; }
-    if (!arc->epoch_ns || !arc->tracker || !arc->obs) { set_err("null tracking arc arrays"); return NYXB_RC_BAD_ARG; }
-    for (int32_t s = 0; s < n_stations; ++s) {
-        const nyxb_ground_station& g = stations[s];
-        if (g.n_types < 1 || g.n_types > 2 || (g.body != NYXB_CENTRAL_BODY && (g.body < 0 || g.body >= eng->S.n_bodies))) {
-            set_err("bad ground station descriptor");
-            return NYXB_RC_BAD_ARG;
-        }
-        for (int q = 0; q < g.n_types; ++q)
-            if (g.types[q] != NYXB_MSR_RANGE && g.types[q] != NYXB_MSR_DOPPLER) { set_err("unsupported measurement type"); return NYXB_RC_UNSUPPORTED; }
-        if (g.n_types % cfg->msr_size != 0) { set_err("filter misconfigured: measurement types per device must be a multiple of msr_size"); return NYXB_RC_UNSUPPORTED; }
-    }
-    if (n == 0) return NYXB_RC_OK;
-    std::vector<DevStation> hs((size_t)n_stations);
-    for (int32_t s = 0; s < n_stations; ++s) {
-        const nyxb_ground_station& g = stations[s];
-        DevStation& d = hs[s];
-        for (int q = 0; q < 3; ++q) { d.pos[q] = g.pos_fixed_km[q]; d.up[q] = g.up_fixed[q]; }
-        d.mask_deg = g.elevation_mask_deg; d.rot = pack_rot(g.rot); d.body = g.body; d.n_types = g.n_types;
-        for (int q = 0; q < 2; ++q) { d.types[q] = g.types[q]; d.noise_var[q] = g.noise_var[q]; d.bias[q] = g.bias[q]; }
-        d.body_radius = g.body_radius_km;
-    }
-    return od_filter_run<DevOd, 2>(eng, cfg, hs, arc->n_msr, arc->epoch_ns, arc->tracker, arc->obs, n, state_soa, consts_soa, epoch0_ns,
-                                   covar0_soa, out, rec);
-}
-
-// The common part of the ground-station and position-fix filter calls: upload, one launch, read-back.  OD: DevOd or DevOdPos, NS its
-// observation slots; hs: the packed devices.
-template <class OD, int NS, class Dev>
-int32_t od_filter_run(nyxb_engine* eng, const nyxb_od_config* cfg, const std::vector<Dev>& hs, int64_t n_msr, const int64_t* arc_epoch,
-                      const int32_t* arc_tracker, const double* arc_obs, size_t n, const double* state_soa, const double* consts_soa,
-                      const int64_t* epoch0_ns, const double* covar0_soa, const nyxb_od_outputs* out, const nyxb_od_records* rec) {
-    CUDA_TRY(cudaSetDevice(eng->device));
-    if (!eng->stream) CUDA_TRY(cudaStreamCreateWithFlags(&eng->stream, cudaStreamNonBlocking));
-    cudaStream_t st = eng->stream;
-    const size_t m = (size_t)n_msr;
-    const int32_t n_stations = (int32_t)hs.size();
-    DevBufs B;
-    OD od{};
-    od.variant = cfg->variant; od.msr_size = cfg->msr_size; od.reject = cfg->reject_num_sigmas;
-    od.max_step_ns = cfg->max_step_ns; od.eps_ns = cfg->epoch_precision_ns;
-    od.snc_enabled = cfg->snc_enabled; od.snc_frame = cfg->snc_frame;
-    for (int q = 0; q < 3; ++q) od.snc_diag[q] = cfg->snc_diag[q];
-    od.snc_disable_ns = cfg->snc_disable_time_ns;
-    od.n_stations = n_stations;
-    od.stations = B.put(hs.data(), hs.size(), st);
-    od.n_msr = n_msr;
-    od.msr_epoch = B.put((const long long*)arc_epoch, m, st);
-    od.msr_tracker = B.put((const int*)arc_tracker, m, st);
-    od.obs = B.put(arc_obs, m * NS * n, st);
-    od.covar0 = B.put(covar0_soa, 81 * n, st);
-    double* d_state = B.put(state_soa, 9 * n, st);
-    double* d_consts = B.put(consts_soa, 4 * n, st);
-    long long* d_ep = B.put((const long long*)epoch0_ns, n, st);
-    double* d_out = B.alloc<double>(9 * n);
-    long long* d_oep = B.alloc<long long>(n);
-    nyxb_details* d_det = B.alloc<nyxb_details>(n);
-    int* d_status = B.alloc<int>(n);
-    od.covar = B.alloc<double>(81 * n);
-    od.state_dev = out->state_dev_soa ? B.alloc<double>(9 * n) : nullptr;
-    od.ratio = out->resid_ratio ? B.alloc<double>(m * NS * n) : nullptr;
-    od.prefit = out->prefit ? B.alloc<double>(m * NS * n) : nullptr;
-    od.postfit = out->postfit ? B.alloc<double>(m * NS * n) : nullptr;
-    od.flags = out->msr_flags ? B.alloc<int>(m * n) : nullptr;
-    od.est_state = out->est_state ? B.alloc<double>(m * 9 * n) : nullptr;
-    od.est_cov = out->est_covar_diag ? B.alloc<double>(m * 9 * n) : nullptr;
-    if (!od.stations || !od.msr_epoch || !od.msr_tracker || !od.obs || !od.covar0 || !d_state || !d_consts || !d_ep || !d_out || !d_oep ||
-        !d_det || !d_status || !od.covar || (out->state_dev_soa && !od.state_dev) || (out->resid_ratio && !od.ratio) ||
-        (out->prefit && !od.prefit) || (out->postfit && !od.postfit) || (out->msr_flags && !od.flags) ||
-        (out->est_state && !od.est_state) || (out->est_covar_diag && !od.est_cov)) {
-        set_err("device allocation / upload failed");
-        return NYXB_RC_CUDA;
-    }
-    // per-measurement records default to NaN (0xFF bytes) / 0 flags where nothing is written
-    if (od.ratio) CUDA_TRY(cudaMemsetAsync(od.ratio, 0xFF, sizeof(double) * m * NS * n, st));
-    if (od.prefit) CUDA_TRY(cudaMemsetAsync(od.prefit, 0xFF, sizeof(double) * m * NS * n, st));
-    if (od.postfit) CUDA_TRY(cudaMemsetAsync(od.postfit, 0xFF, sizeof(double) * m * NS * n, st));
-    if (od.flags) CUDA_TRY(cudaMemsetAsync(od.flags, 0, sizeof(int) * m * n, st));
-    if (od.est_state) CUDA_TRY(cudaMemsetAsync(od.est_state, 0xFF, sizeof(double) * m * 9 * n, st));
-    if (od.est_cov) CUDA_TRY(cudaMemsetAsync(od.est_cov, 0xFF, sizeof(double) * m * 9 * n, st));
-    OdEstRecords er{};
-    const size_t rcap = rec ? (size_t)rec->capacity : 0;
-    if (rec) {
-        er.cap = (long long)rcap;
-        er.count = B.alloc<long long>(n);
-        if (rcap) {
-            er.epoch = B.alloc<long long>(rcap * n);
-            er.tag = B.alloc<long long>(rcap * n);
-            er.nominal = B.alloc<double>(rcap * 9 * n);
-            er.dev = B.alloc<double>(rcap * 9 * n);
-            er.covar = B.alloc<double>(rcap * 81 * n);
-            er.stm = B.alloc<double>(rcap * 81 * n);
-        }
-        if (!er.count || (rcap && (!er.epoch || !er.tag || !er.nominal || !er.dev || !er.covar || !er.stm))) {
-            set_err("device allocation failed (estimate records)");
-            return NYXB_RC_CUDA;
-        }
-        CUDA_TRY(cudaMemsetAsync(er.count, 0, sizeof(long long) * n, st));
-        if (rcap) {                                  // records a filter does not reach: -1 / NaN
-            CUDA_TRY(cudaMemsetAsync(er.epoch, 0xFF, sizeof(long long) * rcap * n, st));
-            CUDA_TRY(cudaMemsetAsync(er.tag, 0xFF, sizeof(long long) * rcap * n, st));
-            CUDA_TRY(cudaMemsetAsync(er.nominal, 0xFF, sizeof(double) * rcap * 9 * n, st));
-            CUDA_TRY(cudaMemsetAsync(er.dev, 0xFF, sizeof(double) * rcap * 9 * n, st));
-            CUDA_TRY(cudaMemsetAsync(er.covar, 0xFF, sizeof(double) * rcap * 81 * n, st));
-            CUDA_TRY(cudaMemsetAsync(er.stm, 0xFF, sizeof(double) * rcap * 81 * n, st));
-        }
-    }
-    const int* d_cols = nullptr;
-    if (int32_t rc = od_coop_cols(eng, B, st, d_cols)) return rc;
-    const bool coop = d_cols != nullptr;
-    CUDA_TRY(cudaEventRecord(eng->ev0, st));
-    cudaError_t err = od_launch(eng, &od, rec ? &er : nullptr, d_cols, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st);
-    if (err != cudaSuccess) { set_err(std::string("kernel launch: ") + cudaGetErrorString(err)); return NYXB_RC_CUDA; }
-    eng->launches += 1;
-    eng->last_kernel = coop ? NYXB_KERNEL_COOP : NYXB_KERNEL_THREAD;
-    CUDA_TRY(cudaEventRecord(eng->ev1, st));
-    CUDA_TRY(cudaMemcpyAsync(out->state_soa, d_out, sizeof(double) * 9 * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(out->epoch_ns, d_oep, sizeof(long long) * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(out->covar_soa, od.covar, sizeof(double) * 81 * n, cudaMemcpyDeviceToHost, st));
-    if (od.state_dev) CUDA_TRY(cudaMemcpyAsync(out->state_dev_soa, od.state_dev, sizeof(double) * 9 * n, cudaMemcpyDeviceToHost, st));
-    if (od.ratio) CUDA_TRY(cudaMemcpyAsync(out->resid_ratio, od.ratio, sizeof(double) * m * NS * n, cudaMemcpyDeviceToHost, st));
-    if (od.prefit) CUDA_TRY(cudaMemcpyAsync(out->prefit, od.prefit, sizeof(double) * m * NS * n, cudaMemcpyDeviceToHost, st));
-    if (od.postfit) CUDA_TRY(cudaMemcpyAsync(out->postfit, od.postfit, sizeof(double) * m * NS * n, cudaMemcpyDeviceToHost, st));
-    if (od.flags) CUDA_TRY(cudaMemcpyAsync(out->msr_flags, od.flags, sizeof(int) * m * n, cudaMemcpyDeviceToHost, st));
-    if (od.est_state) CUDA_TRY(cudaMemcpyAsync(out->est_state, od.est_state, sizeof(double) * m * 9 * n, cudaMemcpyDeviceToHost, st));
-    if (od.est_cov) CUDA_TRY(cudaMemcpyAsync(out->est_covar_diag, od.est_cov, sizeof(double) * m * 9 * n, cudaMemcpyDeviceToHost, st));
-    if (out->details) CUDA_TRY(cudaMemcpyAsync(out->details, d_det, sizeof(nyxb_details) * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(out->status, d_status, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
-    if (rec) {
-        CUDA_TRY(cudaMemcpyAsync(rec->count, er.count, sizeof(long long) * n, cudaMemcpyDeviceToHost, st));
-        if (rcap) {
-            CUDA_TRY(cudaMemcpyAsync(rec->epoch_ns, er.epoch, sizeof(long long) * rcap * n, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(rec->tag, er.tag, sizeof(long long) * rcap * n, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(rec->nominal, er.nominal, sizeof(double) * rcap * 9 * n, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(rec->deviation, er.dev, sizeof(double) * rcap * 9 * n, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(rec->covar, er.covar, sizeof(double) * rcap * 81 * n, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(rec->stm, er.stm, sizeof(double) * rcap * 81 * n, cudaMemcpyDeviceToHost, st));
-        }
-    }
-    CUDA_TRY(cudaStreamSynchronize(st));
-    float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, eng->ev0, eng->ev1) == cudaSuccess) eng->last_ms = ms;
-    return NYXB_RC_OK;
-}
-}  // namespace
-
-extern "C" int32_t nyxb_od_ekf_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations,
-                                     const nyxb_ground_station* stations, const nyxb_tracking_arc* arc, size_t n,
-                                     const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
-                                     const double* covar0_soa, const nyxb_od_outputs* out) {
-    return od_ekf_run(eng, cfg, n_stations, stations, arc, n, state_soa, consts_soa, epoch0_ns, covar0_soa, out, nullptr);
-}
-
-extern "C" int32_t nyxb_od_ekf_record_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations,
-                                            const nyxb_ground_station* stations, const nyxb_tracking_arc* arc, size_t n,
-                                            const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
-                                            const double* covar0_soa, const nyxb_od_outputs* out, const nyxb_od_records* rec) {
-    if (!rec) { set_err("null argument"); return NYXB_RC_BAD_ARG; }
-    return od_ekf_run(eng, cfg, n_stations, stations, arc, n, state_soa, consts_soa, epoch0_ns, covar0_soa, out, rec);
-}
-
-namespace {
-template <class SM, int NS, class Dev>
-int32_t od_smooth_run(nyxb_engine* eng, int M, const std::vector<Dev>& hs, int64_t n_msr, const int32_t* arc_tracker, const double* arc_obs,
-                      size_t n, const nyxb_od_records* rec, const std::vector<int>& pre, nyxb_smooth_outputs* out);
-}  // namespace
-
-extern "C" int32_t nyxb_od_smooth_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations, const nyxb_ground_station* stations,
-                                        const nyxb_tracking_arc* arc, size_t n, const nyxb_od_records* rec, const int32_t* filter_status,
-                                        nyxb_smooth_outputs* out) {
-    if (!eng || !cfg || !arc || !rec || !filter_status || !out || !out->status || (n_stations > 0 && !stations) || n_stations < 0) {
-        set_err("null argument");
-        return NYXB_RC_BAD_ARG;
-    }
-    if (cfg->msr_size != 1 && cfg->msr_size != 2) { set_err("msr_size must be 1 or 2"); return NYXB_RC_BAD_ARG; }
-    if (rec->capacity < 0 || !rec->count ||
-        (rec->capacity > 0 && (!rec->epoch_ns || !rec->tag || !rec->nominal || !rec->deviation || !rec->covar || !rec->stm))) {
-        set_err("bad estimate records: count is required, and every record array when capacity > 0");
-        return NYXB_RC_BAD_ARG;
-    }
-    if (arc->n_msr < 0 || (arc->n_msr > 0 && (!arc->tracker || !arc->obs))) { set_err("null tracking arc arrays"); return NYXB_RC_BAD_ARG; }
-    for (int32_t s = 0; s < n_stations; ++s) {
-        const nyxb_ground_station& g = stations[s];
-        if (g.n_types < 1 || g.n_types > 2 || (g.body != NYXB_CENTRAL_BODY && (g.body < 0 || g.body >= eng->S.n_bodies))) {
-            set_err("bad ground station descriptor");
-            return NYXB_RC_BAD_ARG;
-        }
-    }
-    const size_t cap = (size_t)rec->capacity;
-    const int M = cfg->msr_size;
-    // per-filter statuses decided on the host; the records of the filters left to smooth must belong to this arc and msr_size
-    std::vector<int> pre(n);
-    for (size_t i = 0; i < n; ++i) {
-        const long long cnt = rec->count[i];
-        pre[i] = filter_status[i] ? filter_status[i]
-               : (cnt > (long long)cap) ? NYXB_ERR_RECORDS_TRUNCATED
-               : (cnt < 2) ? NYXB_ERR_TOO_FEW_MEASUREMENTS : 0;
-        if (pre[i]) continue;
-        for (long long k = 0; k < cnt; ++k) {
-            const int64_t tg = rec->tag[(size_t)k * n + i];
-            if (tg == NYXB_OD_TAG_TIME_UPDATE) continue;
-            const int64_t mk = NYXB_OD_TAG_MSR(tg);
-            const int w = (int)NYXB_OD_TAG_WINDOW(tg);
-            if (tg < 0 || NYXB_OD_TAG_MSR_SIZE(tg) != M) { set_err("estimate records written with another msr_size"); return NYXB_RC_BAD_ARG; }
-            if (mk >= arc->n_msr || arc->tracker[mk] < 0 || arc->tracker[mk] >= n_stations ||
-                (w + 1) * M > stations[arc->tracker[mk]].n_types) {
-                set_err("estimate records do not match this tracking arc");
-                return NYXB_RC_BAD_ARG;
-            }
-        }
-    }
-    for (size_t i = 0; i < n; ++i) out->status[i] = pre[i];
-    if (n == 0 || cap == 0) return NYXB_RC_OK;
-    std::vector<DevStation> hs((size_t)n_stations);
-    for (int32_t s = 0; s < n_stations; ++s) {
-        const nyxb_ground_station& g = stations[s];
-        DevStation& d = hs[s];
-        for (int q = 0; q < 3; ++q) { d.pos[q] = g.pos_fixed_km[q]; d.up[q] = g.up_fixed[q]; }
-        d.mask_deg = g.elevation_mask_deg; d.rot = pack_rot(g.rot); d.body = g.body; d.n_types = g.n_types;
-        for (int q = 0; q < 2; ++q) { d.types[q] = g.types[q]; d.noise_var[q] = g.noise_var[q]; d.bias[q] = g.bias[q]; }
-        d.body_radius = g.body_radius_km;
-    }
-    return od_smooth_run<DevSmooth, 2>(eng, M, hs, arc->n_msr, arc->tracker, arc->obs, n, rec, pre, out);
-}
-
-namespace {
-// The common part of the two smoothing calls: upload, the smoothing launch, read-back.  SM: DevSmooth or DevSmoothPos, NS its
-// observation slots; pre: the statuses decided on the host.
-cudaError_t smooth_launch(const nyxb_engine* eng, const DevSmooth* sm, size_t n, cudaStream_t st) { return nyxb_launch_smooth(&eng->S, sm, n, st); }
-cudaError_t smooth_launch(const nyxb_engine* eng, const DevSmoothPos* sm, size_t n, cudaStream_t st) {
-    return nyxb_launch_smooth_pos(&eng->S, sm, n, st);
-}
-
-template <class SM, int NS, class Dev>
-int32_t od_smooth_run(nyxb_engine* eng, int M, const std::vector<Dev>& hs, int64_t n_msr, const int32_t* arc_tracker, const double* arc_obs,
-                      size_t n, const nyxb_od_records* rec, const std::vector<int>& pre, nyxb_smooth_outputs* out) {
-    CUDA_TRY(cudaSetDevice(eng->device));
-    if (!eng->stream) CUDA_TRY(cudaStreamCreateWithFlags(&eng->stream, cudaStreamNonBlocking));
-    cudaStream_t st = eng->stream;
-    const size_t m = (size_t)n_msr, cap = (size_t)rec->capacity;
-    const int32_t n_stations = (int32_t)hs.size();
-    DevBufs B;
-    SM sm{};
-    sm.msr_size = M;
-    sm.n_stations = n_stations;
-    sm.stations = n_stations ? B.put(hs.data(), hs.size(), st) : nullptr;
-    sm.msr_tracker = m ? B.put((const int*)arc_tracker, m, st) : nullptr;
-    sm.obs = m ? B.put(arc_obs, m * NS * n, st) : nullptr;
-    sm.cap = (long long)cap;
-    sm.epoch = B.put((const long long*)rec->epoch_ns, cap * n, st);
-    sm.tag = B.put((const long long*)rec->tag, cap * n, st);
-    sm.nominal = B.put(rec->nominal, cap * 9 * n, st);
-    sm.dev = B.put(rec->deviation, cap * 9 * n, st);
-    sm.covar = B.put(rec->covar, cap * 81 * n, st);
-    sm.stm = B.put(rec->stm, cap * 81 * n, st);
-    sm.count = B.put((const long long*)rec->count, n, st);
-    sm.pre_status = B.put(pre.data(), n, st);
-    sm.state = out->state ? B.alloc<double>(cap * 9 * n) : nullptr;
-    sm.sdev = out->deviation ? B.alloc<double>(cap * 9 * n) : nullptr;
-    sm.scov = out->covar ? B.alloc<double>(cap * 81 * n) : nullptr;
-    sm.ratio = out->fs_ratio ? B.alloc<double>(cap * 9 * n) : nullptr;
-    sm.postfit = out->postfit ? B.alloc<double>(cap * NS * n) : nullptr;
-    sm.err_key = B.alloc<long long>(n);
-    if ((n_stations && !sm.stations) || (m && (!sm.msr_tracker || !sm.obs)) || !sm.epoch || !sm.tag || !sm.nominal || !sm.dev || !sm.covar ||
-        !sm.stm || !sm.count || !sm.pre_status || (out->state && !sm.state) || (out->deviation && !sm.sdev) || (out->covar && !sm.scov) ||
-        (out->fs_ratio && !sm.ratio) || (out->postfit && !sm.postfit) || !sm.err_key) {
-        set_err("device allocation / upload failed");
-        return NYXB_RC_CUDA;
-    }
-    if (sm.state) CUDA_TRY(cudaMemsetAsync(sm.state, 0xFF, sizeof(double) * cap * 9 * n, st));
-    if (sm.sdev) CUDA_TRY(cudaMemsetAsync(sm.sdev, 0xFF, sizeof(double) * cap * 9 * n, st));
-    if (sm.scov) CUDA_TRY(cudaMemsetAsync(sm.scov, 0xFF, sizeof(double) * cap * 81 * n, st));
-    if (sm.ratio) CUDA_TRY(cudaMemsetAsync(sm.ratio, 0xFF, sizeof(double) * cap * 9 * n, st));
-    if (sm.postfit) CUDA_TRY(cudaMemsetAsync(sm.postfit, 0xFF, sizeof(double) * cap * NS * n, st));
-    CUDA_TRY(cudaMemsetAsync(sm.err_key, 0xFF, sizeof(long long) * n, st));
-    CUDA_TRY(cudaEventRecord(eng->ev0, st));
-    cudaError_t err = smooth_launch(eng, &sm, n, st);
-    if (err != cudaSuccess) { set_err(std::string("kernel launch: ") + cudaGetErrorString(err)); return NYXB_RC_CUDA; }
-    eng->launches += 1;
-    eng->last_kernel = NYXB_KERNEL_THREAD;
-    CUDA_TRY(cudaEventRecord(eng->ev1, st));
-    std::vector<long long> key(n);
-    CUDA_TRY(cudaMemcpyAsync(key.data(), sm.err_key, sizeof(long long) * n, cudaMemcpyDeviceToHost, st));
-    if (sm.state) CUDA_TRY(cudaMemcpyAsync(out->state, sm.state, sizeof(double) * cap * 9 * n, cudaMemcpyDeviceToHost, st));
-    if (sm.sdev) CUDA_TRY(cudaMemcpyAsync(out->deviation, sm.sdev, sizeof(double) * cap * 9 * n, cudaMemcpyDeviceToHost, st));
-    if (sm.scov) CUDA_TRY(cudaMemcpyAsync(out->covar, sm.scov, sizeof(double) * cap * 81 * n, cudaMemcpyDeviceToHost, st));
-    if (sm.ratio) CUDA_TRY(cudaMemcpyAsync(out->fs_ratio, sm.ratio, sizeof(double) * cap * 9 * n, cudaMemcpyDeviceToHost, st));
-    if (sm.postfit) CUDA_TRY(cudaMemcpyAsync(out->postfit, sm.postfit, sizeof(double) * cap * NS * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, eng->ev0, eng->ev1) == cudaSuccess) eng->last_ms = ms;
-    // the reference's error is the first one met going backwards from the last estimate: the largest k (singular before measure);
-    // the outputs of such a filter were set to NaN on the device
-    for (size_t i = 0; i < n; ++i)
-        if (key[i] >= 0) out->status[i] = (key[i] & 1) ? NYXB_ERR_SINGULAR_STM : NYXB_ERR_EPHEMERIS;
-    return NYXB_RC_OK;
-}
-
 // the checks and packing of a position device list (nyxb_od_position_batch / _smooth_batch)
 int32_t pack_position_devices(int32_t n_devices, const nyxb_position_device* devices, std::vector<DevPosDevice>& hs) {
     hs.assign((size_t)(n_devices > 0 ? n_devices : 0), DevPosDevice{});
@@ -1261,53 +961,185 @@ int32_t pack_position_devices(int32_t n_devices, const nyxb_position_device* dev
     }
     return NYXB_RC_OK;
 }
-}  // namespace
+bool records_ok(const nyxb_od_records* rec) {
+    if (rec->capacity < 0 || !rec->count ||
+        (rec->capacity > 0 && (!rec->epoch_ns || !rec->tag || !rec->nominal || !rec->deviation || !rec->covar || !rec->stm))) {
+        set_err("bad estimate records: count is required, and every record array when capacity > 0");
+        return false;
+    }
+    return true;
+}
 
-extern "C" int32_t nyxb_od_position_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_devices, const nyxb_position_device* devices,
-                                          const nyxb_position_arc* arc, size_t n, const double* state_soa, const double* consts_soa,
-                                          const int64_t* epoch0_ns, const double* covar0_soa, const nyxb_od_outputs* out,
-                                          const nyxb_od_records* rec) {
+// The argument checks the ground-station (Dev = DevStation) and position-fix filter calls share, in this order.  The ground-station
+// calls check the engine's setup after the records; nyxb_od_position_batch checks it after its devices.
+template <class Dev, class Arc, class Trk>
+int32_t filter_args(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_dev, const Trk* devs, const Arc* arc, const double* state_soa,
+                    const double* consts_soa, const int64_t* epoch0_ns, const double* covar0_soa, const nyxb_od_outputs* out,
+                    const nyxb_od_records* rec) {
+    constexpr bool ground = std::is_same<Dev, DevStation>::value;
     if (!eng || !cfg || !arc || !state_soa || !consts_soa || !epoch0_ns || !covar0_soa || !out || !out->state_soa || !out->epoch_ns ||
-        !out->covar_soa || !out->status || (n_devices > 0 && !devices) || n_devices < 0) {
+        !out->covar_soa || !out->status || (n_dev > 0 && !devs) || n_dev < 0) {
         set_err("null argument");
         return NYXB_RC_BAD_ARG;
     }
-    if (rec && (rec->capacity < 0 || !rec->count ||
-                (rec->capacity > 0 && (!rec->epoch_ns || !rec->tag || !rec->nominal || !rec->deviation || !rec->covar || !rec->stm)))) {
-        set_err("bad estimate records: count is required, and every record array when capacity > 0");
-        return NYXB_RC_BAD_ARG;
-    }
-    if (cfg->msr_size < 1 || cfg->msr_size > 3) { set_err("msr_size must be 1, 2 or 3"); return NYXB_RC_BAD_ARG; }
+    if (rec && !records_ok(rec)) return NYXB_RC_BAD_ARG;
+    if (ground && !stm_supported(eng)) return NYXB_RC_UNSUPPORTED;
+    if (cfg->msr_size < 1 || cfg->msr_size > Dev::NS) { set_err(ground ? "msr_size must be 1 or 2" : "msr_size must be 1, 2 or 3"); return NYXB_RC_BAD_ARG; }
     if (cfg->variant != NYXB_KF_REFERENCE_UPDATE && cfg->variant != NYXB_KF_DEVIATION_TRACKING) { set_err("bad filter variant"); return NYXB_RC_BAD_ARG; }
     if (cfg->max_step_ns <= 0) { set_err("StepSize: max_step must be positive (process/mod.rs:147-150)"); return NYXB_RC_BAD_ARG; }
     if (arc->n_msr < 2) { set_err("TooFewMeasurements: need 2 (process/mod.rs:139-145)"); return NYXB_RC_BAD_ARG; }
     if (!arc->epoch_ns || !arc->tracker || !arc->obs) { set_err("null tracking arc arrays"); return NYXB_RC_BAD_ARG; }
-    std::vector<DevPosDevice> hs;
-    if (int32_t rc = pack_position_devices(n_devices, devices, hs)) return rc;
-    if (!stm_supported(eng)) return NYXB_RC_UNSUPPORTED;
-    if (n == 0) return NYXB_RC_OK;
-    return od_filter_run<DevOdPos, 3>(eng, cfg, hs, arc->n_msr, arc->epoch_ns, arc->tracker, arc->obs, n, state_soa, consts_soa, epoch0_ns,
-                                      covar0_soa, out, rec);
+    return NYXB_RC_OK;
 }
 
-extern "C" int32_t nyxb_od_position_smooth_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_devices,
-                                                 const nyxb_position_device* devices, const nyxb_position_arc* arc, size_t n,
-                                                 const nyxb_od_records* rec, const int32_t* filter_status, nyxb_smooth_outputs* out) {
-    if (!eng || !cfg || !arc || !rec || !filter_status || !out || !out->status || (n_devices > 0 && !devices) || n_devices < 0) {
-        set_err("null argument");
-        return NYXB_RC_BAD_ARG;
+// The common part of the ground-station and position-fix filter calls: upload, one launch, read-back.  hs: the packed devices;
+// rec: null, or the estimate records.
+template <class Dev>
+int32_t od_filter_run(nyxb_engine* eng, const nyxb_od_config* cfg, const std::vector<Dev>& hs, int64_t n_msr, const int64_t* arc_epoch,
+                      const int32_t* arc_tracker, const double* arc_obs, size_t n, const double* state_soa, const double* consts_soa,
+                      const int64_t* epoch0_ns, const double* covar0_soa, const nyxb_od_outputs* out, const nyxb_od_records* rec) {
+    constexpr int NS = Dev::NS;
+    cudaStream_t st;
+    if (int32_t rc = od_stream(eng, st)) return rc;
+    const size_t m = (size_t)n_msr;
+    DevBufs B;
+    DevOdT<Dev> od{};
+    od.variant = cfg->variant; od.msr_size = cfg->msr_size; od.reject = cfg->reject_num_sigmas;
+    od.max_step_ns = cfg->max_step_ns; od.eps_ns = cfg->epoch_precision_ns;
+    od.snc_enabled = cfg->snc_enabled; od.snc_frame = cfg->snc_frame;
+    for (int q = 0; q < 3; ++q) od.snc_diag[q] = cfg->snc_diag[q];
+    od.snc_disable_ns = cfg->snc_disable_time_ns;
+    od.n_stations = (int32_t)hs.size();
+    od.stations = B.put(hs.data(), hs.size(), st);
+    od.n_msr = n_msr;
+    od.msr_epoch = B.put((const long long*)arc_epoch, m, st);
+    od.msr_tracker = B.put((const int*)arc_tracker, m, st);
+    od.obs = B.put(arc_obs, m * NS * n, st);
+    od.covar0 = B.put(covar0_soa, 81 * n, st);
+    const OdIo io = od_io(B, st, n, state_soa, consts_soa, epoch0_ns);
+    od.covar = B.alloc<double>(81 * n);
+    od.state_dev = out->state_dev_soa ? B.alloc<double>(9 * n) : nullptr;
+    od.ratio = out->resid_ratio ? B.alloc<double>(m * NS * n) : nullptr;
+    od.prefit = out->prefit ? B.alloc<double>(m * NS * n) : nullptr;
+    od.postfit = out->postfit ? B.alloc<double>(m * NS * n) : nullptr;
+    od.flags = out->msr_flags ? B.alloc<int>(m * n) : nullptr;
+    od.est_state = out->est_state ? B.alloc<double>(m * 9 * n) : nullptr;
+    od.est_cov = out->est_covar_diag ? B.alloc<double>(m * 9 * n) : nullptr;
+    if (int32_t rc = B.check()) return rc;
+    OdEstRecords er{};
+    const size_t rcap = rec ? (size_t)rec->capacity : 0;
+    if (rec) {
+        er.cap = (long long)rcap;
+        er.count = B.alloc<long long>(n);
+        if (rcap) {
+            er.epoch = B.alloc<long long>(rcap * n);
+            er.tag = B.alloc<long long>(rcap * n);
+            er.nominal = B.alloc<double>(rcap * 9 * n);
+            er.dev = B.alloc<double>(rcap * 9 * n);
+            er.covar = B.alloc<double>(rcap * 81 * n);
+            er.stm = B.alloc<double>(rcap * 81 * n);
+        }
+        if (int32_t rc = B.check("device allocation failed (estimate records)")) return rc;
     }
-    if (cfg->msr_size < 1 || cfg->msr_size > 3) { set_err("msr_size must be 1, 2 or 3"); return NYXB_RC_BAD_ARG; }
-    if (rec->capacity < 0 || !rec->count ||
-        (rec->capacity > 0 && (!rec->epoch_ns || !rec->tag || !rec->nominal || !rec->deviation || !rec->covar || !rec->stm))) {
-        set_err("bad estimate records: count is required, and every record array when capacity > 0");
-        return NYXB_RC_BAD_ARG;
+    // per-measurement records default to NaN (0xFF bytes) / 0 flags where nothing is written
+    if (od.ratio) CUDA_TRY(cudaMemsetAsync(od.ratio, 0xFF, sizeof(double) * m * NS * n, st));
+    if (od.prefit) CUDA_TRY(cudaMemsetAsync(od.prefit, 0xFF, sizeof(double) * m * NS * n, st));
+    if (od.postfit) CUDA_TRY(cudaMemsetAsync(od.postfit, 0xFF, sizeof(double) * m * NS * n, st));
+    if (od.flags) CUDA_TRY(cudaMemsetAsync(od.flags, 0, sizeof(int) * m * n, st));
+    if (od.est_state) CUDA_TRY(cudaMemsetAsync(od.est_state, 0xFF, sizeof(double) * m * 9 * n, st));
+    if (od.est_cov) CUDA_TRY(cudaMemsetAsync(od.est_cov, 0xFF, sizeof(double) * m * 9 * n, st));
+    if (rec) CUDA_TRY(cudaMemsetAsync(er.count, 0, sizeof(long long) * n, st));
+    if (rcap) {                                  // records a filter does not reach: -1 / NaN
+        CUDA_TRY(cudaMemsetAsync(er.epoch, 0xFF, sizeof(long long) * rcap * n, st));
+        CUDA_TRY(cudaMemsetAsync(er.tag, 0xFF, sizeof(long long) * rcap * n, st));
+        CUDA_TRY(cudaMemsetAsync(er.nominal, 0xFF, sizeof(double) * rcap * 9 * n, st));
+        CUDA_TRY(cudaMemsetAsync(er.dev, 0xFF, sizeof(double) * rcap * 9 * n, st));
+        CUDA_TRY(cudaMemsetAsync(er.covar, 0xFF, sizeof(double) * rcap * 81 * n, st));
+        CUDA_TRY(cudaMemsetAsync(er.stm, 0xFF, sizeof(double) * rcap * 81 * n, st));
     }
-    if (arc->n_msr < 0 || (arc->n_msr > 0 && (!arc->tracker || !arc->obs))) { set_err("null tracking arc arrays"); return NYXB_RC_BAD_ARG; }
-    std::vector<DevPosDevice> hs;
-    if (int32_t rc = pack_position_devices(n_devices, devices, hs)) return rc;
-    const size_t cap = (size_t)rec->capacity;
-    const int M = cfg->msr_size;
+    if (int32_t rc = rec ? od_launch(eng, OdFilterJob<Dev, true>{od, er}, B, n, io) : od_launch(eng, OdFilterJob<Dev, false>{od}, B, n, io))
+        return rc;
+    if (int32_t rc = od_io_get(io, n, st, out->state_soa, out->epoch_ns, out->details, out->status)) return rc;
+    CUDA_TRY(get(out->covar_soa, od.covar, 81 * n, st));
+    CUDA_TRY(get(out->state_dev_soa, od.state_dev, 9 * n, st));
+    CUDA_TRY(get(out->resid_ratio, od.ratio, m * NS * n, st));
+    CUDA_TRY(get(out->prefit, od.prefit, m * NS * n, st));
+    CUDA_TRY(get(out->postfit, od.postfit, m * NS * n, st));
+    CUDA_TRY(get(out->msr_flags, od.flags, m * n, st));
+    CUDA_TRY(get(out->est_state, od.est_state, m * 9 * n, st));
+    CUDA_TRY(get(out->est_covar_diag, od.est_cov, m * 9 * n, st));
+    if (rec) CUDA_TRY(get(rec->count, er.count, n, st));
+    if (rcap) {
+        CUDA_TRY(get(rec->epoch_ns, er.epoch, rcap * n, st));
+        CUDA_TRY(get(rec->tag, er.tag, rcap * n, st));
+        CUDA_TRY(get(rec->nominal, er.nominal, rcap * 9 * n, st));
+        CUDA_TRY(get(rec->deviation, er.dev, rcap * 9 * n, st));
+        CUDA_TRY(get(rec->covar, er.covar, rcap * 81 * n, st));
+        CUDA_TRY(get(rec->stm, er.stm, rcap * 81 * n, st));
+    }
+    return od_finish(eng);
+}
+
+// nyxb_od_ekf_batch and nyxb_od_ekf_record_batch: argument checks, packing, one launch, read-back.  rec: null, or the estimate records.
+int32_t od_ekf_run(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations, const nyxb_ground_station* stations,
+                   const nyxb_tracking_arc* arc, size_t n, const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
+                   const double* covar0_soa, const nyxb_od_outputs* out, const nyxb_od_records* rec) {
+    if (int32_t rc = filter_args<DevStation>(eng, cfg, n_stations, stations, arc, state_soa, consts_soa, epoch0_ns, covar0_soa, out, rec))
+        return rc;
+    std::vector<DevStation> hs;
+    for (int32_t s = 0; s < n_stations; ++s) {
+        const nyxb_ground_station& g = stations[s];
+        if (!station_ok(eng, g)) return NYXB_RC_BAD_ARG;
+        for (int q = 0; q < g.n_types; ++q)
+            if (g.types[q] != NYXB_MSR_RANGE && g.types[q] != NYXB_MSR_DOPPLER) { set_err("unsupported measurement type"); return NYXB_RC_UNSUPPORTED; }
+        if (g.n_types % cfg->msr_size != 0) { set_err("filter misconfigured: measurement types per device must be a multiple of msr_size"); return NYXB_RC_UNSUPPORTED; }
+        hs.push_back(pack_station(g));
+    }
+    if (n == 0) return NYXB_RC_OK;
+    return od_filter_run(eng, cfg, hs, arc->n_msr, arc->epoch_ns, arc->tracker, arc->obs, n, state_soa, consts_soa, epoch0_ns, covar0_soa,
+                         out, rec);
+}
+}  // namespace
+
+extern "C" int32_t nyxb_od_ekf_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations,
+                                     const nyxb_ground_station* stations, const nyxb_tracking_arc* arc, size_t n,
+                                     const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
+                                     const double* covar0_soa, const nyxb_od_outputs* out) {
+    return od_ekf_run(eng, cfg, n_stations, stations, arc, n, state_soa, consts_soa, epoch0_ns, covar0_soa, out, nullptr);
+}
+
+extern "C" int32_t nyxb_od_ekf_record_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations,
+                                            const nyxb_ground_station* stations, const nyxb_tracking_arc* arc, size_t n,
+                                            const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
+                                            const double* covar0_soa, const nyxb_od_outputs* out, const nyxb_od_records* rec) {
+    if (!rec) { set_err("null argument"); return NYXB_RC_BAD_ARG; }
+    return od_ekf_run(eng, cfg, n_stations, stations, arc, n, state_soa, consts_soa, epoch0_ns, covar0_soa, out, rec);
+}
+
+namespace {
+// The record tags and windows of each tracker kind (NYXB_OD_TAG_*, NYXB_OD_POS_TAG_*, include/nyxb.h).  A ground station's window must
+// lie within its types; a position device's window need only start within them.
+struct GroundTags {
+    static int64_t msr(int64_t tg) { return NYXB_OD_TAG_MSR(tg); }
+    static int window(int64_t tg) { return (int)NYXB_OD_TAG_WINDOW(tg); }
+    static int64_t msr_size(int64_t tg) { return NYXB_OD_TAG_MSR_SIZE(tg); }
+    static bool outside(int w, int M, int n_types) { return (w + 1) * M > n_types; }
+};
+struct PosTags {
+    static int64_t msr(int64_t tg) { return NYXB_OD_POS_TAG_MSR(tg); }
+    static int window(int64_t tg) { return (int)NYXB_OD_POS_TAG_WINDOW(tg); }
+    static int64_t msr_size(int64_t tg) { return NYXB_OD_POS_TAG_MSR_SIZE(tg); }
+    static bool outside(int w, int M, int n_types) { return w * M >= n_types; }
+};
+
+// The common part of the two smoothing calls: the per-filter statuses decided on the host, then upload, the smoothing launch and
+// read-back.  The records of the filters left to smooth must belong to this arc and msr_size.  hs: the packed devices.
+template <class Tags, class Dev>
+int32_t od_smooth_run(nyxb_engine* eng, int M, const std::vector<Dev>& hs, int64_t n_msr, const int32_t* arc_tracker, const double* arc_obs,
+                      size_t n, const nyxb_od_records* rec, const int32_t* filter_status, nyxb_smooth_outputs* out) {
+    constexpr int NS = Dev::NS;
+    const size_t m = (size_t)n_msr, cap = (size_t)rec->capacity;
+    const int32_t n_stations = (int32_t)hs.size();
     std::vector<int> pre(n);
     for (size_t i = 0; i < n; ++i) {
         const long long cnt = rec->count[i];
@@ -1318,10 +1150,10 @@ extern "C" int32_t nyxb_od_position_smooth_batch(nyxb_engine* eng, const nyxb_od
         for (long long k = 0; k < cnt; ++k) {
             const int64_t tg = rec->tag[(size_t)k * n + i];
             if (tg == NYXB_OD_TAG_TIME_UPDATE) continue;
-            const int64_t mk = NYXB_OD_POS_TAG_MSR(tg);
-            const int w = (int)NYXB_OD_POS_TAG_WINDOW(tg);
-            if (tg < 0 || NYXB_OD_POS_TAG_MSR_SIZE(tg) != M) { set_err("estimate records written with another msr_size"); return NYXB_RC_BAD_ARG; }
-            if (mk >= arc->n_msr || arc->tracker[mk] < 0 || arc->tracker[mk] >= n_devices || w * M >= hs[arc->tracker[mk]].n_types) {
+            const int64_t mk = Tags::msr(tg);
+            const int w = Tags::window(tg);
+            if (tg < 0 || Tags::msr_size(tg) != M) { set_err("estimate records written with another msr_size"); return NYXB_RC_BAD_ARG; }
+            if (mk >= n_msr || arc_tracker[mk] < 0 || arc_tracker[mk] >= n_stations || Tags::outside(w, M, hs[arc_tracker[mk]].n_types)) {
                 set_err("estimate records do not match this tracking arc");
                 return NYXB_RC_BAD_ARG;
             }
@@ -1329,7 +1161,99 @@ extern "C" int32_t nyxb_od_position_smooth_batch(nyxb_engine* eng, const nyxb_od
     }
     for (size_t i = 0; i < n; ++i) out->status[i] = pre[i];
     if (n == 0 || cap == 0) return NYXB_RC_OK;
-    return od_smooth_run<DevSmoothPos, 3>(eng, M, hs, arc->n_msr, arc->tracker, arc->obs, n, rec, pre, out);
+    cudaStream_t st;
+    if (int32_t rc = od_stream(eng, st)) return rc;
+    DevBufs B;
+    DevSmoothT<Dev> sm{};
+    sm.msr_size = M;
+    sm.n_stations = n_stations;
+    sm.stations = n_stations ? B.put(hs.data(), hs.size(), st) : nullptr;
+    sm.msr_tracker = m ? B.put((const int*)arc_tracker, m, st) : nullptr;
+    sm.obs = m ? B.put(arc_obs, m * NS * n, st) : nullptr;
+    sm.cap = (long long)cap;
+    sm.epoch = B.put((const long long*)rec->epoch_ns, cap * n, st);
+    sm.tag = B.put((const long long*)rec->tag, cap * n, st);
+    sm.nominal = B.put(rec->nominal, cap * 9 * n, st);
+    sm.dev = B.put(rec->deviation, cap * 9 * n, st);
+    sm.covar = B.put(rec->covar, cap * 81 * n, st);
+    sm.stm = B.put(rec->stm, cap * 81 * n, st);
+    sm.count = B.put((const long long*)rec->count, n, st);
+    sm.pre_status = B.put(pre.data(), n, st);
+    sm.state = out->state ? B.alloc<double>(cap * 9 * n) : nullptr;
+    sm.sdev = out->deviation ? B.alloc<double>(cap * 9 * n) : nullptr;
+    sm.scov = out->covar ? B.alloc<double>(cap * 81 * n) : nullptr;
+    sm.ratio = out->fs_ratio ? B.alloc<double>(cap * 9 * n) : nullptr;
+    sm.postfit = out->postfit ? B.alloc<double>(cap * NS * n) : nullptr;
+    sm.err_key = B.alloc<long long>(n);
+    if (int32_t rc = B.check()) return rc;
+    if (sm.state) CUDA_TRY(cudaMemsetAsync(sm.state, 0xFF, sizeof(double) * cap * 9 * n, st));
+    if (sm.sdev) CUDA_TRY(cudaMemsetAsync(sm.sdev, 0xFF, sizeof(double) * cap * 9 * n, st));
+    if (sm.scov) CUDA_TRY(cudaMemsetAsync(sm.scov, 0xFF, sizeof(double) * cap * 81 * n, st));
+    if (sm.ratio) CUDA_TRY(cudaMemsetAsync(sm.ratio, 0xFF, sizeof(double) * cap * 9 * n, st));
+    if (sm.postfit) CUDA_TRY(cudaMemsetAsync(sm.postfit, 0xFF, sizeof(double) * cap * NS * n, st));
+    CUDA_TRY(cudaMemsetAsync(sm.err_key, 0xFF, sizeof(long long) * n, st));
+    if (int32_t rc = timed_launch(eng, NYXB_KERNEL_THREAD, [&] { return nyxb_smooth_launch(eng->S, sm, n, st); })) return rc;
+    std::vector<long long> key(n);
+    CUDA_TRY(get(key.data(), sm.err_key, n, st));
+    CUDA_TRY(get(out->state, sm.state, cap * 9 * n, st));
+    CUDA_TRY(get(out->deviation, sm.sdev, cap * 9 * n, st));
+    CUDA_TRY(get(out->covar, sm.scov, cap * 81 * n, st));
+    CUDA_TRY(get(out->fs_ratio, sm.ratio, cap * 9 * n, st));
+    CUDA_TRY(get(out->postfit, sm.postfit, cap * NS * n, st));
+    if (int32_t rc = od_finish(eng)) return rc;
+    // the reference's error is the first one met going backwards from the last estimate: the largest k (singular before measure);
+    // the outputs of such a filter were set to NaN on the device
+    for (size_t i = 0; i < n; ++i)
+        if (key[i] >= 0) out->status[i] = (key[i] & 1) ? NYXB_ERR_SINGULAR_STM : NYXB_ERR_EPHEMERIS;
+    return NYXB_RC_OK;
+}
+}  // namespace
+
+extern "C" int32_t nyxb_od_smooth_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations, const nyxb_ground_station* stations,
+                                        const nyxb_tracking_arc* arc, size_t n, const nyxb_od_records* rec, const int32_t* filter_status,
+                                        nyxb_smooth_outputs* out) {
+    if (!eng || !cfg || !arc || !rec || !filter_status || !out || !out->status || (n_stations > 0 && !stations) || n_stations < 0) {
+        set_err("null argument");
+        return NYXB_RC_BAD_ARG;
+    }
+    if (cfg->msr_size != 1 && cfg->msr_size != 2) { set_err("msr_size must be 1 or 2"); return NYXB_RC_BAD_ARG; }
+    if (!records_ok(rec)) return NYXB_RC_BAD_ARG;
+    if (arc->n_msr < 0 || (arc->n_msr > 0 && (!arc->tracker || !arc->obs))) { set_err("null tracking arc arrays"); return NYXB_RC_BAD_ARG; }
+    std::vector<DevStation> hs;
+    for (int32_t s = 0; s < n_stations; ++s) {
+        if (!station_ok(eng, stations[s])) return NYXB_RC_BAD_ARG;
+        hs.push_back(pack_station(stations[s]));
+    }
+    return od_smooth_run<GroundTags>(eng, cfg->msr_size, hs, arc->n_msr, arc->tracker, arc->obs, n, rec, filter_status, out);
+}
+
+extern "C" int32_t nyxb_od_position_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_devices, const nyxb_position_device* devices,
+                                          const nyxb_position_arc* arc, size_t n, const double* state_soa, const double* consts_soa,
+                                          const int64_t* epoch0_ns, const double* covar0_soa, const nyxb_od_outputs* out,
+                                          const nyxb_od_records* rec) {
+    if (int32_t rc = filter_args<DevPosDevice>(eng, cfg, n_devices, devices, arc, state_soa, consts_soa, epoch0_ns, covar0_soa, out, rec))
+        return rc;
+    std::vector<DevPosDevice> hs;
+    if (int32_t rc = pack_position_devices(n_devices, devices, hs)) return rc;
+    if (!stm_supported(eng)) return NYXB_RC_UNSUPPORTED;
+    if (n == 0) return NYXB_RC_OK;
+    return od_filter_run(eng, cfg, hs, arc->n_msr, arc->epoch_ns, arc->tracker, arc->obs, n, state_soa, consts_soa, epoch0_ns, covar0_soa,
+                         out, rec);
+}
+
+extern "C" int32_t nyxb_od_position_smooth_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_devices,
+                                                 const nyxb_position_device* devices, const nyxb_position_arc* arc, size_t n,
+                                                 const nyxb_od_records* rec, const int32_t* filter_status, nyxb_smooth_outputs* out) {
+    if (!eng || !cfg || !arc || !rec || !filter_status || !out || !out->status || (n_devices > 0 && !devices) || n_devices < 0) {
+        set_err("null argument");
+        return NYXB_RC_BAD_ARG;
+    }
+    if (cfg->msr_size < 1 || cfg->msr_size > 3) { set_err("msr_size must be 1, 2 or 3"); return NYXB_RC_BAD_ARG; }
+    if (!records_ok(rec)) return NYXB_RC_BAD_ARG;
+    if (arc->n_msr < 0 || (arc->n_msr > 0 && (!arc->tracker || !arc->obs))) { set_err("null tracking arc arrays"); return NYXB_RC_BAD_ARG; }
+    std::vector<DevPosDevice> hs;
+    if (int32_t rc = pack_position_devices(n_devices, devices, hs)) return rc;
+    return od_smooth_run<PosTags>(eng, cfg->msr_size, hs, arc->n_msr, arc->tracker, arc->obs, n, rec, filter_status, out);
 }
 
 extern "C" int32_t nyxb_od_predict_batch(nyxb_engine* eng, const nyxb_od_config* cfg, size_t n, const double* state_soa,
@@ -1347,12 +1271,12 @@ extern "C" int32_t nyxb_od_predict_batch(nyxb_engine* eng, const nyxb_od_config*
     if (out->capacity < 0) { set_err("negative record capacity"); return NYXB_RC_BAD_ARG; }
     if (!stm_supported(eng)) return NYXB_RC_UNSUPPORTED;
     if (n == 0) return NYXB_RC_OK;
-    CUDA_TRY(cudaSetDevice(eng->device));
-    if (!eng->stream) CUDA_TRY(cudaStreamCreateWithFlags(&eng->stream, cudaStreamNonBlocking));
-    cudaStream_t st = eng->stream;
+    cudaStream_t st;
+    if (int32_t rc = od_stream(eng, st)) return rc;
     const size_t cap = (size_t)out->capacity;
     DevBufs B;
-    DevOd od{};
+    OdPredictJob job{};
+    DevOd& od = job.od;
     od.variant = cfg->variant;
     od.max_step_ns = cfg->max_step_ns;
     od.snc_enabled = cfg->snc_enabled; od.snc_frame = cfg->snc_frame;
@@ -1361,54 +1285,25 @@ extern "C" int32_t nyxb_od_predict_batch(nyxb_engine* eng, const nyxb_od_config*
     od.covar0 = B.put(covar0_soa, 81 * n, st);
     od.covar = B.alloc<double>(81 * n);
     od.state_dev = out->state_dev_soa ? B.alloc<double>(9 * n) : nullptr;
-    double* d_state = B.put(state_soa, 9 * n, st);
-    double* d_consts = B.put(consts_soa, 4 * n, st);
-    long long* d_ep = B.put((const long long*)epoch0_ns, n, st);
-    long long* d_end = B.put((const long long*)end_epoch_ns, n, st);
-    double* d_dev0 = state_dev0_soa ? B.put(state_dev0_soa, 9 * n, st) : nullptr;
-    double* d_out = B.alloc<double>(9 * n);
-    long long* d_oep = B.alloc<long long>(n);
-    nyxb_details* d_det = B.alloc<nyxb_details>(n);
-    int* d_status = B.alloc<int>(n);
-    long long* d_cnt = out->rec_count ? B.alloc<long long>(n) : nullptr;
-    OdRecords rec{ (long long)cap, nullptr, nullptr };
-    if (cap && out->rec_state) rec.state = B.alloc<double>(cap * 9 * n);
-    if (cap && out->rec_covar) rec.covar = B.alloc<double>(cap * 81 * n);
-    if (!od.covar0 || !od.covar || (out->state_dev_soa && !od.state_dev) || !d_state || !d_consts || !d_ep || !d_end ||
-        (state_dev0_soa && !d_dev0) || !d_out || !d_oep || !d_det || !d_status || (out->rec_count && !d_cnt) ||
-        (cap && out->rec_state && !rec.state) || (cap && out->rec_covar && !rec.covar)) {
-        set_err("device allocation / upload failed");
-        return NYXB_RC_CUDA;
-    }
+    const OdIo io = od_io(B, st, n, state_soa, consts_soa, epoch0_ns);
+    job.end_epoch = B.put((const long long*)end_epoch_ns, n, st);
+    job.dev0 = state_dev0_soa ? B.put(state_dev0_soa, 9 * n, st) : nullptr;
+    job.rec_count = out->rec_count ? B.alloc<long long>(n) : nullptr;
+    job.rec.cap = (long long)cap;
+    if (cap && out->rec_state) job.rec.state = B.alloc<double>(cap * 9 * n);
+    if (cap && out->rec_covar) job.rec.covar = B.alloc<double>(cap * 81 * n);
+    if (int32_t rc = B.check()) return rc;
     // records a run does not reach read back as NaN (0xFF bytes)
-    if (rec.state) CUDA_TRY(cudaMemsetAsync(rec.state, 0xFF, sizeof(double) * cap * 9 * n, st));
-    if (rec.covar) CUDA_TRY(cudaMemsetAsync(rec.covar, 0xFF, sizeof(double) * cap * 81 * n, st));
-    const int* d_cols = nullptr;
-    if (int32_t rc = od_coop_cols(eng, B, st, d_cols)) return rc;
-    const bool coop = d_cols != nullptr;
-    CUDA_TRY(cudaEventRecord(eng->ev0, st));
-    cudaError_t err = coop
-        ? nyxb_launch_pred_coop(&eng->S, &od, d_cols, n, d_state, d_consts, d_ep, d_end, d_dev0, &rec, d_cnt, d_out, d_oep, d_det, d_status, st)
-        : (eng->mode == NYXB_MODE_STRICT)
-            ? nyxb_launch_pred_strict(&eng->S, &od, n, d_state, d_consts, d_ep, d_end, d_dev0, &rec, d_cnt, d_out, d_oep, d_det, d_status, st)
-            : nyxb_launch_pred_fast(&eng->S, &od, n, d_state, d_consts, d_ep, d_end, d_dev0, &rec, d_cnt, d_out, d_oep, d_det, d_status, st);
-    if (err != cudaSuccess) { set_err(std::string("kernel launch: ") + cudaGetErrorString(err)); return NYXB_RC_CUDA; }
-    eng->launches += 1;
-    eng->last_kernel = coop ? NYXB_KERNEL_COOP : NYXB_KERNEL_THREAD;
-    CUDA_TRY(cudaEventRecord(eng->ev1, st));
-    CUDA_TRY(cudaMemcpyAsync(out->state_soa, d_out, sizeof(double) * 9 * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(out->epoch_ns, d_oep, sizeof(long long) * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(out->covar_soa, od.covar, sizeof(double) * 81 * n, cudaMemcpyDeviceToHost, st));
-    if (od.state_dev) CUDA_TRY(cudaMemcpyAsync(out->state_dev_soa, od.state_dev, sizeof(double) * 9 * n, cudaMemcpyDeviceToHost, st));
-    if (out->details) CUDA_TRY(cudaMemcpyAsync(out->details, d_det, sizeof(nyxb_details) * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(out->status, d_status, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
-    if (d_cnt) CUDA_TRY(cudaMemcpyAsync(out->rec_count, d_cnt, sizeof(long long) * n, cudaMemcpyDeviceToHost, st));
-    if (rec.state) CUDA_TRY(cudaMemcpyAsync(out->rec_state, rec.state, sizeof(double) * cap * 9 * n, cudaMemcpyDeviceToHost, st));
-    if (rec.covar) CUDA_TRY(cudaMemcpyAsync(out->rec_covar, rec.covar, sizeof(double) * cap * 81 * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, eng->ev0, eng->ev1) == cudaSuccess) eng->last_ms = ms;
-    return NYXB_RC_OK;
+    if (job.rec.state) CUDA_TRY(cudaMemsetAsync(job.rec.state, 0xFF, sizeof(double) * cap * 9 * n, st));
+    if (job.rec.covar) CUDA_TRY(cudaMemsetAsync(job.rec.covar, 0xFF, sizeof(double) * cap * 81 * n, st));
+    if (int32_t rc = od_launch(eng, job, B, n, io)) return rc;
+    if (int32_t rc = od_io_get(io, n, st, out->state_soa, out->epoch_ns, out->details, out->status)) return rc;
+    CUDA_TRY(get(out->covar_soa, od.covar, 81 * n, st));
+    CUDA_TRY(get(out->state_dev_soa, od.state_dev, 9 * n, st));
+    CUDA_TRY(get(out->rec_count, job.rec_count, n, st));
+    if (job.rec.state) CUDA_TRY(get(out->rec_state, job.rec.state, cap * 9 * n, st));
+    if (job.rec.covar) CUDA_TRY(get(out->rec_covar, job.rec.covar, cap * 81 * n, st));
+    return od_finish(eng);
 }
 
 namespace {
@@ -1436,34 +1331,24 @@ int32_t od_bls_run(nyxb_engine* eng, const nyxb_bls_config* cfg, int32_t n_stati
     }
     if (arc->n_msr < 0 || (arc->n_msr > 0 && (!arc->epoch_ns || !arc->tracker || !arc->obs))) { set_err("null tracking arc arrays"); return NYXB_RC_BAD_ARG; }
     if (!stm_supported(eng)) return NYXB_RC_UNSUPPORTED;
+    std::vector<DevStation> hs;
     for (int32_t s = 0; s < n_stations; ++s) {
         const nyxb_ground_station& g = stations[s];
-        if (g.n_types < 1 || g.n_types > 2 || (g.body != NYXB_CENTRAL_BODY && (g.body < 0 || g.body >= eng->S.n_bodies))) {
-            set_err("bad ground station descriptor");
-            return NYXB_RC_BAD_ARG;
-        }
+        if (!station_ok(eng, g)) return NYXB_RC_BAD_ARG;
         for (int q = 0; q < g.n_types; ++q) {
             if (g.types[q] != NYXB_MSR_RANGE && g.types[q] != NYXB_MSR_DOPPLER) { set_err("unsupported measurement type"); return NYXB_RC_UNSUPPORTED; }
             // earlier than the reference, which fails with SingularNoiseRk at the first measurement of this station
             if (!(g.noise_var[q] > 0.0)) { set_err("SingularNoiseRk: a station's noise variance must be positive"); return NYXB_RC_BAD_ARG; }
         }
+        hs.push_back(pack_station(g));
     }
     if (n == 0) return NYXB_RC_OK;
-    CUDA_TRY(cudaSetDevice(eng->device));
-    if (!eng->stream) CUDA_TRY(cudaStreamCreateWithFlags(&eng->stream, cudaStreamNonBlocking));
-    cudaStream_t st = eng->stream;
+    cudaStream_t st;
+    if (int32_t rc = od_stream(eng, st)) return rc;
     const size_t m = (size_t)arc->n_msr;
     DevBufs B;
-    std::vector<DevStation> hs((size_t)n_stations);
-    for (int32_t s = 0; s < n_stations; ++s) {
-        const nyxb_ground_station& g = stations[s];
-        DevStation& d = hs[s];
-        for (int q = 0; q < 3; ++q) { d.pos[q] = g.pos_fixed_km[q]; d.up[q] = g.up_fixed[q]; }
-        d.mask_deg = g.elevation_mask_deg; d.rot = pack_rot(g.rot); d.body = g.body; d.n_types = g.n_types;
-        for (int q = 0; q < 2; ++q) { d.types[q] = g.types[q]; d.noise_var[q] = g.noise_var[q]; d.bias[q] = g.bias[q]; }
-        d.body_radius = g.body_radius_km;
-    }
-    DevOd od{};
+    OdBlsJob job{};
+    DevOd& od = job.od;
     od.msr_size = 1;
     od.max_step_ns = cfg->max_step_ns; od.eps_ns = cfg->epoch_precision_ns;
     od.n_stations = n_stations;
@@ -1472,50 +1357,22 @@ int32_t od_bls_run(nyxb_engine* eng, const nyxb_bls_config* cfg, int32_t n_stati
     od.msr_epoch = m ? B.put((const long long*)arc->epoch_ns, m, st) : nullptr;
     od.msr_tracker = m ? B.put((const int*)arc->tracker, m, st) : nullptr;
     od.obs = m ? B.put(arc->obs, m * 2 * n, st) : nullptr;
-    double* d_state = B.put(state_soa, 9 * n, st);
-    double* d_consts = B.put(consts_soa, 4 * n, st);
-    long long* d_ep = B.put((const long long*)epoch0_ns, n, st);
-    double* d_out = B.alloc<double>(9 * n);
-    long long* d_oep = B.alloc<long long>(n);
-    nyxb_details* d_det = B.alloc<nyxb_details>(n);
-    int* d_status = B.alloc<int>(n);
-    bl.covar = out_covar ? B.alloc<double>(81 * n) : nullptr;
-    bl.iters = out_iters ? B.alloc<int>(n) : nullptr;
-    bl.rms = out_rms ? B.alloc<double>(n) : nullptr;
-    bl.corr_pos_km = out_corr ? B.alloc<double>(n) : nullptr;
-    bl.converged = out_conv ? B.alloc<int>(n) : nullptr;
-    if ((n_stations && !od.stations) || (m && (!od.msr_epoch || !od.msr_tracker || !od.obs)) || !d_state || !d_consts || !d_ep || !d_out ||
-        !d_oep || !d_det || !d_status || (out_covar && !bl.covar) || (out_iters && !bl.iters) || (out_rms && !bl.rms) ||
-        (out_corr && !bl.corr_pos_km) || (out_conv && !bl.converged)) {
-        set_err("device allocation / upload failed");
-        return NYXB_RC_CUDA;
-    }
-    const int* d_cols = nullptr;
-    if (int32_t rc = od_coop_cols(eng, B, st, d_cols)) return rc;
-    const bool coop = d_cols != nullptr;
-    CUDA_TRY(cudaEventRecord(eng->ev0, st));
-    cudaError_t err = coop
-        ? nyxb_launch_bls_coop(&eng->S, &od, &bl, d_cols, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
-        : (eng->mode == NYXB_MODE_STRICT)
-            ? nyxb_launch_bls_strict(&eng->S, &od, &bl, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st)
-            : nyxb_launch_bls_fast(&eng->S, &od, &bl, n, d_state, d_consts, d_ep, d_out, d_oep, d_det, d_status, st);
-    if (err != cudaSuccess) { set_err(std::string("kernel launch: ") + cudaGetErrorString(err)); return NYXB_RC_CUDA; }
-    eng->launches += 1;
-    eng->last_kernel = coop ? NYXB_KERNEL_COOP : NYXB_KERNEL_THREAD;
-    CUDA_TRY(cudaEventRecord(eng->ev1, st));
-    if (out_state) CUDA_TRY(cudaMemcpyAsync(out_state, d_out, sizeof(double) * 9 * n, cudaMemcpyDeviceToHost, st));
-    if (out_epoch) CUDA_TRY(cudaMemcpyAsync(out_epoch, d_oep, sizeof(long long) * n, cudaMemcpyDeviceToHost, st));
-    if (bl.covar) CUDA_TRY(cudaMemcpyAsync(out_covar, bl.covar, sizeof(double) * 81 * n, cudaMemcpyDeviceToHost, st));
-    if (bl.iters) CUDA_TRY(cudaMemcpyAsync(out_iters, bl.iters, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
-    if (bl.rms) CUDA_TRY(cudaMemcpyAsync(out_rms, bl.rms, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
-    if (bl.corr_pos_km) CUDA_TRY(cudaMemcpyAsync(out_corr, bl.corr_pos_km, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
-    if (bl.converged) CUDA_TRY(cudaMemcpyAsync(out_conv, bl.converged, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
-    if (out_details) CUDA_TRY(cudaMemcpyAsync(out_details, d_det, sizeof(nyxb_details) * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(out_status, d_status, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, eng->ev0, eng->ev1) == cudaSuccess) eng->last_ms = ms;
-    return NYXB_RC_OK;
+    const OdIo io = od_io(B, st, n, state_soa, consts_soa, epoch0_ns);
+    job.bl = bl;
+    job.bl.covar = out_covar ? B.alloc<double>(81 * n) : nullptr;
+    job.bl.iters = out_iters ? B.alloc<int>(n) : nullptr;
+    job.bl.rms = out_rms ? B.alloc<double>(n) : nullptr;
+    job.bl.corr_pos_km = out_corr ? B.alloc<double>(n) : nullptr;
+    job.bl.converged = out_conv ? B.alloc<int>(n) : nullptr;
+    if (int32_t rc = B.check()) return rc;
+    if (int32_t rc = od_launch(eng, job, B, n, io)) return rc;
+    if (int32_t rc = od_io_get(io, n, st, out_state, out_epoch, out_details, out_status)) return rc;
+    CUDA_TRY(get(out_covar, job.bl.covar, 81 * n, st));
+    CUDA_TRY(get(out_iters, job.bl.iters, n, st));
+    CUDA_TRY(get(out_rms, job.bl.rms, n, st));
+    CUDA_TRY(get(out_corr, job.bl.corr_pos_km, n, st));
+    CUDA_TRY(get(out_conv, job.bl.converged, n, st));
+    return od_finish(eng);
 }
 }  // namespace
 

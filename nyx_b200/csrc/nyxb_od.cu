@@ -3,10 +3,11 @@
 // between measurements, time updates, measurement updates, state replacement — runs inside ONE kernel launch; state,
 // STM, covariance and stage data stay in registers / L1-resident local memory, HBM sees the inputs once and the
 // per-measurement residual records as coalesced [m][..][n] stores.  The propagation and the filter loop are the templates of
-// nyxb_od_arc.cuh; this file gives them the per-thread backend (ThreadB) and holds the kernels and their launchers.
+// nyxb_od_arc.cuh; this file gives them the per-thread backend (ThreadBT) and holds one kernel template, nyxb_k_od<Job>, and its
+// launcher, instantiated for every OD job of nyxb_od.cuh.
 //
 // Built twice like nyxb_kernels.cu: -DNYXB_STRICT=1 -fmad=false (same operation order as oracle/nyx_oracle_od.c for
-// the dynamics) and -DNYXB_STRICT=0 -fmad=true.
+// the dynamics) and -DNYXB_STRICT=0 -fmad=true, in the namespaces nyxb_od_strict and nyxb_od_fast.
 //
 // Reference behaviour (paths relative to /root/reference/nyx-core/src):
 //   SpacecraftDynamics::eom `Some(stm)` branch / dual_eom      dynamics/spacecraft.rs:203-227, 312-363
@@ -27,33 +28,9 @@
 #error "NYXB_STRICT must be defined to 0 or 1"
 #endif
 #if NYXB_STRICT
-#define NYXB_KSTM nyxb_k_stm_strict
-#define NYXB_KOD nyxb_k_od_strict
-#define NYXB_KPRED nyxb_k_pred_strict
-#define NYXB_LAUNCH_STM nyxb_launch_stm_strict
-#define NYXB_LAUNCH_OD nyxb_launch_od_strict
-#define NYXB_LAUNCH_PRED nyxb_launch_pred_strict
-#define NYXB_KBLS nyxb_k_bls_strict
-#define NYXB_LAUNCH_BLS nyxb_launch_bls_strict
-#define NYXB_KODREC nyxb_k_od_rec_strict
-#define NYXB_LAUNCH_ODREC nyxb_launch_od_rec_strict
-#define NYXB_KODPOS nyxb_k_odpos_strict
-#define NYXB_KODPOSREC nyxb_k_odpos_rec_strict
-#define NYXB_LAUNCH_ODPOS nyxb_launch_odpos_strict
+#define NYXB_OD_NS nyxb_od_strict
 #else
-#define NYXB_KSTM nyxb_k_stm_fast
-#define NYXB_KOD nyxb_k_od_fast
-#define NYXB_KPRED nyxb_k_pred_fast
-#define NYXB_LAUNCH_STM nyxb_launch_stm_fast
-#define NYXB_LAUNCH_OD nyxb_launch_od_fast
-#define NYXB_LAUNCH_PRED nyxb_launch_pred_fast
-#define NYXB_KBLS nyxb_k_bls_fast
-#define NYXB_LAUNCH_BLS nyxb_launch_bls_fast
-#define NYXB_KODREC nyxb_k_od_rec_fast
-#define NYXB_LAUNCH_ODREC nyxb_launch_od_rec_fast
-#define NYXB_KODPOS nyxb_k_odpos_fast
-#define NYXB_KODPOSREC nyxb_k_odpos_rec_fast
-#define NYXB_LAUNCH_ODPOS nyxb_launch_odpos_fast
+#define NYXB_OD_NS nyxb_od_fast
 #endif
 
 // ------------------------------------------------------------------------- per-thread backend of nyxb_od_arc.cuh
@@ -99,156 +76,35 @@ struct ThreadBT {
         return eom_stm(S, in, delta_t_s, ys, st.k[slot], st.Ai[slot], st.Ai[slot] + 9);
     }
 };
-using ThreadB = ThreadBT<2>;
+namespace NYXB_OD_NS {
 
+template <class Job>
 __global__ void __launch_bounds__(64)
-NYXB_KSTM(const __grid_constant__ DevSetup S, size_t n, const double* __restrict__ state, const double* __restrict__ consts,
-          const long long* __restrict__ epoch0, long long end_epoch, long long* __restrict__ step_io,
-          const double* __restrict__ stm_in, double* __restrict__ out_state, long long* __restrict__ out_epoch,
-          double* __restrict__ out_stm, nyxb_details* __restrict__ out_details, int* __restrict__ out_status) {
+nyxb_k_od(const __grid_constant__ DevSetup S, const __grid_constant__ Job job, size_t n, const double* __restrict__ state,
+          const double* __restrict__ consts, const long long* __restrict__ epoch0, double* __restrict__ out_state,
+          long long* __restrict__ out_epoch, nyxb_details* __restrict__ out_details, int* __restrict__ out_status) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    ThreadB b(S);
-    OdInst in;
-    od_load(S, in, i, n, state, consts, epoch0, step_io);
-    if (stm_in) { for (int e = 0; e < 81; ++e) b.phi[e] = stm_in[(size_t)e * n + i]; }
-    else od_reset_stm(b);
-    int rc = od_propagate(b, in, end_epoch - in.epoch_ns);
-    for (int e = 0; e < 81; ++e) out_stm[(size_t)e * n + i] = b.phi[e];
-    if (step_io) step_io[i] = in.step_ns;
-    od_store(b, in, rc, i, n, out_state, out_epoch, out_details, out_status);
+    ThreadBT<Job::NS> b(S);
+    od_run(job, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
 }
 
-__global__ void __launch_bounds__(64)
-NYXB_KOD(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od, size_t n, const double* __restrict__ state,
-         const double* __restrict__ consts, const long long* __restrict__ epoch0, double* __restrict__ out_state,
-         long long* __restrict__ out_epoch, nyxb_details* __restrict__ out_details, int* __restrict__ out_status) {
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    ThreadB b(S);
-    od_process_arc(od, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
-}
-
-// the filter with every estimate recorded (ODSolution.estimates, for ODSolution::smooth)
-__global__ void __launch_bounds__(64)
-NYXB_KODREC(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od, const OdEstRecords er, size_t n,
-            const double* __restrict__ state, const double* __restrict__ consts, const long long* __restrict__ epoch0,
-            double* __restrict__ out_state, long long* __restrict__ out_epoch, nyxb_details* __restrict__ out_details,
-            int* __restrict__ out_status) {
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    ThreadB b(S);
-    od_process_arc<ThreadB, true>(od, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status, &er);
-}
-
-__global__ void __launch_bounds__(64)
-NYXB_KPRED(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od, size_t n, const double* __restrict__ state,
-           const double* __restrict__ consts, const long long* __restrict__ epoch0, const long long* __restrict__ end_epoch,
-           const double* __restrict__ dev0, const OdRecords rec, long long* __restrict__ rec_count, double* __restrict__ out_state,
-           long long* __restrict__ out_epoch, nyxb_details* __restrict__ out_details, int* __restrict__ out_status) {
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    ThreadB b(S);
-    od_predict(od, b, i, n, state, consts, epoch0, end_epoch, dev0, rec, rec_count, out_state, out_epoch, out_details, out_status);
-}
-
-__global__ void __launch_bounds__(64)
-NYXB_KBLS(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od, const __grid_constant__ DevBls bl, size_t n,
-          const double* __restrict__ state, const double* __restrict__ consts, const long long* __restrict__ epoch0,
-          double* __restrict__ out_state, long long* __restrict__ out_epoch, nyxb_details* __restrict__ out_details,
-          int* __restrict__ out_status) {
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    ThreadB b(S);
-    od_bls(od, bl, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
-}
-
-// the filter over position fixes (PositionDevice), without and with the estimate records
-__global__ void __launch_bounds__(64)
-NYXB_KODPOS(const __grid_constant__ DevSetup S, const __grid_constant__ DevOdPos od, size_t n, const double* __restrict__ state,
-            const double* __restrict__ consts, const long long* __restrict__ epoch0, double* __restrict__ out_state,
-            long long* __restrict__ out_epoch, nyxb_details* __restrict__ out_details, int* __restrict__ out_status) {
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    ThreadBT<3> b(S);
-    od_process_arc<ThreadBT<3>, false, PosTrk>(od, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
-}
-
-__global__ void __launch_bounds__(64)
-NYXB_KODPOSREC(const __grid_constant__ DevSetup S, const __grid_constant__ DevOdPos od, const OdEstRecords er, size_t n,
-               const double* __restrict__ state, const double* __restrict__ consts, const long long* __restrict__ epoch0,
-               double* __restrict__ out_state, long long* __restrict__ out_epoch, nyxb_details* __restrict__ out_details,
-               int* __restrict__ out_status) {
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    ThreadBT<3> b(S);
-    od_process_arc<ThreadBT<3>, true, PosTrk>(od, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status, &er);
-}
-
-extern "C" cudaError_t NYXB_LAUNCH_STM(const DevSetup* S, size_t n, const double* state, const double* consts, const long long* epoch0,
-                                       long long end_epoch, long long* step_io, const double* stm_in, double* out_state,
-                                       long long* out_epoch, double* out_stm, nyxb_details* out_details, int* out_status,
-                                       cudaStream_t stream) {
-    if (n == 0) return cudaSuccess;
-    const int block = 32;
-    unsigned grid = (unsigned)((n + block - 1) / block);
-    NYXB_KSTM<<<grid, block, 0, stream>>>(*S, n, state, consts, epoch0, end_epoch, step_io, stm_in, out_state, out_epoch, out_stm,
-                                          out_details, out_status);
-    return cudaGetLastError();
-}
-
-extern "C" cudaError_t NYXB_LAUNCH_OD(const DevSetup* S, const DevOd* od, size_t n, const double* state, const double* consts,
-                                      const long long* epoch0, double* out_state, long long* out_epoch, nyxb_details* out_details,
-                                      int* out_status, cudaStream_t stream) {
+template <class Job>
+cudaError_t launch(const DevSetup& S, const Job& job, size_t n, const OdIo& io, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     const int block = 32;  // few, long-running threads: spread them over as many SMs as possible
     unsigned grid = (unsigned)((n + block - 1) / block);
-    NYXB_KOD<<<grid, block, 0, stream>>>(*S, *od, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
+    nyxb_k_od<Job><<<grid, block, 0, st>>>(S, job, n, io.state, io.consts, io.epoch0, io.out_state, io.out_epoch, io.out_details,
+                                           io.out_status);
     return cudaGetLastError();
 }
 
-extern "C" cudaError_t NYXB_LAUNCH_ODREC(const DevSetup* S, const DevOd* od, const OdEstRecords* er, size_t n, const double* state,
-                                         const double* consts, const long long* epoch0, double* out_state, long long* out_epoch,
-                                         nyxb_details* out_details, int* out_status, cudaStream_t stream) {
-    if (n == 0) return cudaSuccess;
-    const int block = 32;  // as the filter kernel
-    unsigned grid = (unsigned)((n + block - 1) / block);
-    NYXB_KODREC<<<grid, block, 0, stream>>>(*S, *od, *er, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
-    return cudaGetLastError();
-}
+template cudaError_t launch(const DevSetup&, const OdStmJob&, size_t, const OdIo&, cudaStream_t);
+template cudaError_t launch(const DevSetup&, const OdFilterJob<DevStation, false>&, size_t, const OdIo&, cudaStream_t);
+template cudaError_t launch(const DevSetup&, const OdFilterJob<DevStation, true>&, size_t, const OdIo&, cudaStream_t);
+template cudaError_t launch(const DevSetup&, const OdFilterJob<DevPosDevice, false>&, size_t, const OdIo&, cudaStream_t);
+template cudaError_t launch(const DevSetup&, const OdFilterJob<DevPosDevice, true>&, size_t, const OdIo&, cudaStream_t);
+template cudaError_t launch(const DevSetup&, const OdPredictJob&, size_t, const OdIo&, cudaStream_t);
+template cudaError_t launch(const DevSetup&, const OdBlsJob&, size_t, const OdIo&, cudaStream_t);
 
-extern "C" cudaError_t NYXB_LAUNCH_PRED(const DevSetup* S, const DevOd* od, size_t n, const double* state, const double* consts,
-                                        const long long* epoch0, const long long* end_epoch, const double* dev0, const OdRecords* rec,
-                                        long long* rec_count, double* out_state, long long* out_epoch, nyxb_details* out_details,
-                                        int* out_status, cudaStream_t stream) {
-    if (n == 0) return cudaSuccess;
-    const int block = 32;  // as the filter kernel
-    unsigned grid = (unsigned)((n + block - 1) / block);
-    NYXB_KPRED<<<grid, block, 0, stream>>>(*S, *od, n, state, consts, epoch0, end_epoch, dev0, *rec, rec_count, out_state, out_epoch,
-                                           out_details, out_status);
-    return cudaGetLastError();
-}
-
-extern "C" cudaError_t NYXB_LAUNCH_BLS(const DevSetup* S, const DevOd* od, const DevBls* bl, size_t n, const double* state,
-                                       const double* consts, const long long* epoch0, double* out_state, long long* out_epoch,
-                                       nyxb_details* out_details, int* out_status, cudaStream_t stream) {
-    if (n == 0) return cudaSuccess;
-    const int block = 32;  // as the filter kernel
-    unsigned grid = (unsigned)((n + block - 1) / block);
-    NYXB_KBLS<<<grid, block, 0, stream>>>(*S, *od, *bl, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
-    return cudaGetLastError();
-}
-
-// er: null for the filter alone
-extern "C" cudaError_t NYXB_LAUNCH_ODPOS(const DevSetup* S, const DevOdPos* od, const OdEstRecords* er, size_t n, const double* state,
-                                         const double* consts, const long long* epoch0, double* out_state, long long* out_epoch,
-                                         nyxb_details* out_details, int* out_status, cudaStream_t stream) {
-    if (n == 0) return cudaSuccess;
-    const int block = 32;  // as the filter kernel
-    unsigned grid = (unsigned)((n + block - 1) / block);
-    if (er)
-        NYXB_KODPOSREC<<<grid, block, 0, stream>>>(*S, *od, *er, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
-    else
-        NYXB_KODPOS<<<grid, block, 0, stream>>>(*S, *od, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
-    return cudaGetLastError();
-}
+}  // namespace NYXB_OD_NS

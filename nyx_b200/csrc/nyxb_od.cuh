@@ -3,7 +3,15 @@
 #pragma once
 #include "nyxb_device.cuh"
 
+#define ODC_KMAX 4           // columns of the Legendre triangle per lane of a warp kernel (>= the host's deal over 32 lanes: 4 at N = 96)
+
+struct GroundTrk;            // the measurement model of each tracker kind (nyxb_od_device.cuh)
+struct PosTrk;
+
+// NS: the observation slots of one measurement (obs is [m][NS][n])
 struct DevStation {
+    static constexpr int NS = 2;
+    using Trk = GroundTrk;
     double pos[3], up[3];
     double mask_deg;
     DevRotation rot;
@@ -16,6 +24,8 @@ struct DevStation {
 // GNSS-style position fixes (od/position): X, Y, Z of the spacecraft in the integration frame.  types[] in the device's list order,
 // as NYXB_MSR_X.. (the observation slot of a type is type - NYXB_MSR_X); noise_var / bias per list position.
 struct DevPosDevice {
+    static constexpr int NS = 3;
+    using Trk = PosTrk;
     int n_types;
     int types[3];
     double noise_var[3], bias[3];
@@ -98,7 +108,6 @@ struct DevSmoothT {
     double* postfit;               // [cap][2][n] or null
     long long* err_key;            // [n] -1, or the largest 2k + (1: singular Phi, 0: ephemeris) among the failing estimates k
 };
-struct DevSmooth : DevSmoothT<DevStation> {};
 
 // Batch least squares (BatchLeastSquares::estimate / evaluate, od/blse/mod.rs:146-541).  The schedule, stations, observations,
 // max_step and epoch precision come from DevOd; this holds the solver settings and the per-problem outputs ([n], covar [81][n]).
@@ -116,35 +125,67 @@ struct DevBls {
     int* converged;
 };
 
-extern "C" cudaError_t nyxb_launch_stm_strict(const DevSetup*, size_t, const double*, const double*, const long long*, long long,
-                                              long long*, const double*, double*, long long*, double*, nyxb_details*, int*, cudaStream_t);
-extern "C" cudaError_t nyxb_launch_stm_fast(const DevSetup*, size_t, const double*, const double*, const long long*, long long,
-                                            long long*, const double*, double*, long long*, double*, nyxb_details*, int*, cudaStream_t);
-extern "C" cudaError_t nyxb_launch_od_strict(const DevSetup*, const DevOd*, size_t, const double*, const double*, const long long*,
-                                             double*, long long*, nyxb_details*, int*, cudaStream_t);
-extern "C" cudaError_t nyxb_launch_od_fast(const DevSetup*, const DevOd*, size_t, const double*, const double*, const long long*,
-                                           double*, long long*, nyxb_details*, int*, cudaStream_t);
-extern "C" cudaError_t nyxb_launch_pred_strict(const DevSetup*, const DevOd*, size_t, const double*, const double*, const long long*,
-                                               const long long*, const double*, const OdRecords*, long long*, double*, long long*,
-                                               nyxb_details*, int*, cudaStream_t);
-extern "C" cudaError_t nyxb_launch_pred_fast(const DevSetup*, const DevOd*, size_t, const double*, const double*, const long long*,
-                                             const long long*, const double*, const OdRecords*, long long*, double*, long long*,
-                                             nyxb_details*, int*, cudaStream_t);
-extern "C" cudaError_t nyxb_launch_od_rec_strict(const DevSetup*, const DevOd*, const OdEstRecords*, size_t, const double*, const double*,
-                                                 const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
-extern "C" cudaError_t nyxb_launch_od_rec_fast(const DevSetup*, const DevOd*, const OdEstRecords*, size_t, const double*, const double*,
-                                               const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
-extern "C" cudaError_t nyxb_launch_bls_strict(const DevSetup*, const DevOd*, const DevBls*, size_t, const double*, const double*,
-                                              const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
-extern "C" cudaError_t nyxb_launch_bls_fast(const DevSetup*, const DevOd*, const DevBls*, size_t, const double*, const double*,
-                                            const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
-extern "C" cudaError_t nyxb_launch_smooth(const DevSetup*, const DevSmooth*, size_t, cudaStream_t);
+// ------------------------------------------------------------------------- OD jobs: what one launch of nyxb_k_od / nyxb_k_od_coop runs
+// Each job holds what is specific to it; od_run (nyxb_od_arc.cuh) runs it.  NS: the observation slots of the gain scratch.
 
-// position fixes (DevOdT<DevPosDevice>): the same filter and smoother, three observation slots
-struct DevOdPos : DevOdT<DevPosDevice> {};
-struct DevSmoothPos : DevSmoothT<DevPosDevice> {};
-extern "C" cudaError_t nyxb_launch_odpos_strict(const DevSetup*, const DevOdPos*, const OdEstRecords*, size_t, const double*, const double*,
-                                                const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
-extern "C" cudaError_t nyxb_launch_odpos_fast(const DevSetup*, const DevOdPos*, const OdEstRecords*, size_t, const double*, const double*,
-                                              const long long*, double*, long long*, nyxb_details*, int*, cudaStream_t);
-extern "C" cudaError_t nyxb_launch_smooth_pos(const DevSetup*, const DevSmoothPos*, size_t, cudaStream_t);
+// STM propagation to end_epoch (nyxb_propagate_batch_stm); per-thread kernels only
+struct OdStmJob {
+    static constexpr int NS = 2;   // no filter storage is used
+    long long end_epoch;
+    long long* step_io;            // [n] initial step in, last step out, or null
+    const double* stm_in;          // [81][n] or null (identity)
+    double* out_stm;               // [81][n]
+};
+
+// the filter (KalmanODProcess::process_arc) over the trackers Dev; REC: every estimate also recorded into er
+template <class Dev, bool REC>
+struct OdFilterJob {
+    static constexpr int NS = Dev::NS;
+    DevOdT<Dev> od;
+    OdEstRecords er;
+};
+template <class Dev>
+struct OdFilterJob<Dev, false> {
+    static constexpr int NS = Dev::NS;
+    DevOdT<Dev> od;
+};
+
+// covariance prediction (KalmanODProcess::predict_until)
+struct OdPredictJob {
+    static constexpr int NS = DevStation::NS;
+    DevOd od;
+    const long long* end_epoch;    // [n]
+    const double* dev0;            // [9][n] initial deviation or null
+    OdRecords rec;
+    long long* rec_count;          // [n] or null
+};
+
+// batch least squares (BatchLeastSquares::estimate / evaluate)
+struct OdBlsJob {
+    static constexpr int NS = DevStation::NS;
+    DevOd od;
+    DevBls bl;
+};
+
+// the per-filter arrays every job reads and writes (device pointers): state [9][n], consts [4][n], epoch0 [n]; out_details may be null
+struct OdIo {
+    const double* state;
+    const double* consts;
+    const long long* epoch0;
+    double* out_state;
+    long long* out_epoch;
+    nyxb_details* out_details;
+    int* out_status;
+};
+
+// Launchers.  The per-thread kernels are built twice (nyxb_od.cu), STRICT and FAST, each in its own namespace so that the two
+// builds' instantiations of one kernel template stay distinct symbols; the warp kernels (nyxb_od_coop.cu) are FAST only.
+namespace nyxb_od_strict {
+template <class Job> cudaError_t launch(const DevSetup& S, const Job& job, size_t n, const OdIo& io, cudaStream_t st);
+}
+namespace nyxb_od_fast {
+template <class Job> cudaError_t launch(const DevSetup& S, const Job& job, size_t n, const OdIo& io, cudaStream_t st);
+}
+template <class Job> cudaError_t nyxb_od_coop_launch(const DevSetup& S, const Job& job, const int* cols, size_t n, const OdIo& io, cudaStream_t st);
+// ODSolution::smooth over the records of the filters of tracker kind Dev (nyxb_smooth.cu)
+template <class Dev> cudaError_t nyxb_smooth_launch(const DevSetup& S, const DevSmoothT<Dev>& sm, size_t n, cudaStream_t st);

@@ -504,9 +504,9 @@ __device__ void od_predict(const DevOd& od, B& b, size_t i, size_t n, const doub
         const int r = e / 9, c = e - 9 * r;
         f.P[e] = od.covar0[(size_t)(c * 9 + r) * n + i];
     }
-    for (int r = b.first(); r < 9; r += B::stride) f.xdev[r] = dev0 ? dev0[(size_t)r * n + i] : 0.0;
+    for (int r = b.first(); r < 9; r += B::stride) f.xdev[r] = dev0 ? __ldg(dev0 + (size_t)r * n + i) : 0.0;
     od_reset_stm(b);                                          // prop.with(nominal.with_stm()) :452
-    const long long end = end_epoch[i];
+    const long long end = __ldg(end_epoch + i);
     long long prev_epoch = in.epoch_ns;
     long long k = 0;
     od_record(rec, k++, in, b, f, i, n);                      // push_time_update(initial_estimate) :448
@@ -777,4 +777,48 @@ __device__ void od_bls(const DevOd& od, const DevBls& bl, B& b, size_t i, size_t
         if (bl.converged) bl.converged[i] = converged ? 1 : 0;
     }
     od_store(b, in, rc, i, n, out_state, out_epoch, out_details, out_status);
+}
+
+// ------------------------------------------------------------------------- one entry per OD job (nyxb_od.cuh), for either backend
+// The job's input arrays are read through __ldg: unlike __restrict__ kernel arguments, pointers inside a descriptor do not tell the
+// compiler that nothing the kernel writes aliases them, so the read-only path has to be asked for.
+template <class B>
+__device__ __forceinline__ void od_run(const OdStmJob& job, B& b, size_t i, size_t n, const double* state, const double* consts,
+                                       const long long* epoch0, double* out_state, long long* out_epoch, nyxb_details* out_details,
+                                       int* out_status) {
+    OdInst in;
+    od_load(b.S, in, i, n, state, consts, epoch0, job.step_io);
+    if (job.stm_in) { for (int e = 0; e < 81; ++e) b.phi[e] = __ldg(job.stm_in + (size_t)e * n + i); }
+    else od_reset_stm(b);
+    int rc = od_propagate(b, in, job.end_epoch - in.epoch_ns);
+    for (int e = 0; e < 81; ++e) job.out_stm[(size_t)e * n + i] = b.phi[e];
+    if (job.step_io) job.step_io[i] = in.step_ns;
+    od_store(b, in, rc, i, n, out_state, out_epoch, out_details, out_status);
+}
+
+template <class B, class Dev, bool REC>
+__device__ __forceinline__ void od_run(const OdFilterJob<Dev, REC>& job, B& b, size_t i, size_t n, const double* state, const double* consts,
+                                       const long long* epoch0, double* out_state, long long* out_epoch, nyxb_details* out_details,
+                                       int* out_status) {
+    if constexpr (REC) {
+        const OdEstRecords er = job.er;
+        od_process_arc<B, true, typename Dev::Trk>(job.od, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status, &er);
+    } else {
+        od_process_arc<B, false, typename Dev::Trk>(job.od, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
+    }
+}
+
+template <class B>
+__device__ __forceinline__ void od_run(const OdPredictJob& job, B& b, size_t i, size_t n, const double* state, const double* consts,
+                                       const long long* epoch0, double* out_state, long long* out_epoch, nyxb_details* out_details,
+                                       int* out_status) {
+    od_predict(job.od, b, i, n, state, consts, epoch0, job.end_epoch, job.dev0, job.rec, job.rec_count, out_state, out_epoch, out_details,
+               out_status);
+}
+
+template <class B>
+__device__ __forceinline__ void od_run(const OdBlsJob& job, B& b, size_t i, size_t n, const double* state, const double* consts,
+                                       const long long* epoch0, double* out_state, long long* out_epoch, nyxb_details* out_details,
+                                       int* out_status) {
+    od_bls(job.od, job.bl, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
 }

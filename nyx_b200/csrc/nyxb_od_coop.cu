@@ -13,26 +13,22 @@
 //   * STM, covariance, stage derivatives and stage A-matrices live in shared memory (one slab per warp); the 9x9
 //     algebra of the filter (Phi P Phi^T, Joseph update) is spread over the lanes entry by entry.
 // The propagation and the filter loop are the templates of nyxb_od_arc.cuh, shared with the per-thread kernels (nyxb_od.cu),
-// which remain the STRICT (oracle-order) path; this file gives them the warp backend (WarpB).  Its right-hand side sums in
+// which remain the STRICT (oracle-order) path; this file gives them the warp backend (WarpBT) and holds one kernel template,
+// nyxb_k_od_coop<Job>, and its launcher, instantiated for the filter, prediction and BLS jobs of nyxb_od.cuh.  Its right-hand side sums in
 // another order than the per-thread one (tolerance parity, tests/test_gpu_stm_od.py).
 #include "nyxb_od_arc.cuh"
 
-#define ODC_KMAX 4           // columns per lane (>= the host's deal of the N+1 columns over 32 lanes: 4 at N = 96)
 #define ODC_WPB 4            // warps (filters) per block
 #define FULL 0xffffffffu
 
-struct WarpS {
+// the warp's slab in shared memory; NS: the tracker kind's observation slots (the gain scratch PHt and K is 9 x NS)
+template <int NS>
+struct WarpST {
     double phi[81], nphi[81];          // STM (column-major like the ABI) and its candidate
     double P[81], T[81], Pb[81], F[81];
     double k[NYXB_MAX_STAGES][6];
     double Ai[NYXB_MAX_STAGES][12];
-    double PHt[18], K[18], xdev[9];
-};
-
-// the slab of a position-fix filter: the gain scratch has 9 x 3 entries (WarpS's PHt and K stay unused)
-struct WarpSPos {
-    WarpS s;
-    double PHt[27], K[27];
+    double PHt[9 * NS], K[9 * NS], xdev[9];
 };
 
 __device__ __forceinline__ double wsum(double v) {
@@ -168,18 +164,20 @@ __device__ static void grav_gradient_coop(const DevGrav& g, const int* __restric
 
 // ------------------------------------------------------------------------- warp backend of nyxb_od_arc.cuh
 // what the right-hand side reads
+template <int NS>
 struct Ctx {
     const DevSetup* S;
     const int* mycols;   // this lane's columns of the Legendre triangle
     D3* pw;              // the warp's power tables
-    WarpS* W;
+    WarpST<NS>* W;
     int lane;
 };
 
 // one RHS: stage slot `slot` of the shared k / Ai arrays receives (v, a) and the A-matrix parts
 // __noinline__: called from two places in od_derive; one copy keeps the kernel's instruction footprint (and the
 // instruction-cache misses ncu shows as `no_inst` stalls) down
-__device__ __noinline__ static int eom_coop(const Ctx& cx, OdInst& in, double delta_t_s, const double ys[9], int slot) {
+template <int NS>
+__device__ __noinline__ static int eom_coop(const Ctx<NS>& cx, OdInst& in, double delta_t_s, const double ys[9], int slot) {
     const DevSetup& S = *cx.S;
     long long t_ns = in.epoch_ns + dur_from_seconds(delta_t_s);
     double yy[9];
@@ -213,23 +211,24 @@ __device__ __noinline__ static int eom_coop(const Ctx& cx, OdInst& in, double de
 }
 
 // Every lane holds the same OdInst; the arrays live in the warp's slab and an 81-entry loop gives entry e to lane e % 32.
-struct WarpB {
+template <int NS>
+struct WarpBT {
     static constexpr int stride = 32;
-    const Ctx& cx;
+    const Ctx<NS>& cx;
     const DevSetup& S;
-    WarpS& W;
+    WarpST<NS>& W;
     double (&phi)[81];
     struct Step {
         double (&nphi)[81];
         double (&k)[NYXB_MAX_STAGES][6];
         double (&Ai)[NYXB_MAX_STAGES][12];
-        __device__ explicit Step(WarpB& b) : nphi(b.W.nphi), k(b.W.k), Ai(b.W.Ai) {}
+        __device__ explicit Step(WarpBT& b) : nphi(b.W.nphi), k(b.W.k), Ai(b.W.Ai) {}
     };
     struct Filt {
-        double (&P)[81], (&xdev)[9], (&Pb)[81], (&T)[81], (&F)[81], (&PHt)[18], (&K)[18];
-        __device__ explicit Filt(WarpB& b) : P(b.W.P), xdev(b.W.xdev), Pb(b.W.Pb), T(b.W.T), F(b.W.F), PHt(b.W.PHt), K(b.W.K) {}
+        double (&P)[81], (&xdev)[9], (&Pb)[81], (&T)[81], (&F)[81], (&PHt)[9 * NS], (&K)[9 * NS];
+        __device__ explicit Filt(WarpBT& b) : P(b.W.P), xdev(b.W.xdev), Pb(b.W.Pb), T(b.W.T), F(b.W.F), PHt(b.W.PHt), K(b.W.K) {}
     };
-    __device__ explicit WarpB(const Ctx& c) : cx(c), S(*c.S), W(*c.W), phi(c.W->phi) {}
+    __device__ explicit WarpBT(const Ctx<NS>& c) : cx(c), S(*c.S), W(*c.W), phi(c.W->phi) {}
     __device__ int first() const { return cx.lane; }
     __device__ bool lead() const { return cx.lane == 0; }
     __device__ void sync() const { __syncwarp(); }
@@ -239,211 +238,50 @@ struct WarpB {
     }
 };
 
-// the warp backend of a position-fix filter: WarpB with its gain scratch in WarpSPos
-struct WarpBPos : WarpB {
-    WarpSPos& X;
-    struct Filt {
-        double (&P)[81], (&xdev)[9], (&Pb)[81], (&T)[81], (&F)[81], (&PHt)[27], (&K)[27];
-        __device__ explicit Filt(WarpBPos& b) : P(b.W.P), xdev(b.W.xdev), Pb(b.W.Pb), T(b.W.T), F(b.W.F), PHt(b.X.PHt), K(b.X.K) {}
-    };
-    __device__ WarpBPos(const Ctx& c, WarpSPos& x) : WarpB(c), X(x) {}
-};
+// bytes of one warp's slab: WarpST, then the D3 power tables RM / IM / RP of grav_gradient_coop, N + 2 entries each (the launcher
+// and the kernel both size it here)
+template <int NS>
+__host__ __device__ __forceinline__ size_t od_coop_slab(int has_grav, int N) {
+    const int npw = has_grav ? 3 * (N + 2) : 0;
+    return (sizeof(WarpST<NS>) + sizeof(D3) * (size_t)npw + 15) & ~(size_t)15;
+}
 
+// one warp per filter, run, or problem; the host's column deal gives lane l the columns cols[l * ODC_KMAX ..] (-1 ends them)
+template <class Job>
 __global__ void __launch_bounds__(32 * ODC_WPB)
-nyxb_k_od_coop(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od, const int* __restrict__ cols, size_t n,
+nyxb_k_od_coop(const __grid_constant__ DevSetup S, const __grid_constant__ Job job, const int* __restrict__ cols, size_t n,
                const double* __restrict__ state, const double* __restrict__ consts, const long long* __restrict__ epoch0,
                double* __restrict__ out_state, long long* __restrict__ out_epoch, nyxb_details* __restrict__ out_details,
                int* __restrict__ out_status) {
+    constexpr int NS = Job::NS;
     extern __shared__ __align__(16) unsigned char smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const size_t i = (size_t)blockIdx.x * ODC_WPB + wib;
     if (i >= n) return;   // whole warps leave together
-    const int npw = S.has_grav ? 3 * (S.grav.N + 2) : 0;
-    const size_t slab = (sizeof(WarpS) + sizeof(D3) * (size_t)npw + 15) & ~(size_t)15;
-    WarpS& W = *reinterpret_cast<WarpS*>(smem + slab * wib);
-    Ctx cx;
+    const size_t slab = od_coop_slab<NS>(S.has_grav, S.grav.N);
+    WarpST<NS>& W = *reinterpret_cast<WarpST<NS>*>(smem + slab * wib);
+    Ctx<NS> cx;
     cx.S = &S; cx.mycols = cols + lane * ODC_KMAX; cx.W = &W; cx.lane = lane;
-    cx.pw = reinterpret_cast<D3*>(smem + slab * wib + sizeof(WarpS));
-    WarpB b(cx);
-    od_process_arc(od, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
+    cx.pw = reinterpret_cast<D3*>(smem + slab * wib + sizeof(WarpST<NS>));
+    WarpBT<NS> b(cx);
+    od_run(job, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
 }
 
-// the filter with every estimate recorded (ODSolution.estimates, for ODSolution::smooth), one warp per filter
-__global__ void __launch_bounds__(32 * ODC_WPB)
-nyxb_k_od_rec_coop(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od, const OdEstRecords er, const int* __restrict__ cols,
-                   size_t n, const double* __restrict__ state, const double* __restrict__ consts, const long long* __restrict__ epoch0,
-                   double* __restrict__ out_state, long long* __restrict__ out_epoch, nyxb_details* __restrict__ out_details,
-                   int* __restrict__ out_status) {
-    extern __shared__ __align__(16) unsigned char smem[];
-    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    const size_t i = (size_t)blockIdx.x * ODC_WPB + wib;
-    if (i >= n) return;   // whole warps leave together
-    const int npw = S.has_grav ? 3 * (S.grav.N + 2) : 0;
-    const size_t slab = (sizeof(WarpS) + sizeof(D3) * (size_t)npw + 15) & ~(size_t)15;
-    WarpS& W = *reinterpret_cast<WarpS*>(smem + slab * wib);
-    Ctx cx;
-    cx.S = &S; cx.mycols = cols + lane * ODC_KMAX; cx.W = &W; cx.lane = lane;
-    cx.pw = reinterpret_cast<D3*>(smem + slab * wib + sizeof(WarpS));
-    WarpB b(cx);
-    od_process_arc<WarpB, true>(od, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status, &er);
-}
-
-// covariance prediction (KalmanODProcess::predict_until), one warp per run: same slab and column deal as the filter kernel
-__global__ void __launch_bounds__(32 * ODC_WPB)
-nyxb_k_pred_coop(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od, const int* __restrict__ cols, size_t n,
-                 const double* __restrict__ state, const double* __restrict__ consts, const long long* __restrict__ epoch0,
-                 const long long* __restrict__ end_epoch, const double* __restrict__ dev0, const OdRecords rec,
-                 long long* __restrict__ rec_count, double* __restrict__ out_state, long long* __restrict__ out_epoch,
-                 nyxb_details* __restrict__ out_details, int* __restrict__ out_status) {
-    extern __shared__ __align__(16) unsigned char smem[];
-    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    const size_t i = (size_t)blockIdx.x * ODC_WPB + wib;
-    if (i >= n) return;   // whole warps leave together
-    const int npw = S.has_grav ? 3 * (S.grav.N + 2) : 0;
-    const size_t slab = (sizeof(WarpS) + sizeof(D3) * (size_t)npw + 15) & ~(size_t)15;
-    WarpS& W = *reinterpret_cast<WarpS*>(smem + slab * wib);
-    Ctx cx;
-    cx.S = &S; cx.mycols = cols + lane * ODC_KMAX; cx.W = &W; cx.lane = lane;
-    cx.pw = reinterpret_cast<D3*>(smem + slab * wib + sizeof(WarpS));
-    WarpB b(cx);
-    od_predict(od, b, i, n, state, consts, epoch0, end_epoch, dev0, rec, rec_count, out_state, out_epoch, out_details, out_status);
-}
-
-// batch least squares (BatchLeastSquares::estimate / evaluate), one warp per problem: same slab and column deal as the filter kernel
-__global__ void __launch_bounds__(32 * ODC_WPB)
-nyxb_k_bls_coop(const __grid_constant__ DevSetup S, const __grid_constant__ DevOd od, const __grid_constant__ DevBls bl,
-                const int* __restrict__ cols, size_t n, const double* __restrict__ state, const double* __restrict__ consts,
-                const long long* __restrict__ epoch0, double* __restrict__ out_state, long long* __restrict__ out_epoch,
-                nyxb_details* __restrict__ out_details, int* __restrict__ out_status) {
-    extern __shared__ __align__(16) unsigned char smem[];
-    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    const size_t i = (size_t)blockIdx.x * ODC_WPB + wib;
-    if (i >= n) return;   // whole warps leave together
-    const int npw = S.has_grav ? 3 * (S.grav.N + 2) : 0;
-    const size_t slab = (sizeof(WarpS) + sizeof(D3) * (size_t)npw + 15) & ~(size_t)15;
-    WarpS& W = *reinterpret_cast<WarpS*>(smem + slab * wib);
-    Ctx cx;
-    cx.S = &S; cx.mycols = cols + lane * ODC_KMAX; cx.W = &W; cx.lane = lane;
-    cx.pw = reinterpret_cast<D3*>(smem + slab * wib + sizeof(WarpS));
-    WarpB b(cx);
-    od_bls(od, bl, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
-}
-
-// the filter over position fixes, one warp per filter, without and with the estimate records
-template <bool REC>
-__device__ __forceinline__ void odpos_coop(const DevSetup& S, const DevOdPos& od, const OdEstRecords* er, const int* __restrict__ cols,
-                                           size_t n, const double* state, const double* consts, const long long* epoch0, double* out_state,
-                                           long long* out_epoch, nyxb_details* out_details, int* out_status) {
-    extern __shared__ __align__(16) unsigned char smem[];
-    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    const size_t i = (size_t)blockIdx.x * ODC_WPB + wib;
-    if (i >= n) return;   // whole warps leave together
-    const int npw = S.has_grav ? 3 * (S.grav.N + 2) : 0;
-    const size_t slab = (sizeof(WarpSPos) + sizeof(D3) * (size_t)npw + 15) & ~(size_t)15;
-    WarpSPos& X = *reinterpret_cast<WarpSPos*>(smem + slab * wib);
-    Ctx cx;
-    cx.S = &S; cx.mycols = cols + lane * ODC_KMAX; cx.W = &X.s; cx.lane = lane;
-    cx.pw = reinterpret_cast<D3*>(smem + slab * wib + sizeof(WarpSPos));
-    WarpBPos b(cx, X);
-    od_process_arc<WarpBPos, REC, PosTrk>(od, b, i, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status, er);
-}
-
-__global__ void __launch_bounds__(32 * ODC_WPB)
-nyxb_k_odpos_coop(const __grid_constant__ DevSetup S, const __grid_constant__ DevOdPos od, const int* __restrict__ cols, size_t n,
-                  const double* __restrict__ state, const double* __restrict__ consts, const long long* __restrict__ epoch0,
-                  double* __restrict__ out_state, long long* __restrict__ out_epoch, nyxb_details* __restrict__ out_details,
-                  int* __restrict__ out_status) {
-    odpos_coop<false>(S, od, nullptr, cols, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
-}
-
-__global__ void __launch_bounds__(32 * ODC_WPB)
-nyxb_k_odpos_rec_coop(const __grid_constant__ DevSetup S, const __grid_constant__ DevOdPos od, const OdEstRecords er,
-                      const int* __restrict__ cols, size_t n, const double* __restrict__ state, const double* __restrict__ consts,
-                      const long long* __restrict__ epoch0, double* __restrict__ out_state, long long* __restrict__ out_epoch,
-                      nyxb_details* __restrict__ out_details, int* __restrict__ out_status) {
-    odpos_coop<true>(S, od, &er, cols, n, state, consts, epoch0, out_state, out_epoch, out_details, out_status);
-}
-
-extern "C" size_t nyxb_od_coop_smem_bytes(int degree_or_zero) {
-    const size_t npw = degree_or_zero > 0 ? 3 * (size_t)(degree_or_zero + 2) : 0;
-    const size_t slab = (sizeof(WarpS) + sizeof(D3) * npw + 15) & ~(size_t)15;
-    return slab * ODC_WPB;
-}
-
-extern "C" int nyxb_od_coop_kmax(void) { return ODC_KMAX; }
-
-extern "C" cudaError_t nyxb_launch_od_coop(const DevSetup* S, const DevOd* od, const int* cols, size_t n, const double* state,
-                                           const double* consts, const long long* epoch0, double* out_state, long long* out_epoch,
-                                           nyxb_details* out_details, int* out_status, cudaStream_t stream) {
+template <class Job>
+cudaError_t nyxb_od_coop_launch(const DevSetup& S, const Job& job, const int* cols, size_t n, const OdIo& io, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
-    const size_t smem = nyxb_od_coop_smem_bytes(S->has_grav ? S->grav.N : 0);
-    cudaError_t e = cudaFuncSetAttribute(nyxb_k_od_coop, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const size_t smem = od_coop_slab<Job::NS>(S.has_grav, S.grav.N) * ODC_WPB;
+    cudaError_t e = cudaFuncSetAttribute(nyxb_k_od_coop<Job>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     unsigned grid = (unsigned)((n + ODC_WPB - 1) / ODC_WPB);
-    nyxb_k_od_coop<<<grid, 32 * ODC_WPB, smem, stream>>>(*S, *od, cols, n, state, consts, epoch0, out_state, out_epoch, out_details,
-                                                         out_status);
+    nyxb_k_od_coop<Job><<<grid, 32 * ODC_WPB, smem, st>>>(S, job, cols, n, io.state, io.consts, io.epoch0, io.out_state, io.out_epoch,
+                                                            io.out_details, io.out_status);
     return cudaGetLastError();
 }
 
-extern "C" cudaError_t nyxb_launch_od_rec_coop(const DevSetup* S, const DevOd* od, const OdEstRecords* er, const int* cols, size_t n,
-                                               const double* state, const double* consts, const long long* epoch0, double* out_state,
-                                               long long* out_epoch, nyxb_details* out_details, int* out_status, cudaStream_t stream) {
-    if (n == 0) return cudaSuccess;
-    const size_t smem = nyxb_od_coop_smem_bytes(S->has_grav ? S->grav.N : 0);
-    cudaError_t e = cudaFuncSetAttribute(nyxb_k_od_rec_coop, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    unsigned grid = (unsigned)((n + ODC_WPB - 1) / ODC_WPB);
-    nyxb_k_od_rec_coop<<<grid, 32 * ODC_WPB, smem, stream>>>(*S, *od, *er, cols, n, state, consts, epoch0, out_state, out_epoch,
-                                                             out_details, out_status);
-    return cudaGetLastError();
-}
-
-extern "C" cudaError_t nyxb_launch_pred_coop(const DevSetup* S, const DevOd* od, const int* cols, size_t n, const double* state,
-                                             const double* consts, const long long* epoch0, const long long* end_epoch, const double* dev0,
-                                             const OdRecords* rec, long long* rec_count, double* out_state, long long* out_epoch,
-                                             nyxb_details* out_details, int* out_status, cudaStream_t stream) {
-    if (n == 0) return cudaSuccess;
-    const size_t smem = nyxb_od_coop_smem_bytes(S->has_grav ? S->grav.N : 0);
-    cudaError_t e = cudaFuncSetAttribute(nyxb_k_pred_coop, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    unsigned grid = (unsigned)((n + ODC_WPB - 1) / ODC_WPB);
-    nyxb_k_pred_coop<<<grid, 32 * ODC_WPB, smem, stream>>>(*S, *od, cols, n, state, consts, epoch0, end_epoch, dev0, *rec, rec_count,
-                                                           out_state, out_epoch, out_details, out_status);
-    return cudaGetLastError();
-}
-
-extern "C" cudaError_t nyxb_launch_bls_coop(const DevSetup* S, const DevOd* od, const DevBls* bl, const int* cols, size_t n,
-                                            const double* state, const double* consts, const long long* epoch0, double* out_state,
-                                            long long* out_epoch, nyxb_details* out_details, int* out_status, cudaStream_t stream) {
-    if (n == 0) return cudaSuccess;
-    const size_t smem = nyxb_od_coop_smem_bytes(S->has_grav ? S->grav.N : 0);
-    cudaError_t e = cudaFuncSetAttribute(nyxb_k_bls_coop, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    unsigned grid = (unsigned)((n + ODC_WPB - 1) / ODC_WPB);
-    nyxb_k_bls_coop<<<grid, 32 * ODC_WPB, smem, stream>>>(*S, *od, *bl, cols, n, state, consts, epoch0, out_state, out_epoch, out_details,
-                                                          out_status);
-    return cudaGetLastError();
-}
-
-// er: null for the filter alone
-extern "C" cudaError_t nyxb_launch_odpos_coop(const DevSetup* S, const DevOdPos* od, const OdEstRecords* er, const int* cols, size_t n,
-                                              const double* state, const double* consts, const long long* epoch0, double* out_state,
-                                              long long* out_epoch, nyxb_details* out_details, int* out_status, cudaStream_t stream) {
-    if (n == 0) return cudaSuccess;
-    const size_t npw = S->has_grav ? 3 * (size_t)(S->grav.N + 2) : 0;
-    const size_t smem = ((sizeof(WarpSPos) + sizeof(D3) * npw + 15) & ~(size_t)15) * ODC_WPB;
-    unsigned grid = (unsigned)((n + ODC_WPB - 1) / ODC_WPB);
-    cudaError_t e;
-    if (er) {
-        e = cudaFuncSetAttribute(nyxb_k_odpos_rec_coop, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        nyxb_k_odpos_rec_coop<<<grid, 32 * ODC_WPB, smem, stream>>>(*S, *od, *er, cols, n, state, consts, epoch0, out_state, out_epoch,
-                                                                    out_details, out_status);
-    } else {
-        e = cudaFuncSetAttribute(nyxb_k_odpos_coop, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        nyxb_k_odpos_coop<<<grid, 32 * ODC_WPB, smem, stream>>>(*S, *od, cols, n, state, consts, epoch0, out_state, out_epoch, out_details,
-                                                                out_status);
-    }
-    return cudaGetLastError();
-}
+template cudaError_t nyxb_od_coop_launch(const DevSetup&, const OdFilterJob<DevStation, false>&, const int*, size_t, const OdIo&, cudaStream_t);
+template cudaError_t nyxb_od_coop_launch(const DevSetup&, const OdFilterJob<DevStation, true>&, const int*, size_t, const OdIo&, cudaStream_t);
+template cudaError_t nyxb_od_coop_launch(const DevSetup&, const OdFilterJob<DevPosDevice, false>&, const int*, size_t, const OdIo&, cudaStream_t);
+template cudaError_t nyxb_od_coop_launch(const DevSetup&, const OdFilterJob<DevPosDevice, true>&, const int*, size_t, const OdIo&, cudaStream_t);
+template cudaError_t nyxb_od_coop_launch(const DevSetup&, const OdPredictJob&, const int*, size_t, const OdIo&, cudaStream_t);
+template cudaError_t nyxb_od_coop_launch(const DevSetup&, const OdBlsJob&, const int*, size_t, const OdIo&, cudaStream_t);

@@ -343,8 +343,8 @@ __device__ static bool od_sinv(int M, const double Sk[2][2], double Si[2][2]) {
 //              entry q of row r of K from row r of P H^T;
 // tag(..)      the estimate record's tag, and tag_msr / tag_window its measurement index and window.
 struct GroundTrk {
-    static constexpr int NS = 2;
     using Dev = DevStation;
+    static constexpr int NS = Dev::NS;
     using Win = OdWindow;
     struct Gain { double Si[2][2]; };
     __device__ __forceinline__ static bool absent(const double o[2]) { return o[0] != o[0] && o[1] != o[1]; }
@@ -423,8 +423,8 @@ __device__ __forceinline__ void od_fwd3(const double L[3][3], const double b[3],
 }
 
 struct PosTrk {
-    static constexpr int NS = 3;
     using Dev = DevPosDevice;
+    static constexpr int NS = Dev::NS;
     using Win = OdWindowT<3>;
     // chol: S = L L^T (M = 3), else Si: S^-1 (M <= 2: od_sinv, M = 3: the closed-form 3x3 inverse after a failed Cholesky)
     struct Gain { bool chol; double L[3][3]; double Si[3][3]; };

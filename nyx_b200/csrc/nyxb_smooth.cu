@@ -8,7 +8,7 @@
 // bias subtracted) at estimate k's epoch with the measurement of record k+1.
 //
 // Built once, STRICT and without FMA contraction, like the host API: the 9x9 part is then bit-identical to its host build.  The same
-// body serves the ground station's records (nyxb_k_smooth) and those of position fixes (nyxb_k_smooth_pos).
+// kernel template serves the ground station's records (nyxb_k_smooth<GroundTrk>) and those of position fixes (nyxb_k_smooth<PosTrk>).
 #include "nyxb_od_device.cuh"
 #include "nyxb_smooth.h"
 
@@ -84,20 +84,18 @@ __device__ __forceinline__ void smooth_one(const DevSetup& S, const DevSmoothT<t
         }
 }
 
+template <class TRK>
 __global__ void __launch_bounds__(128)
-nyxb_k_smooth(const __grid_constant__ DevSetup S, const __grid_constant__ DevSmooth sm, size_t n) {
-    smooth_one<GroundTrk>(S, sm, n);
-}
-
-__global__ void __launch_bounds__(128)
-nyxb_k_smooth_pos(const __grid_constant__ DevSetup S, const __grid_constant__ DevSmoothPos sm, size_t n) {
-    smooth_one<PosTrk>(S, sm, n);
+nyxb_k_smooth(const __grid_constant__ DevSetup S, const __grid_constant__ DevSmoothT<typename TRK::Dev> sm, size_t n) {
+    smooth_one<TRK>(S, sm, n);
 }
 
 // A filter whose smoothing failed (err_key >= 0) has no solution in the reference: every output of it becomes NaN, also those that
 // threads of its other estimates wrote.  Runs after nyxb_k_smooth on the same grid.
-template <class Dev, int NS>
-__device__ __forceinline__ void smooth_fail(const DevSmoothT<Dev>& sm, size_t n) {
+template <class TRK>
+__global__ void __launch_bounds__(128)
+nyxb_k_smooth_fail(const __grid_constant__ DevSmoothT<typename TRK::Dev> sm, size_t n) {
+    constexpr int NS = TRK::NS;
     const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (size_t)sm.cap * n) return;
     const size_t i = t % n, k = t / n;
@@ -112,36 +110,18 @@ __device__ __forceinline__ void smooth_fail(const DevSmoothT<Dev>& sm, size_t n)
     if (sm.postfit) for (int q = 0; q < NS; ++q) sm.postfit[(k * NS + q) * n + i] = nan;
 }
 
-__global__ void __launch_bounds__(128)
-nyxb_k_smooth_fail(const __grid_constant__ DevSmooth sm, size_t n) {
-    smooth_fail<DevStation, 2>(sm, n);
-}
-
-__global__ void __launch_bounds__(128)
-nyxb_k_smooth_fail_pos(const __grid_constant__ DevSmoothPos sm, size_t n) {
-    smooth_fail<DevPosDevice, 3>(sm, n);
-}
-
-extern "C" cudaError_t nyxb_launch_smooth(const DevSetup* S, const DevSmooth* sm, size_t n, cudaStream_t stream) {
-    const size_t total = (size_t)sm->cap * n;
+template <class Dev>
+cudaError_t nyxb_smooth_launch(const DevSetup& S, const DevSmoothT<Dev>& sm, size_t n, cudaStream_t st) {
+    const size_t total = (size_t)sm.cap * n;
     if (total == 0) return cudaSuccess;
     const int block = 128;
     const unsigned grid = (unsigned)((total + block - 1) / block);
-    nyxb_k_smooth<<<grid, block, 0, stream>>>(*S, *sm, n);
+    nyxb_k_smooth<typename Dev::Trk><<<grid, block, 0, st>>>(S, sm, n);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
-    nyxb_k_smooth_fail<<<grid, block, 0, stream>>>(*sm, n);
+    nyxb_k_smooth_fail<typename Dev::Trk><<<grid, block, 0, st>>>(sm, n);
     return cudaGetLastError();
 }
 
-extern "C" cudaError_t nyxb_launch_smooth_pos(const DevSetup* S, const DevSmoothPos* sm, size_t n, cudaStream_t stream) {
-    const size_t total = (size_t)sm->cap * n;
-    if (total == 0) return cudaSuccess;
-    const int block = 128;
-    const unsigned grid = (unsigned)((total + block - 1) / block);
-    nyxb_k_smooth_pos<<<grid, block, 0, stream>>>(*S, *sm, n);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    nyxb_k_smooth_fail_pos<<<grid, block, 0, stream>>>(*sm, n);
-    return cudaGetLastError();
-}
+template cudaError_t nyxb_smooth_launch(const DevSetup&, const DevSmoothT<DevStation>&, size_t, cudaStream_t);
+template cudaError_t nyxb_smooth_launch(const DevSetup&, const DevSmoothT<DevPosDevice>&, size_t, cudaStream_t);

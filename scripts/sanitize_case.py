@@ -57,7 +57,7 @@ def run(which):
         sol = sc["odp"].process_arcs(sc["ests"], sc["arc"], record_estimates=True)
         assert (sol.status == 0).all()
         print(which, "filters", 3, "accepted", int(sol.accepted().sum()))
-    elif which == "blse":   # nyxb_k_bls_coop: 3 problems, 4 measurements, LM with a rejected step (lambda0 = 1e-12)
+    elif which == "blse":   # nyxb_k_od_coop<OdBlsJob>: 3 problems, 4 measurements, LM with a rejected step (lambda0 = 1e-12)
         from oracle import pyoracle
         from tests.blse_util import blse_scenario
 

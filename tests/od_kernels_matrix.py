@@ -1,10 +1,10 @@
 """Inputs of the parity matrix of the three ensemble entry points that share the filter's kernels (tests/test_gpu_od_kernels_matrix.py)
 and of its CPU companion (tests/test_od_kernels_matrix_inputs.py):
 
-  predict   nyxb_od_predict_batch (KalmanODProcess::predict_until)            NYXB_KPRED, nyxb_k_pred_coop
-  bls       nyxb_od_bls_batch / nyxb_od_bls_evaluate_batch (BatchLeastSquares) NYXB_KBLS, nyxb_k_bls_coop
-  position  nyxb_od_position_batch + nyxb_od_position_smooth_batch            NYXB_KODPOS[REC], nyxb_k_odpos[_rec]_coop,
-                                                                              nyxb_k_smooth_pos
+  predict   nyxb_od_predict_batch (KalmanODProcess::predict_until)            nyxb_k_od[_coop]<OdPredictJob>
+  bls       nyxb_od_bls_batch / nyxb_od_bls_evaluate_batch (BatchLeastSquares) nyxb_k_od[_coop]<OdBlsJob>
+  position  nyxb_od_position_batch + nyxb_od_position_smooth_batch            nyxb_k_od[_coop]<OdFilterJob<DevPosDevice, REC>>,
+                                                                              nyxb_k_smooth<PosTrk>
 
 Everything is built from tests/od_matrix.py: its four force-model configurations at fixed 45.5 s DP78, its truth orbits, its 13
 initial estimates (dispersed states, per-filter Cr, masses and SRP areas, a covariance with position-velocity and velocity-Cr

@@ -4,9 +4,9 @@ position-fix filter and smoother (nyxb_od_position_batch, nyxb_od_position_smoot
 across the filter matrix of tests/od_matrix.py.  Inputs: tests/od_kernels_matrix.py.
 
 Families, each forced explicitly and checked with `last_kernel()`:
-  STRICT       per-thread kernels (NYXB_KPRED, NYXB_KBLS, NYXB_KODPOS[REC]), STRICT arithmetic
+  STRICT       per-thread kernels (nyxb_k_od<Job> of the prediction, BLS and position-fix jobs), STRICT arithmetic
   FAST-thread  the same kernels, FAST arithmetic                          set_kernel(KERNEL_THREAD)
-  FAST-coop    warp kernels (nyxb_k_pred_coop, nyxb_k_bls_coop, nyxb_k_odpos[_rec]_coop), the FAST default at degree >= 8
+  FAST-coop    warp kernels (nyxb_k_od_coop<Job> of the same jobs), the FAST default at degree >= 8
 
 Cases: every configuration at 21x21 (predict EKF and CKF, BLS normal equations and Levenberg-Marquardt on "srp", the position filter
 at msr_size 3 and 1); the field shapes where the warp kernels' column deal switches (1, 2, 3 and 4 columns per lane, order 0 and
