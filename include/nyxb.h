@@ -38,7 +38,8 @@ extern "C" {
                               nyxb_integ_opts.state_center, nyxb_gravity_field.body, nyxb_dynamics.n_gravity / n_point_masses / point_mass_order; nyxb_od_predict_batch
                               and nyxb_predict_outputs, then nyxb_od_bls_batch, nyxb_od_bls_evaluate_batch, nyxb_bls_config, nyxb_bls_outputs and
                               the status codes 6-8, then nyxb_od_records, nyxb_od_ekf_record_batch, nyxb_smooth_outputs, nyxb_od_smooth_batch,
-                              then NYXB_MSR_X/Y/Z, nyxb_position_device, nyxb_position_arc, nyxb_od_position_batch, nyxb_od_position_smooth_batch
+                              then NYXB_MSR_X/Y/Z, nyxb_position_device, nyxb_position_arc, nyxb_od_position_batch, nyxb_od_position_smooth_batch,
+                              then NYXB_MSR_AZIMUTH/ELEVATION, nyxb_aer_station, nyxb_od_aer_batch, nyxb_od_aer_smooth_batch
                               and the status codes 9-10 were added later without a bump (a pure addition: no existing type or entry point changed).  Earlier: 2: nyxb_srp gained `estimate`; STM, filter and dispersion entry points.  3: nyxb_traj_resample[_dev], nyxb_event_locate[_dev] */
 
 /* ---- IntegratorMethod — propagators/rk_methods/mod.rs:65-79 (same order) ---- */
@@ -402,6 +403,7 @@ int32_t nyxb_propagate_batch_stm(nyxb_engine* eng, size_t n,
  * to each measurement, `KalmanFilter::time_update` / `measurement_update` (od/kalman/filtering.rs:59-316), state
  * replacement (EKF) and STM reset — in ONE kernel launch, one filter per trajectory. */
 enum nyxb_msr_type { NYXB_MSR_RANGE = 0, NYXB_MSR_DOPPLER = 1,   /* od/msr/types.rs:31-45 (the two-way capable ones) */
+                     NYXB_MSR_AZIMUTH = 2, NYXB_MSR_ELEVATION = 3, /* degrees; ground stations with angles (nyxb_aer_station) */
                      NYXB_MSR_X = 6, NYXB_MSR_Y = 7, NYXB_MSR_Z = 8 }; /* position fixes (nyxb_position_device) */
 
 /* GroundStation (od/ground_station/mod.rs:47-75) reduced to what the filter needs.  The host converts latitude /
@@ -608,6 +610,50 @@ int32_t nyxb_od_position_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int3
 int32_t nyxb_od_position_smooth_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_devices, const nyxb_position_device* devices,
                                       const nyxb_position_arc* arc, size_t n, const nyxb_od_records* rec, const int32_t* filter_status,
                                       nyxb_smooth_outputs* out);
+
+/* ---- Angle tracking: a ground station that measures azimuth and elevation (degrees) next to range and Doppler, the filter of
+ * nyxb_od_ekf_batch with nyxb_aer_station in place of nyxb_ground_station.  The observation slot of a type is its value, so the arc
+ * (nyxb_tracking_arc) carries obs [n_msr][4][n] for these entry points: obs[(k*4 + t)*n + i].  As coded in the reference
+ * (ground_station/trk_device.rs:158-208, msr/types.rs:102-117, msr/sensitivity.rs:188-226):
+ *   - rho = r_sc - r_station in the integration frame; elevation = asin(rho . up / |rho|), the value the mask test reads; azimuth =
+ *     atan2(rho . E, rho . N) mapped into [0, 360), E and N the geodetic east and north rotated like up.  The bias is subtracted as for
+ *     range and Doppler; there is no wrap handling (an observed 359.99 deg against a computed 0.01 deg is a prefit of 359.98 deg);
+ *   - h_tilde rows from the integration-frame rho (the reference's comment says "rotate back", the code does not), in rad/km while
+ *     the observations are in degrees: azimuth [-dy, dx, 0] / (dx^2 + dy^2); elevation [-dx dz, -dy dz, .] / (r^2 sqrt(r^2 - dz^2)) and
+ *     sqrt(dx^2 + dy^2) / r^2, r^2 = (sqrt(dx^2 + dy^2 + dz^2))^2.  Identity rows for types absent from the measurement;
+ *   - windows as nyxb_od_ekf_batch: types w*msr_size .. of the station's list; [R, D, Az, El] at msr_size 2 gives [R, D] then
+ *     [Az, El], at msr_size 1 four windows.  n_types need not be a multiple of msr_size (the last window is short, with an identity
+ *     row, a zero R entry and a zero real observation, as the reference).  Range and Doppler are the ground station's arithmetic. */
+typedef struct {
+    double pos_fixed_km[3];
+    double up_fixed[3];          /* unit local zenith in the body-fixed frame */
+    double north_fixed[3];       /* unit geodetic north in the body-fixed frame: (-sin lat cos lon, -sin lat sin lon, cos lat) */
+    double east_fixed[3];        /* unit geodetic east in the body-fixed frame: (-sin lon, cos lon, 0) */
+    double elevation_mask_deg;
+    nyxb_rotation rot;           /* as nyxb_ground_station */
+    int32_t body;
+    int32_t n_types;             /* 1 to 4 */
+    int32_t types[4];            /* NYXB_MSR_RANGE / _DOPPLER / _AZIMUTH / _ELEVATION, distinct, in the device's list order */
+    double noise_var[4];         /* per list position: km^2, km^2/s^2, deg^2 */
+    double bias[4];              /* per list position */
+    double body_radius_km;       /* as nyxb_ground_station */
+} nyxb_aer_station;
+
+/* n filters over one schedule.  cfg as nyxb_od_ekf_batch with msr_size 1 or 2; arc->obs [n_msr][4][n].  out: nyxb_od_outputs whose
+ * per-measurement arrays resid_ratio, prefit and postfit are [n_msr][4][n] (prefit / postfit slot = position of the type in the
+ * station's list; the ratio of window w in slot w).  rec: NULL, or the estimate records of nyxb_od_ekf_record_batch tagged by
+ * NYXB_OD_POS_TAG; `out` is bit-identical either way.  NYXB_RC_BAD_ARG: a type outside 0..3, a duplicate type, n_types outside 1..4,
+ * msr_size outside 1..2, a bad body index, a NULL required pointer; NYXB_RC_UNSUPPORTED: the setups nyxb_propagate_batch_stm rejects.
+ * Per-filter failures are statuses.  Kernel family as nyxb_od_ekf_batch.  HOST pointers everywhere. */
+int32_t nyxb_od_aer_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations, const nyxb_aer_station* stations,
+                          const nyxb_tracking_arc* arc, size_t n, const double* state_soa, const double* consts_soa,
+                          const int64_t* epoch0_ns, const double* covar0_soa, const nyxb_od_outputs* out, const nyxb_od_records* rec);
+
+/* ODSolution::smooth of angle-tracking filters: the contract of nyxb_od_smooth_batch, with the records of nyxb_od_aer_batch, arc->obs
+ * [n_msr][4][n] and out->postfit [capacity][4][n]. */
+int32_t nyxb_od_aer_smooth_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations, const nyxb_aer_station* stations,
+                                 const nyxb_tracking_arc* arc, size_t n, const nyxb_od_records* rec, const int32_t* filter_status,
+                                 nyxb_smooth_outputs* out);
 
 /* ---- Covariance mapping over an ensemble: n independent `KalmanODProcess::predict_until` runs (od/process/mod.rs:440-486) in ONE
  * kernel launch.  Record 0 is the initial estimate; then chunks of cfg->max_step_ns (`for_duration(max_step)`: adaptive steps, the

@@ -14,6 +14,7 @@
 //
 // No arithmetic of the hot path lives here: every propagate call is one nyxb_propagate_batch on the GPU.
 #pragma once
+#include <algorithm>
 #include <cmath>
 #include <cstdint>
 #include <memory>
@@ -435,18 +436,21 @@ class MonteCarlo {
 // Orbit determination (SURVEY.md §8 (f)-2): n sequential Kalman filters over one tracking schedule in ONE launch.
 // ---------------------------------------------------------------------------------------------------------------------
 enum class MeasurementType : int32_t { Range = NYXB_MSR_RANGE, Doppler = NYXB_MSR_DOPPLER,           // od/msr/types.rs:31-45
+                                       Azimuth = NYXB_MSR_AZIMUTH, Elevation = NYXB_MSR_ELEVATION,   // degrees (nyxb_aer_station)
                                        X = NYXB_MSR_X, Y = NYXB_MSR_Y, Z = NYXB_MSR_Z };              // position fixes
 enum class KalmanVariant : int32_t { ReferenceUpdate = NYXB_KF_REFERENCE_UPDATE, DeviationTracking = NYXB_KF_DEVIATION_TRACKING };
 struct StochasticNoise { double sigma = 0.0, bias_constant = 0.0; double covariance() const { return sigma * sigma; } };
 struct SigmaRejection { double num_sigmas = 3.0; };                                                        // process/rejectcrit.rs:35-46
 
-// GroundStation (od/ground_station/mod.rs:47-75; builtin.rs:25-117), instantaneous Range + Doppler
+// GroundStation (od/ground_station/mod.rs:47-75; builtin.rs:25-117), instantaneous Range + Doppler, and Azimuth / Elevation added by
+// with_msr_type (a station with angles runs through nyxb_od_aer_batch)
 struct GroundStation {
     std::string name;
     double latitude_deg = 0, longitude_deg = 0, height_km = 0, elevation_mask_deg = 0;
     Frame frame = IAU_EARTH();
     std::vector<MeasurementType> measurement_types{MeasurementType::Range, MeasurementType::Doppler};
     StochasticNoise range_noise_km{2e-3, 0.0}, doppler_noise_km_s{3e-6, 0.0};
+    StochasticNoise azimuth_noise_deg{}, elevation_noise_deg{};
     static GroundStation dss65_madrid(double mask, StochasticNoise r, StochasticNoise d) { return {"Madrid", 40.427222, 4.250556, 0.834939, mask, IAU_EARTH(), {MeasurementType::Range, MeasurementType::Doppler}, r, d}; }
     static GroundStation dss34_canberra(double mask, StochasticNoise r, StochasticNoise d) { return {"Canberra", -35.398333, 148.981944, 0.691750, mask, IAU_EARTH(), {MeasurementType::Range, MeasurementType::Doppler}, r, d}; }
     static GroundStation dss13_goldstone(double mask, StochasticNoise r, StochasticNoise d) { return {"Goldstone", 35.247164, 243.205, 1.07114904, mask, IAU_EARTH(), {MeasurementType::Range, MeasurementType::Doppler}, r, d}; }
@@ -458,6 +462,47 @@ struct GroundStation {
         const double nu = a / std::sqrt(1.0 - e2 * sl * sl);
         pos[0] = (nu + height_km) * cl * co; pos[1] = (nu + height_km) * cl * so; pos[2] = (nu * (1.0 - e2) + height_km) * sl;
         up[0] = cl * co; up[1] = cl * so; up[2] = sl;
+    }
+    // GroundStation::with_msr_type (ground_station/mod.rs:137-150): sets the type's noise, appends the type unless it is listed
+    GroundStation& with_msr_type(MeasurementType t, StochasticNoise nz) {
+        noise(t) = nz;
+        if (std::find(measurement_types.begin(), measurement_types.end(), t) == measurement_types.end()) measurement_types.push_back(t);
+        return *this;
+    }
+    StochasticNoise& noise(MeasurementType t) {
+        switch (t) {
+            case MeasurementType::Range: return range_noise_km;
+            case MeasurementType::Doppler: return doppler_noise_km_s;
+            case MeasurementType::Azimuth: return azimuth_noise_deg;
+            case MeasurementType::Elevation: return elevation_noise_deg;
+            default: throw std::runtime_error("a ground station measures Range, Doppler, Azimuth or Elevation");
+        }
+    }
+    const StochasticNoise& noise(MeasurementType t) const { return const_cast<GroundStation*>(this)->noise(t); }
+    bool has_angles() const {
+        for (auto t : measurement_types) if (t == MeasurementType::Azimuth || t == MeasurementType::Elevation) return true;
+        return false;
+    }
+    // the station for nyxb_od_aer_batch: the geometry of to_c plus the body-fixed geodetic north and east
+    nyxb_aer_station to_aer_c(const Frame& integration_frame, int32_t body_index, double central_radius_km) const {
+        if (measurement_types.empty() || measurement_types.size() > 4) throw std::runtime_error("a ground station carries one to four types");
+        nyxb_aer_station g{};
+        body_fixed(g.pos_fixed_km, g.up_fixed);
+        const double d2r = 3.14159265358979323846 / 180.0;
+        const double sl = std::sin(latitude_deg * d2r), cl = std::cos(latitude_deg * d2r), so = std::sin(longitude_deg * d2r), co = std::cos(longitude_deg * d2r);
+        g.north_fixed[0] = -sl * co; g.north_fixed[1] = -sl * so; g.north_fixed[2] = cl;
+        g.east_fixed[0] = -so; g.east_fixed[1] = co; g.east_fixed[2] = 0.0;
+        g.elevation_mask_deg = elevation_mask_deg; g.rot = frame.rotation;
+        const bool same = frame.ephemeris_id == integration_frame.ephemeris_id;
+        g.body = same ? NYXB_CENTRAL_BODY : body_index;
+        g.body_radius_km = same ? -1.0 : central_radius_km;
+        g.n_types = (int32_t)measurement_types.size();
+        for (int q = 0; q < g.n_types; ++q) {
+            g.types[q] = (int32_t)measurement_types[q];
+            const StochasticNoise& nz = noise(measurement_types[q]);
+            g.noise_var[q] = nz.covariance(); g.bias[q] = nz.bias_constant;
+        }
+        return g;
     }
     nyxb_ground_station to_c(const Frame& integration_frame, int32_t body_index, double central_radius_km) const {
         nyxb_ground_station g{};
@@ -490,7 +535,8 @@ struct KfEstimate {   // od/estimate/kfestimate.rs: nominal state + 9x9 covarian
 };
 
 // one tracking schedule, n observation sets: obs[(k*ns + slot)*n + i], NaN = type not in the measurement's data; ns = 2 (slot =
-// Range / Doppler) for ground stations, 3 (slot = type - X) for position fixes
+// Range / Doppler) for ground stations, 4 (slot = Range / Doppler / Azimuth / Elevation) for ground stations with angles, 3 (slot =
+// type - X) for position fixes
 struct TrackingDataArc { std::vector<int64_t> epoch_ns; std::vector<std::string> tracker; std::vector<double> obs; size_t n = 0; size_t ns = 2; };
 
 // PositionDevice (od/position/mod.rs): X / Y / Z fixes of the position in the integration frame; with_noise appends the type to the
@@ -516,7 +562,7 @@ class KalmanODProcess;
 class PositionKalmanODProcess;
 
 struct ODSolution {
-    size_t n = 0, m = 0, ns = 2;   // ns: observation slots, 2 (ground stations) or 3 (position fixes)
+    size_t n = 0, m = 0, ns = 2;   // ns: observation slots, 2 (ground stations), 4 (ground stations with angles) or 3 (position fixes)
     std::vector<double> state, covar, state_dev, resid_ratio, prefit, postfit;   // [9][n], [81][n] (c*9+r), [9][n], [m][ns][n] x3
     std::vector<int64_t> epoch; std::vector<int32_t> msr_flags, status; std::vector<nyxb_details> details;
     // every estimate (ODSolution.estimates) when process_arcs ran with an estimates capacity (nyxb_od_records): epoch / tag
@@ -524,7 +570,7 @@ struct ODSolution {
     int64_t rec_capacity = 0;
     std::vector<int64_t> rec_epoch, rec_tag, rec_count;
     std::vector<double> rec_nominal, rec_deviation, rec_covar, rec_stm;
-    // set by smooth(): smoothed state() / deviation / filter-smoother ratios [cap][9][n], covar [cap][81][n], postfit [cap][2][n]
+    // set by smooth(): smoothed state() / deviation / filter-smoother ratios [cap][9][n], covar [cap][81][n], postfit [cap][ns][n]
     // by estimate position (NaN where the reference has None), and the status of each filter's smoothing
     Frame frame = EARTH_J2000();   // integration frame of the run
     bool smoother_run = false;
@@ -534,6 +580,7 @@ struct ODSolution {
     int64_t n_estimates(size_t i) const { return rec_count.empty() ? 0 : std::min(rec_count[i], rec_capacity); }
     bool is_smoother_run() const { return smoother_run; }
     // ODSolution::smooth (od/process/solution/smooth.rs:104-249) of all n filters in one launch; `odp` and `arc` are those of the run
+    // (an arc of four slots: nyxb_od_aer_smooth_batch)
     inline ODSolution smooth(const KalmanODProcess& odp, const TrackingDataArc& arc) const;
     // the same for position fixes (nyxb_od_position_smooth_batch; sm_postfit [cap][3][n])
     inline ODSolution smooth(const PositionKalmanODProcess& odp, const TrackingDataArc& arc) const;
@@ -558,20 +605,43 @@ inline nyxb_od_config od_config(KalmanVariant variant, const std::optional<Sigma
     if (snc) { cfg.snc_enabled = 1; cfg.snc_frame = snc->ric ? 1 : 0; for (int i = 0; i < 3; ++i) cfg.snc_diag[i] = snc->diag[i]; cfg.snc_disable_time_ns = snc->disable_time; }
     return cfg;
 }
-// the devices as nyxb_ground_station, in order; a station on another body than the integration centre needs its ephemeris
+// the index of the station's body in the almanac, or NYXB_CENTRAL_BODY; a station on another body than the integration centre needs
+// its ephemeris
+inline int32_t station_body(const GroundStation& d, const Frame& frame, const Almanac* almanac) {
+    if (d.frame.ephemeris_id == frame.ephemeris_id) return NYXB_CENTRAL_BODY;
+    if (!almanac) throw std::runtime_error("an almanac with the station's body is needed");
+    for (size_t j = 0; j < almanac->bodies.size(); ++j) if (almanac->bodies[j].ephemeris_id == d.frame.ephemeris_id) return (int32_t)j;
+    throw std::runtime_error("no ephemeris loaded for the station's body");
+}
+// the devices as nyxb_ground_station, in order
 inline std::vector<nyxb_ground_station> pack_stations(const std::vector<GroundStation>& devices, const Frame& frame, const Almanac* almanac) {
     std::vector<nyxb_ground_station> st;
-    for (auto& d : devices) {
-        int32_t bi = NYXB_CENTRAL_BODY;
-        if (d.frame.ephemeris_id != frame.ephemeris_id) {
-            if (!almanac) throw std::runtime_error("an almanac with the station's body is needed");
-            bi = -2;
-            for (size_t j = 0; j < almanac->bodies.size(); ++j) if (almanac->bodies[j].ephemeris_id == d.frame.ephemeris_id) bi = (int32_t)j;
-            if (bi == -2) throw std::runtime_error("no ephemeris loaded for the station's body");
-        }
-        st.push_back(d.to_c(frame, bi, frame.mean_equatorial_radius_km));
-    }
+    for (auto& d : devices) st.push_back(d.to_c(frame, station_body(d, frame, almanac), frame.mean_equatorial_radius_km));
     return st;
+}
+// the devices as nyxb_aer_station, in order (nyxb_od_aer_batch)
+inline std::vector<nyxb_aer_station> pack_aer_stations(const std::vector<GroundStation>& devices, const Frame& frame, const Almanac* almanac) {
+    std::vector<nyxb_aer_station> st;
+    for (auto& d : devices) st.push_back(d.to_aer_c(frame, station_body(d, frame, almanac), frame.mean_equatorial_radius_km));
+    return st;
+}
+// the observation slots of a ground-station arc: 4 runs through nyxb_od_aer_batch, 2 through nyxb_od_ekf_batch, which takes no angles
+inline size_t station_slots(const std::vector<GroundStation>& devices, const TrackingDataArc& arc) {
+    if (arc.ns == 4) return 4;
+    for (auto& d : devices)
+        if (d.has_angles()) throw std::runtime_error("stations that measure azimuth or elevation need an arc of four slots (Range, Doppler, Azimuth, Elevation)");
+    return 2;
+}
+// the solution's record arrays for estimates_capacity records of each filter and the nyxb_od_records pointing at them (empty for a
+// negative capacity: no records)
+inline nyxb_od_records alloc_records(ODSolution& s, int64_t estimates_capacity) {
+    if (estimates_capacity < 0) return nyxb_od_records{};
+    const size_t cap = (size_t)estimates_capacity, n = s.n;
+    s.rec_capacity = estimates_capacity;
+    s.rec_epoch.resize(cap * n); s.rec_tag.resize(cap * n); s.rec_count.resize(n);
+    s.rec_nominal.resize(cap * 9 * n); s.rec_deviation.resize(cap * 9 * n); s.rec_covar.resize(cap * 81 * n); s.rec_stm.resize(cap * 81 * n);
+    return nyxb_od_records{estimates_capacity, s.rec_epoch.data(), s.rec_tag.data(), s.rec_nominal.data(), s.rec_deviation.data(), s.rec_covar.data(),
+                           s.rec_stm.data(), s.rec_count.data()};
 }
 // index of each measurement's tracker in `devices`; -1 for an unknown tracker
 inline std::vector<int32_t> tracker_index(const std::vector<GroundStation>& devices, const TrackingDataArc& arc) {
@@ -619,36 +689,41 @@ class KalmanODProcess {
     }
 
     // estimates_capacity >= 0: also record the first estimates_capacity entries of each filter's ODSolution.estimates
-    // (nyxb_od_ekf_record_batch); the filter's outputs are the same bits
+    // (nyxb_od_ekf_record_batch); the filter's outputs are the same bits.  An arc of four slots (arc.ns = 4: Range, Doppler, Azimuth,
+    // Elevation) runs through nyxb_od_aer_batch, with record tags NYXB_OD_POS_TAG; stations with angles need one.
     ODSolution process_arcs(const std::vector<KfEstimate>& initial, const TrackingDataArc& arc, int64_t estimates_capacity = -1) const {
         const size_t n = initial.size(), m = arc.epoch_ns.size();
-        if (arc.n != n || arc.obs.size() != m * 2 * n || arc.tracker.size() != m) throw std::runtime_error("arc shape does not match the filters");
+        const size_t ns = detail::station_slots(devices, arc);
+        if (arc.n != n || arc.obs.size() != m * ns * n || arc.tracker.size() != m) throw std::runtime_error("arc shape does not match the filters");
         std::vector<Spacecraft> noms; for (auto& e : initial) noms.push_back(e.nominal_state);
         const Frame& frame = noms.at(0).frame;
         auto eng = detail::make_engine(prop.dynamics, frame, almanac, prop.method, prop.opts, prop.mode, prop.device);
         detail::Soa soa(noms);
         std::vector<double> cov0(81 * n);
         for (size_t i = 0; i < n; ++i) for (int r = 0; r < 9; ++r) for (int c = 0; c < 9; ++c) cov0[(size_t)(c * 9 + r) * n + i] = initial[i].covar[r * 9 + c];
-        std::vector<nyxb_ground_station> st = detail::pack_stations(devices, frame, almanac);
         std::vector<int32_t> trk = detail::tracker_index(devices, arc);
         const nyxb_od_config cfg = config();
         nyxb_tracking_arc carc{(int64_t)m, arc.epoch_ns.data(), trk.data(), arc.obs.data()};
-        ODSolution s; s.n = n; s.m = m; s.frame = frame;
-        s.state.resize(9 * n); s.epoch.resize(n); s.covar.resize(81 * n); s.state_dev.resize(9 * n); s.resid_ratio.resize(m * 2 * n); s.prefit.resize(m * 2 * n);
-        s.postfit.resize(m * 2 * n); s.msr_flags.resize(m * n); s.details.resize(n); s.status.resize(n);
+        ODSolution s; s.n = n; s.m = m; s.ns = ns; s.frame = frame;
+        s.state.resize(9 * n); s.epoch.resize(n); s.covar.resize(81 * n); s.state_dev.resize(9 * n); s.resid_ratio.resize(m * ns * n); s.prefit.resize(m * ns * n);
+        s.postfit.resize(m * ns * n); s.msr_flags.resize(m * n); s.details.resize(n); s.status.resize(n);
         nyxb_od_outputs out{s.state.data(), s.epoch.data(), s.covar.data(), s.state_dev.data(), s.resid_ratio.data(), s.prefit.data(), s.postfit.data(),
                             s.msr_flags.data(), nullptr, nullptr, s.details.data(), s.status.data()};
+        if (ns == 4) {
+            const std::vector<nyxb_aer_station> ast = detail::pack_aer_stations(devices, frame, almanac);
+            nyxb_od_records rec = detail::alloc_records(s, estimates_capacity);
+            if (nyxb_od_aer_batch(eng.get(), &cfg, (int32_t)ast.size(), ast.data(), &carc, n, soa.state.data(), soa.consts.data(), soa.epoch.data(),
+                                  cov0.data(), &out, estimates_capacity >= 0 ? &rec : nullptr) != NYXB_RC_OK)
+                throw std::runtime_error(std::string("nyxb_od_aer_batch: ") + nyxb_last_error());
+            return s;
+        }
+        std::vector<nyxb_ground_station> st = detail::pack_stations(devices, frame, almanac);
         if (estimates_capacity < 0) {
             if (nyxb_od_ekf_batch(eng.get(), &cfg, (int32_t)st.size(), st.data(), &carc, n, soa.state.data(), soa.consts.data(), soa.epoch.data(), cov0.data(), &out) != NYXB_RC_OK)
                 throw std::runtime_error(std::string("nyxb_od_ekf_batch: ") + nyxb_last_error());
             return s;
         }
-        const size_t cap = (size_t)estimates_capacity;
-        s.rec_capacity = estimates_capacity;
-        s.rec_epoch.resize(cap * n); s.rec_tag.resize(cap * n); s.rec_count.resize(n);
-        s.rec_nominal.resize(cap * 9 * n); s.rec_deviation.resize(cap * 9 * n); s.rec_covar.resize(cap * 81 * n); s.rec_stm.resize(cap * 81 * n);
-        nyxb_od_records rec{estimates_capacity, s.rec_epoch.data(), s.rec_tag.data(), s.rec_nominal.data(), s.rec_deviation.data(), s.rec_covar.data(),
-                            s.rec_stm.data(), s.rec_count.data()};
+        nyxb_od_records rec = detail::alloc_records(s, estimates_capacity);
         if (nyxb_od_ekf_record_batch(eng.get(), &cfg, (int32_t)st.size(), st.data(), &carc, n, soa.state.data(), soa.consts.data(), soa.epoch.data(),
                                      cov0.data(), &out, &rec) != NYXB_RC_OK)
             throw std::runtime_error(std::string("nyxb_od_ekf_record_batch: ") + nyxb_last_error());
@@ -662,7 +737,7 @@ inline ODSolution ODSolution::smooth(const KalmanODProcess& odp, const TrackingD
     // the engine of the filter run (its dynamics and integration frame) supplies the stations' ephemerides
     const Frame& integ = frame;
     auto eng = detail::make_engine(odp.prop.dynamics, integ, odp.almanac, odp.prop.method, odp.prop.opts, odp.prop.mode, odp.prop.device);
-    std::vector<nyxb_ground_station> st = detail::pack_stations(odp.devices, integ, odp.almanac);
+    const size_t slots = detail::station_slots(odp.devices, arc);
     std::vector<int32_t> trk = detail::tracker_index(odp.devices, arc);
     const nyxb_od_config cfg = odp.config();
     nyxb_tracking_arc carc{(int64_t)m, arc.epoch_ns.data(), trk.data(), arc.obs.data()};
@@ -673,8 +748,15 @@ inline ODSolution ODSolution::smooth(const KalmanODProcess& odp, const TrackingD
     const size_t cap = (size_t)rec_capacity;
     s.smoother_run = true;
     s.sm_state.resize(cap * 9 * n); s.sm_deviation.resize(cap * 9 * n); s.sm_covar.resize(cap * 81 * n); s.sm_fs_ratio.resize(cap * 9 * n);
-    s.sm_postfit.resize(cap * 2 * n); s.sm_status.resize(n);
+    s.sm_postfit.resize(cap * slots * n); s.sm_status.resize(n);
     nyxb_smooth_outputs out{s.sm_state.data(), s.sm_deviation.data(), s.sm_covar.data(), s.sm_fs_ratio.data(), s.sm_postfit.data(), s.sm_status.data()};
+    if (slots == 4) {
+        const std::vector<nyxb_aer_station> ast = detail::pack_aer_stations(odp.devices, integ, odp.almanac);
+        if (nyxb_od_aer_smooth_batch(eng.get(), &cfg, (int32_t)ast.size(), ast.data(), &carc, n, &rec, status.data(), &out) != NYXB_RC_OK)
+            throw std::runtime_error(std::string("nyxb_od_aer_smooth_batch: ") + nyxb_last_error());
+        return s;
+    }
+    std::vector<nyxb_ground_station> st = detail::pack_stations(odp.devices, integ, odp.almanac);
     if (nyxb_od_smooth_batch(eng.get(), &cfg, (int32_t)st.size(), st.data(), &carc, n, &rec, status.data(), &out) != NYXB_RC_OK)
         throw std::runtime_error(std::string("nyxb_od_smooth_batch: ") + nyxb_last_error());
     return s;
@@ -716,15 +798,7 @@ class PositionKalmanODProcess {
         s.postfit.resize(m * 3 * n); s.msr_flags.resize(m * n); s.details.resize(n); s.status.resize(n);
         nyxb_od_outputs out{s.state.data(), s.epoch.data(), s.covar.data(), s.state_dev.data(), s.resid_ratio.data(), s.prefit.data(), s.postfit.data(),
                             s.msr_flags.data(), nullptr, nullptr, s.details.data(), s.status.data()};
-        nyxb_od_records rec{};
-        if (estimates_capacity >= 0) {
-            const size_t cap = (size_t)estimates_capacity;
-            s.rec_capacity = estimates_capacity;
-            s.rec_epoch.resize(cap * n); s.rec_tag.resize(cap * n); s.rec_count.resize(n);
-            s.rec_nominal.resize(cap * 9 * n); s.rec_deviation.resize(cap * 9 * n); s.rec_covar.resize(cap * 81 * n); s.rec_stm.resize(cap * 81 * n);
-            rec = nyxb_od_records{estimates_capacity, s.rec_epoch.data(), s.rec_tag.data(), s.rec_nominal.data(), s.rec_deviation.data(), s.rec_covar.data(),
-                                  s.rec_stm.data(), s.rec_count.data()};
-        }
+        nyxb_od_records rec = detail::alloc_records(s, estimates_capacity);
         if (nyxb_od_position_batch(eng.get(), &cfg, (int32_t)dev.size(), dev.data(), &carc, n, soa.state.data(), soa.consts.data(), soa.epoch.data(),
                                    cov0.data(), &out, estimates_capacity >= 0 ? &rec : nullptr) != NYXB_RC_OK)
             throw std::runtime_error(std::string("nyxb_od_position_batch: ") + nyxb_last_error());

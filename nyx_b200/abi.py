@@ -162,6 +162,7 @@ class EventC(C.Structure):
 # ---- orbit determination (SURVEY.md §8 (f)-2): mirrors of nyxb_ground_station / nyxb_od_config / nyxb_tracking_arc / nyxb_od_outputs /
 # nyxb_od_records / nyxb_smooth_outputs / nyxb_predict_outputs / nyxb_bls_config / nyxb_bls_outputs
 MSR_RANGE, MSR_DOPPLER = 0, 1
+MSR_AZIMUTH, MSR_ELEVATION = 2, 3  # degrees; ground stations with angles (nyxb_aer_station)
 MSR_X, MSR_Y, MSR_Z = 6, 7, 8      # position fixes (nyxb_position_device)
 KF_REFERENCE_UPDATE, KF_DEVIATION_TRACKING = 0, 1
 MSRF_PROCESSED, MSRF_REJECTED, MSRF_NOT_VISIBLE, MSRF_ABSENT = 1, 2, 4, 8
@@ -201,6 +202,23 @@ class GroundStationC(C.Structure):
         ("_pad", C.c_int32),
         ("noise_var", C.c_double * 2),
         ("bias", C.c_double * 2),
+        ("body_radius_km", C.c_double),
+    ]
+
+
+class AerStationC(C.Structure):
+    _fields_ = [
+        ("pos_fixed_km", C.c_double * 3),
+        ("up_fixed", C.c_double * 3),
+        ("north_fixed", C.c_double * 3),
+        ("east_fixed", C.c_double * 3),
+        ("elevation_mask_deg", C.c_double),
+        ("rot", Rotation),
+        ("body", C.c_int32),
+        ("n_types", C.c_int32),
+        ("types", C.c_int32 * 4),
+        ("noise_var", C.c_double * 4),
+        ("bias", C.c_double * 4),
         ("body_radius_km", C.c_double),
     ]
 
@@ -410,6 +428,12 @@ def _declare(lib):
     lib.nyxb_od_smooth_batch.restype = C.c_int32
     lib.nyxb_od_smooth_batch.argtypes = [vp, C.POINTER(OdConfigC), C.c_int32, C.POINTER(GroundStationC), C.POINTER(TrackingArcC),
                                          C.c_size_t, C.POINTER(OdRecordsC), vp, C.POINTER(SmoothOutputsC)]
+    lib.nyxb_od_aer_batch.restype = C.c_int32
+    lib.nyxb_od_aer_batch.argtypes = [vp, C.POINTER(OdConfigC), C.c_int32, C.POINTER(AerStationC), C.POINTER(TrackingArcC), C.c_size_t,
+                                      vp, vp, vp, vp, C.POINTER(OdOutputsC), C.POINTER(OdRecordsC)]
+    lib.nyxb_od_aer_smooth_batch.restype = C.c_int32
+    lib.nyxb_od_aer_smooth_batch.argtypes = [vp, C.POINTER(OdConfigC), C.c_int32, C.POINTER(AerStationC), C.POINTER(TrackingArcC),
+                                             C.c_size_t, C.POINTER(OdRecordsC), vp, C.POINTER(SmoothOutputsC)]
     lib.nyxb_od_position_batch.restype = C.c_int32
     lib.nyxb_od_position_batch.argtypes = [vp, C.POINTER(OdConfigC), C.c_int32, C.POINTER(PositionDeviceC), C.POINTER(PositionArcC),
                                            C.c_size_t, vp, vp, vp, vp, C.POINTER(OdOutputsC), C.POINTER(OdRecordsC)]
@@ -482,6 +506,8 @@ EXPORTED_SYMBOLS = [
     "nyxb_od_smooth_batch",
     "nyxb_od_position_batch",
     "nyxb_od_position_smooth_batch",
+    "nyxb_od_aer_batch",
+    "nyxb_od_aer_smooth_batch",
     "nyxb_od_predict_batch",
     "nyxb_od_bls_batch",
     "nyxb_od_bls_evaluate_batch",

@@ -38,7 +38,7 @@ static_assert(sizeof(nyxb_integ_opts) == 56 && sizeof(nyxb_gravity_field) == 104
 static_assert(sizeof(nyxb_ground_station) == 176 && sizeof(nyxb_od_config) == 72 && sizeof(nyxb_tracking_arc) == 32 && sizeof(nyxb_od_outputs) == 96, "ABI layout");
 static_assert(sizeof(nyxb_bls_config) == 80 && sizeof(nyxb_bls_outputs) == 72, "ABI layout");
 static_assert(sizeof(nyxb_od_records) == 64 && sizeof(nyxb_smooth_outputs) == 48, "ABI layout");
-static_assert(sizeof(nyxb_position_device) == 64 && sizeof(nyxb_position_arc) == 32, "ABI layout");
+static_assert(sizeof(nyxb_position_device) == 64 && sizeof(nyxb_position_arc) == 32 && sizeof(nyxb_aer_station) == 256, "ABI layout");
 
 static thread_local std::string g_err;
 static void set_err(const std::string& s) { g_err = s; }
@@ -941,6 +941,29 @@ DevStation pack_station(const nyxb_ground_station& g) {
     d.body_radius = g.body_radius_km;
     return d;
 }
+// the checks and packing of a list of stations with angles (nyxb_od_aer_batch / _smooth_batch)
+int32_t pack_aer_stations(const nyxb_engine* eng, int32_t n_stations, const nyxb_aer_station* stations, std::vector<DevAerStation>& hs) {
+    hs.assign((size_t)(n_stations > 0 ? n_stations : 0), DevAerStation{});
+    for (int32_t s = 0; s < n_stations; ++s) {
+        const nyxb_aer_station& g = stations[s];
+        if (g.n_types < 1 || g.n_types > 4) { set_err("bad station: n_types must be 1 to 4"); return NYXB_RC_BAD_ARG; }
+        if (g.body != NYXB_CENTRAL_BODY && (g.body < 0 || g.body >= eng->S.n_bodies)) { set_err("bad ground station descriptor"); return NYXB_RC_BAD_ARG; }
+        for (int q = 0; q < g.n_types; ++q) {
+            if (g.types[q] < NYXB_MSR_RANGE || g.types[q] > NYXB_MSR_ELEVATION) {
+                set_err("bad station: measurement types must be Range, Doppler, Azimuth or Elevation");
+                return NYXB_RC_BAD_ARG;
+            }
+            for (int p = 0; p < q; ++p)
+                if (g.types[p] == g.types[q]) { set_err("bad station: duplicate measurement type"); return NYXB_RC_BAD_ARG; }
+        }
+        DevAerStation& d = hs[s];
+        for (int q = 0; q < 3; ++q) { d.pos[q] = g.pos_fixed_km[q]; d.up[q] = g.up_fixed[q]; d.north[q] = g.north_fixed[q]; d.east[q] = g.east_fixed[q]; }
+        d.mask_deg = g.elevation_mask_deg; d.rot = pack_rot(g.rot); d.body = g.body; d.n_types = g.n_types;
+        for (int q = 0; q < 4; ++q) { d.types[q] = g.types[q]; d.noise_var[q] = g.noise_var[q]; d.bias[q] = g.bias[q]; }
+        d.body_radius = g.body_radius_km;
+    }
+    return NYXB_RC_OK;
+}
 // the checks and packing of a position device list (nyxb_od_position_batch / _smooth_batch)
 int32_t pack_position_devices(int32_t n_devices, const nyxb_position_device* devices, std::vector<DevPosDevice>& hs) {
     hs.assign((size_t)(n_devices > 0 ? n_devices : 0), DevPosDevice{});
@@ -970,13 +993,13 @@ bool records_ok(const nyxb_od_records* rec) {
     return true;
 }
 
-// The argument checks the ground-station (Dev = DevStation) and position-fix filter calls share, in this order.  The ground-station
-// calls check the engine's setup after the records; nyxb_od_position_batch checks it after its devices.
+// The argument checks the ground-station (Dev = DevStation or DevAerStation) and position-fix filter calls share, in this order.  The
+// ground-station calls check the engine's setup after the records; nyxb_od_position_batch checks it after its devices.
 template <class Dev, class Arc, class Trk>
 int32_t filter_args(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_dev, const Trk* devs, const Arc* arc, const double* state_soa,
                     const double* consts_soa, const int64_t* epoch0_ns, const double* covar0_soa, const nyxb_od_outputs* out,
                     const nyxb_od_records* rec) {
-    constexpr bool ground = std::is_same<Dev, DevStation>::value;
+    constexpr bool ground = !std::is_same<Dev, DevPosDevice>::value;
     if (!eng || !cfg || !arc || !state_soa || !consts_soa || !epoch0_ns || !covar0_soa || !out || !out->state_soa || !out->epoch_ns ||
         !out->covar_soa || !out->status || (n_dev > 0 && !devs) || n_dev < 0) {
         set_err("null argument");
@@ -984,7 +1007,7 @@ int32_t filter_args(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_dev, 
     }
     if (rec && !records_ok(rec)) return NYXB_RC_BAD_ARG;
     if (ground && !stm_supported(eng)) return NYXB_RC_UNSUPPORTED;
-    if (cfg->msr_size < 1 || cfg->msr_size > Dev::NS) { set_err(ground ? "msr_size must be 1 or 2" : "msr_size must be 1, 2 or 3"); return NYXB_RC_BAD_ARG; }
+    if (cfg->msr_size < 1 || cfg->msr_size > (ground ? 2 : 3)) { set_err(ground ? "msr_size must be 1 or 2" : "msr_size must be 1, 2 or 3"); return NYXB_RC_BAD_ARG; }
     if (cfg->variant != NYXB_KF_REFERENCE_UPDATE && cfg->variant != NYXB_KF_DEVIATION_TRACKING) { set_err("bad filter variant"); return NYXB_RC_BAD_ARG; }
     if (cfg->max_step_ns <= 0) { set_err("StepSize: max_step must be positive (process/mod.rs:147-150)"); return NYXB_RC_BAD_ARG; }
     if (arc->n_msr < 2) { set_err("TooFewMeasurements: need 2 (process/mod.rs:139-145)"); return NYXB_RC_BAD_ARG; }
@@ -1118,7 +1141,7 @@ extern "C" int32_t nyxb_od_ekf_record_batch(nyxb_engine* eng, const nyxb_od_conf
 
 namespace {
 // The record tags and windows of each tracker kind (NYXB_OD_TAG_*, NYXB_OD_POS_TAG_*, include/nyxb.h).  A ground station's window must
-// lie within its types; a position device's window need only start within them.
+// lie within its types; the window of a position device or of a station with angles need only start within them.
 struct GroundTags {
     static int64_t msr(int64_t tg) { return NYXB_OD_TAG_MSR(tg); }
     static int window(int64_t tg) { return (int)NYXB_OD_TAG_WINDOW(tg); }
@@ -1253,6 +1276,33 @@ extern "C" int32_t nyxb_od_position_smooth_batch(nyxb_engine* eng, const nyxb_od
     if (arc->n_msr < 0 || (arc->n_msr > 0 && (!arc->tracker || !arc->obs))) { set_err("null tracking arc arrays"); return NYXB_RC_BAD_ARG; }
     std::vector<DevPosDevice> hs;
     if (int32_t rc = pack_position_devices(n_devices, devices, hs)) return rc;
+    return od_smooth_run<PosTags>(eng, cfg->msr_size, hs, arc->n_msr, arc->tracker, arc->obs, n, rec, filter_status, out);
+}
+
+extern "C" int32_t nyxb_od_aer_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations, const nyxb_aer_station* stations,
+                                     const nyxb_tracking_arc* arc, size_t n, const double* state_soa, const double* consts_soa,
+                                     const int64_t* epoch0_ns, const double* covar0_soa, const nyxb_od_outputs* out, const nyxb_od_records* rec) {
+    if (int32_t rc = filter_args<DevAerStation>(eng, cfg, n_stations, stations, arc, state_soa, consts_soa, epoch0_ns, covar0_soa, out, rec))
+        return rc;
+    std::vector<DevAerStation> hs;
+    if (int32_t rc = pack_aer_stations(eng, n_stations, stations, hs)) return rc;
+    if (n == 0) return NYXB_RC_OK;
+    return od_filter_run(eng, cfg, hs, arc->n_msr, arc->epoch_ns, arc->tracker, arc->obs, n, state_soa, consts_soa, epoch0_ns, covar0_soa,
+                         out, rec);
+}
+
+extern "C" int32_t nyxb_od_aer_smooth_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations, const nyxb_aer_station* stations,
+                                            const nyxb_tracking_arc* arc, size_t n, const nyxb_od_records* rec, const int32_t* filter_status,
+                                            nyxb_smooth_outputs* out) {
+    if (!eng || !cfg || !arc || !rec || !filter_status || !out || !out->status || (n_stations > 0 && !stations) || n_stations < 0) {
+        set_err("null argument");
+        return NYXB_RC_BAD_ARG;
+    }
+    if (cfg->msr_size != 1 && cfg->msr_size != 2) { set_err("msr_size must be 1 or 2"); return NYXB_RC_BAD_ARG; }
+    if (!records_ok(rec)) return NYXB_RC_BAD_ARG;
+    if (arc->n_msr < 0 || (arc->n_msr > 0 && (!arc->tracker || !arc->obs))) { set_err("null tracking arc arrays"); return NYXB_RC_BAD_ARG; }
+    std::vector<DevAerStation> hs;
+    if (int32_t rc = pack_aer_stations(eng, n_stations, stations, hs)) return rc;
     return od_smooth_run<PosTags>(eng, cfg->msr_size, hs, arc->n_msr, arc->tracker, arc->obs, n, rec, filter_status, out);
 }
 

@@ -19,7 +19,7 @@
 //   KalmanFilter::{time_update, measurement_update}            od/kalman/filtering.rs:59-316
 //   BatchLeastSquares::{estimate, evaluate}                    od/blse/mod.rs:146-541
 //   ProcessNoise::propagate                                    od/snc.rs:175-286
-//   GroundStation::measure_instantaneous, ScalarSensitivity    od/ground_station/trk_device.rs:154-200, od/msr/sensitivity.rs:118-239
+//   GroundStation::measure_instantaneous, ScalarSensitivity    od/ground_station/trk_device.rs:154-208, od/msr/sensitivity.rs:118-239
 // The reference gets the partials from forward-mode dual numbers (hyperdual 1.5.0); so does this file, with a 3-partial
 // dual type (only d/d(position) is ever read).
 #include "nyxb_od_arc.cuh"
@@ -104,6 +104,8 @@ template cudaError_t launch(const DevSetup&, const OdFilterJob<DevStation, false
 template cudaError_t launch(const DevSetup&, const OdFilterJob<DevStation, true>&, size_t, const OdIo&, cudaStream_t);
 template cudaError_t launch(const DevSetup&, const OdFilterJob<DevPosDevice, false>&, size_t, const OdIo&, cudaStream_t);
 template cudaError_t launch(const DevSetup&, const OdFilterJob<DevPosDevice, true>&, size_t, const OdIo&, cudaStream_t);
+template cudaError_t launch(const DevSetup&, const OdFilterJob<DevAerStation, false>&, size_t, const OdIo&, cudaStream_t);
+template cudaError_t launch(const DevSetup&, const OdFilterJob<DevAerStation, true>&, size_t, const OdIo&, cudaStream_t);
 template cudaError_t launch(const DevSetup&, const OdPredictJob&, size_t, const OdIo&, cudaStream_t);
 template cudaError_t launch(const DevSetup&, const OdBlsJob&, size_t, const OdIo&, cudaStream_t);
 

@@ -7,6 +7,7 @@
 
 struct GroundTrk;            // the measurement model of each tracker kind (nyxb_od_device.cuh)
 struct PosTrk;
+struct AerTrk;
 
 // NS: the observation slots of one measurement (obs is [m][NS][n])
 struct DevStation {
@@ -31,7 +32,22 @@ struct DevPosDevice {
     double noise_var[3], bias[3];
 };
 
-// Dev: the tracker kind (DevStation, or DevPosDevice for position fixes, whose observations are [m][3][n])
+// A ground station that may also measure azimuth and elevation: DevStation's geometry plus the body-fixed geodetic north and east,
+// with up to four types (range, Doppler, azimuth, elevation).  The observation slot of a type is its value (obs is [m][4][n]);
+// noise_var / bias per list position.
+struct DevAerStation {
+    static constexpr int NS = 4;
+    using Trk = AerTrk;
+    double pos[3], up[3], north[3], east[3];
+    double mask_deg;
+    DevRotation rot;
+    int body, n_types;
+    int types[4];
+    double noise_var[4], bias[4];
+    double body_radius;
+};
+
+// Dev: the tracker kind (DevStation, DevPosDevice for position fixes, whose observations are [m][3][n], or DevAerStation, [m][4][n])
 template <class Dev>
 struct DevOdT {
     int variant, msr_size;
@@ -45,14 +61,14 @@ struct DevOdT {
     long long n_msr;
     const long long* msr_epoch;    // [m]
     const int* msr_tracker;        // [m]
-    const double* obs;             // [m][2][n] ([m][3][n] for position fixes)
+    const double* obs;             // [m][Dev::NS][n]
     const double* covar0;          // [81][n]
     // outputs (any of the per-measurement ones may be null)
     double* covar;                 // [81][n]
     double* state_dev;             // [9][n] or null
-    double* ratio;                 // [m][2][n] (slots: as obs)
-    double* prefit;                // [m][2][n]
-    double* postfit;               // [m][2][n]
+    double* ratio;                 // [m][Dev::NS][n] (slots: as obs)
+    double* prefit;                // [m][Dev::NS][n]
+    double* postfit;               // [m][Dev::NS][n]
     int* flags;                    // [m][n]
     double* est_state;             // [m][9][n]
     double* est_cov;               // [m][9][n]
@@ -91,7 +107,7 @@ struct DevSmoothT {
     int n_stations;
     const Dev* stations;
     const int* msr_tracker;        // [m]
-    const double* obs;             // [m][2][n]
+    const double* obs;             // [m][Dev::NS][n]
     long long cap;
     const long long* epoch;        // records, layout of OdEstRecords (nyxb_od.cuh)
     const long long* tag;
@@ -105,7 +121,7 @@ struct DevSmoothT {
     double* sdev;                  // [cap][9][n] or null
     double* scov;                  // [cap][81][n] or null
     double* ratio;                 // [cap][9][n] or null
-    double* postfit;               // [cap][2][n] or null
+    double* postfit;               // [cap][Dev::NS][n] or null
     long long* err_key;            // [n] -1, or the largest 2k + (1: singular Phi, 0: ephemeris) among the failing estimates k
 };
 

@@ -284,7 +284,7 @@ __device__ __forceinline__ void od_est_push(const OdEstRecords& er, long long& c
 
 // Loads filter i, runs the whole arc and stores the final covariance, deviation, state, details and status.  REC: also write one
 // estimate record per entry of the reference's ODSolution.estimates into *er (null when REC is false); the filter's arithmetic and
-// outputs are the same either way.  TRK: the tracker kind (GroundTrk, PosTrk in nyxb_od_device.cuh); B::Filt's PHt and K hold
+// outputs are the same either way.  TRK: the tracker kind (GroundTrk, PosTrk, AerTrk in nyxb_od_device.cuh); B::Filt's PHt and K hold
 // 9 x TRK::NS entries.
 template <class B, bool REC = false, class TRK = GroundTrk>
 __device__ void od_process_arc(const DevOdT<typename TRK::Dev>& od, B& b, size_t i, size_t n, const double* state, const double* consts, const long long* epoch0,
@@ -375,7 +375,7 @@ __device__ void od_process_arc(const DevOdT<typename TRK::Dev>& od, B& b, size_t
                 for (int q = 0; q < M; ++q) pre[q] = w.real_obs[q] - w.comp[q];
                 double ratio;
                 if (!TRK::ratio(M, Sk, Rk, pre, ratio)) { rc = NYXB_ERR_PROP_MATH; break; }   // SingularNoiseRk
-                const int rslot = (M == 1) ? wno : 0;
+                const int rslot = TRK::ratio_slot(M, wno);
                 if (b.lead()) {
                     if (od.ratio) od.ratio[((size_t)k * NS + rslot) * n + i] = ratio;
                     if (od.prefit) for (int q = 0; q < w.ncur; ++q) od.prefit[((size_t)k * NS + wno * M + q) * n + i] = pre[q];

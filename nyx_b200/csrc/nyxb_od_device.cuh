@@ -207,8 +207,10 @@ __device__ static int dual_eom_dev(const DevSetup& S, long long t_ns, const doub
 }
 
 // ------------------------------------------------------------------------- tracking geometry
-// trk_device.rs:150-152 `location`: antenna position / velocity in the integration frame and the inertial zenith
-__device__ static bool station_state(const DevSetup& S, const DevStation& st, long long t_ns, double r[3], double v[3], double up[3]) {
+// trk_device.rs:150-152 `location`: antenna position / velocity in the integration frame and the inertial zenith.  St: DevStation, or
+// DevAerStation, whose body-fixed north and east are rotated alike into ne[0] and ne[1].
+template <class St>
+__device__ static bool station_state(const DevSetup& S, const St& st, long long t_ns, double r[3], double v[3], double up[3], double ne[2][3]) {
     double R[9];
     rotation_dcm(st.rot, t_ns, R);
     const double wdot = st.rot.kind ? st.rot.wdot : 0.0;
@@ -218,6 +220,10 @@ __device__ static bool station_state(const DevSetup& S, const DevStation& st, lo
         r[i] = (R[i] * st.pos[0] + R[3 + i] * st.pos[1]) + R[6 + i] * st.pos[2];
         v[i] = (R[i] * vf[0] + R[3 + i] * vf[1]) + R[6 + i] * vf[2];
         up[i] = (R[i] * st.up[0] + R[3 + i] * st.up[1]) + R[6 + i] * st.up[2];
+        if constexpr (St::NS == 4) {
+            ne[0][i] = (R[i] * st.north[0] + R[3 + i] * st.north[1]) + R[6 + i] * st.north[2];
+            ne[1][i] = (R[i] * st.east[0] + R[3 + i] * st.east[1]) + R[6 + i] * st.east[2];
+        }
     }
     if (st.body != NYXB_CENTRAL_BODY) {
         double bp[3], bv[3];
@@ -235,7 +241,7 @@ __device__ static bool station_state(const DevSetup& S, const DevStation& st, lo
 // noise and the computed observation minus the device bias.  Shared by the per-thread and the warp-cooperative filter kernels.
 // SUB_BIAS = false leaves the bias in: the batch least-squares estimator compares with measure_instantaneous(state, None), which
 // has no noise and no bias (blse/mod.rs:248-249).
-// NS: observation slots of the tracker kind (2 for the ground station, 3 for position fixes)
+// NS: observation slots of the tracker kind (2 for the ground station, 3 for position fixes, 4 for a station with angles)
 template <int NS>
 struct OdWindowT {
     int ncur;
@@ -247,20 +253,28 @@ struct OdWindowT {
 using OdWindow = OdWindowT<2>;
 enum { OD_WIN_OK = 0, OD_WIN_EMPTY = 1, OD_WIN_UNAVAILABLE = 2, OD_WIN_NOT_VISIBLE = 3, OD_WIN_EPHEMERIS = 4 };
 
-template <bool SUB_BIAS = true>
-__device__ static int od_window_setup(const DevSetup& S, const DevStation& gs, int M, int wno, const double o[2], long long t_k,
-                                      const double y[9], OdWindow& w) {
+// St: DevStation (range, Doppler) or DevAerStation, which adds azimuth and elevation (trk_device.rs:158-208, msr/types.rs:102-117,
+// sensitivity.rs:188-226).  The observation slot of a type is its value.  The angles, in degrees, come from rho = r_sc - r_station in
+// the integration frame: elevation asin(rho.up / |rho|), the very value the mask test reads; azimuth atan2(rho.E, rho.N) mapped into
+// [0, 360) (anise's atan2(rho_SEZ.y, -rho_SEZ.x) and between_0_360), with E and N the geodetic east and north.  Their h_tilde rows are
+// the reference's as coded: in rad/km, from the integration-frame rho, with r^2 = |rho|^2 formed as (sqrt(sum))^2.
+template <bool SUB_BIAS = true, class St>
+__device__ static int od_window_setup(const DevSetup& S, const St& gs, int M, int wno, const double o[St::NS], long long t_k,
+                                      const double y[9], OdWindowT<St::NS>& w) {
+    constexpr int NS = St::NS;
     w.ncur = 0;
     for (int q = wno * M; q < (wno + 1) * M && q < gs.n_types; ++q) w.cur[w.ncur++] = gs.types[q];
     if (w.ncur == 0) return OD_WIN_EMPTY;
     bool any = false;
-    w.avail[0] = w.avail[1] = false;
+#pragma unroll
+    for (int q = 0; q < NS; ++q) w.avail[q] = false;
     for (int q = 0; q < w.ncur; ++q) { w.avail[q] = (o[w.cur[q]] == o[w.cur[q]]); any = any || w.avail[q]; }
     if (!any) return OD_WIN_UNAVAILABLE;
-    w.real_obs[0] = w.real_obs[1] = 0.0;
+#pragma unroll
+    for (int q = 0; q < NS; ++q) w.real_obs[q] = 0.0;
     for (int q = 0; q < w.ncur; ++q) if (w.avail[q]) w.real_obs[q] = o[w.cur[q]];
-    double r_tx[3], v_tx[3], up[3];
-    if (!station_state(S, gs, t_k, r_tx, v_tx, up)) return OD_WIN_EPHEMERIS;
+    double r_tx[3], v_tx[3], up[3], ne[2][3];
+    if (!station_state(S, gs, t_k, r_tx, v_tx, up, ne)) return OD_WIN_EPHEMERIS;
     const double dr[3] = { y[0] - r_tx[0], y[1] - r_tx[1], y[2] - r_tx[2] };
     const double dv[3] = { y[3] - v_tx[0], y[4] - v_tx[1], y[5] - v_tx[2] };
     const double rng = sqrt((dr[0] * dr[0] + dr[1] * dr[1]) + dr[2] * dr[2]);
@@ -275,22 +289,48 @@ __device__ static int od_window_setup(const DevSetup& S, const DevStation& gs, i
         if (tau >= 0.0 && tau <= 1.0 && (1.0 - tau) * r1sq + r12 * tau <= gs.body_radius * gs.body_radius) visible = false;
     }
     if (!visible) return OD_WIN_NOT_VISIBLE;   // device.measure() -> None (process/mod.rs:386-392)
-    for (int q = 0; q < 2; ++q)
+#pragma unroll
+    for (int q = 0; q < NS; ++q)
+#pragma unroll
         for (int c = 0; c < 9; ++c) w.H[q][c] = (q == c) ? 1.0 : 0.0;
-    w.Rk[0] = w.Rk[1] = 0.0; w.comp[0] = w.comp[1] = 0.0;
+#pragma unroll
+    for (int q = 0; q < NS; ++q) { w.Rk[q] = 0.0; w.comp[q] = 0.0; }
     for (int q = 0; q < w.ncur; ++q) {
         const int slot = wno * M + q;  // position of the type in the device's list
+        const int t = w.cur[q];
         w.Rk[q] = gs.noise_var[slot];
-        w.comp[q] = ((w.cur[q] == NYXB_MSR_RANGE) ? rng : rr);
+        w.comp[q] = ((t == NYXB_MSR_RANGE) ? rng : rr);
+        if constexpr (NS == 4) {
+            if (t == NYXB_MSR_ELEVATION) w.comp[q] = elev;
+            if (t == NYXB_MSR_AZIMUTH) {
+                const double rn = (dr[0] * ne[0][0] + dr[1] * ne[0][1]) + dr[2] * ne[0][2];
+                const double re = (dr[0] * ne[1][0] + dr[1] * ne[1][1]) + dr[2] * ne[1][2];
+                double az = fmod(atan2(re, rn) * (180.0 / 3.14159265358979323846), 360.0);
+                if (az < 0.0) az += 360.0;
+                w.comp[q] = az;
+            }
+        }
         if (SUB_BIAS) w.comp[q] -= gs.bias[slot];
         if (!w.avail[q]) continue;
-        if (w.cur[q] == NYXB_MSR_DOPPLER) {
+        if (t == NYXB_MSR_DOPPLER) {
             const double rho = rng, rho_dot = o[NYXB_MSR_DOPPLER], rho2 = rho * rho;
             w.H[q][0] = dv[0] / rho - rho_dot * dr[0] / rho2;
             w.H[q][1] = dv[1] / rho - rho_dot * dr[1] / rho2;
             w.H[q][2] = dv[2] / rho - rho_dot * dr[2] / rho2;
             w.H[q][3] = dr[0] / rho; w.H[q][4] = dr[1] / rho; w.H[q][5] = dr[2] / rho;
             w.H[q][6] = 0.0; w.H[q][7] = 0.0; w.H[q][8] = 0.0;
+        } else if (NS == 4 && (t == NYXB_MSR_AZIMUTH || t == NYXB_MSR_ELEVATION)) {
+            const double xy2 = dr[0] * dr[0] + dr[1] * dr[1];
+            for (int c = 0; c < 9; ++c) w.H[q][c] = 0.0;
+            if (t == NYXB_MSR_AZIMUTH) {
+                w.H[q][0] = -dr[1] / xy2;
+                w.H[q][1] = dr[0] / xy2;
+            } else {
+                const double nrm = sqrt(xy2 + dr[2] * dr[2]), r2 = nrm * nrm, z2 = dr[2] * dr[2];
+                w.H[q][0] = -(dr[0] * dr[2]) / (r2 * sqrt(r2 - z2));
+                w.H[q][1] = -(dr[1] * dr[2]) / (r2 * sqrt(r2 - z2));
+                w.H[q][2] = sqrt(xy2) / r2;
+            }
         } else {
             const double rho = o[NYXB_MSR_RANGE];
             w.H[q][0] = dr[0] / rho; w.H[q][1] = dr[1] / rho; w.H[q][2] = dr[2] / rho;
@@ -334,13 +374,14 @@ __device__ static bool od_sinv(int M, const double Sk[2][2], double Si[2][2]) {
 
 // ------------------------------------------------------------------------- tracker kinds of the filter loop (od_process_arc's TRK)
 // TRK::NS      observation slots per measurement: obs, ratio, prefit and postfit are [m][NS][n], and slot wno*M + q is the position of
-//              the window's type in the device's list (the ratio takes slot wno when M == 1, else 0);
+//              the window's type in the device's list (the ratio takes slot ratio_slot(M, wno));
 // TRK::Dev     the device struct of DevOdT;
 // absent(o)    no type of the measurement is in this filter's arc;
 // setup(..)    the window (od_window_setup's contract);
 // ratio(..)    residual ratio of filtering.rs:152-167, false on SingularNoiseRk;
 // gain_setup / gain_entry   K = P H^T S^-1 (filtering.rs:206-231): gain_setup factors S (false on SingularKalmanGain), gain_entry gives
 //              entry q of row r of K from row r of P H^T;
+// ratio_slot   the ratio's slot of window wno;
 // tag(..)      the estimate record's tag, and tag_msr / tag_window its measurement index and window.
 struct GroundTrk {
     using Dev = DevStation;
@@ -362,6 +403,7 @@ struct GroundTrk {
             for (int bb = 0; bb < M; ++bb) s += pht[bb] * g.Si[bb][q];
         return s;
     }
+    __device__ __forceinline__ static int ratio_slot(int M, int wno) { return (M == 1) ? wno : 0; }
     __device__ __forceinline__ static long long tag(long long k, int wno, int rej, int M) { return ((k * 2 + wno) * 2 + rej) * 2 + (M - 1); }
     __device__ __forceinline__ static long long tag_msr(long long tg) { return tg >> 3; }
     __device__ __forceinline__ static int tag_window(long long tg) { return (int)((tg >> 2) & 1); }
@@ -493,7 +535,37 @@ struct PosTrk {
             for (int bb = 0; bb < M; ++bb) s += pht[bb] * g.Si[bb][q];
         return s;
     }
+    __device__ __forceinline__ static int ratio_slot(int M, int wno) { return (M == 1) ? wno : 0; }
     __device__ __forceinline__ static long long tag(long long k, int wno, int rej, int M) { return ((k * 4 + wno) * 2 + rej) * 4 + (M - 1); }
     __device__ __forceinline__ static long long tag_msr(long long tg) { return tg >> 5; }
     __device__ __forceinline__ static int tag_window(long long tg) { return (int)((tg >> 3) & 3); }
+};
+
+// A ground station with angles (DevAerStation): the window of od_window_setup over four slots, msr_size 1 or 2.  Ratio and gain are the
+// ground station's (od_ratio, od_sinv) on the leading 2x2 block.  The ratio takes slot wno: four types at msr_size 2 make two windows.
+// Record tags use the position filter's layout (window 0..3).
+struct AerTrk {
+    using Dev = DevAerStation;
+    static constexpr int NS = Dev::NS;
+    using Win = OdWindowT<4>;
+    using Gain = GroundTrk::Gain;
+    __device__ __forceinline__ static bool absent(const double o[4]) { return o[0] != o[0] && o[1] != o[1] && o[2] != o[2] && o[3] != o[3]; }
+    __device__ __forceinline__ static int setup(const DevSetup& S, const Dev& gs, int M, int wno, const double o[4], long long t_k, const double y[9],
+                                Win& w) {
+        return od_window_setup(S, gs, M, wno, o, t_k, y, w);
+    }
+    __device__ __forceinline__ static bool ratio(int M, const double Sk[4][4], const double Rk[4], const double pre[4], double& r) {
+        const double S2[2][2] = { { Sk[0][0], Sk[0][1] }, { Sk[1][0], Sk[1][1] } };
+        const double R2[2] = { Rk[0], Rk[1] }, p2[2] = { pre[0], pre[1] };
+        return od_ratio(M, S2, R2, p2, r);
+    }
+    __device__ __forceinline__ static bool gain_setup(int M, const double Sk[4][4], Gain& g) {
+        const double S2[2][2] = { { Sk[0][0], Sk[0][1] }, { Sk[1][0], Sk[1][1] } };
+        return od_sinv(M, S2, g.Si);
+    }
+    __device__ __forceinline__ static double gain_entry(int M, const Gain& g, const double* pht, int q) { return GroundTrk::gain_entry(M, g, pht, q); }
+    __device__ __forceinline__ static int ratio_slot(int, int wno) { return wno; }
+    __device__ __forceinline__ static long long tag(long long k, int wno, int rej, int M) { return PosTrk::tag(k, wno, rej, M); }
+    __device__ __forceinline__ static long long tag_msr(long long tg) { return PosTrk::tag_msr(tg); }
+    __device__ __forceinline__ static int tag_window(long long tg) { return PosTrk::tag_window(tg); }
 };

@@ -8,11 +8,12 @@
 // bias subtracted) at estimate k's epoch with the measurement of record k+1.
 //
 // Built once, STRICT and without FMA contraction, like the host API: the 9x9 part is then bit-identical to its host build.  The same
-// kernel template serves the ground station's records (nyxb_k_smooth<GroundTrk>) and those of position fixes (nyxb_k_smooth<PosTrk>).
+// kernel template serves the ground station's records (nyxb_k_smooth<GroundTrk>), those of position fixes (nyxb_k_smooth<PosTrk>) and
+// those of stations with angles (nyxb_k_smooth<AerTrk>).
 #include "nyxb_od_device.cuh"
 #include "nyxb_smooth.h"
 
-// TRK: the tracker kind of the filter that wrote the records (GroundTrk, PosTrk; nyxb_od_device.cuh)
+// TRK: the tracker kind of the filter that wrote the records (GroundTrk, PosTrk, AerTrk; nyxb_od_device.cuh)
 template <class TRK>
 __device__ __forceinline__ void smooth_one(const DevSetup& S, const DevSmoothT<typename TRK::Dev>& sm, size_t n) {
     constexpr int NS = TRK::NS;
@@ -125,3 +126,4 @@ cudaError_t nyxb_smooth_launch(const DevSetup& S, const DevSmoothT<Dev>& sm, siz
 
 template cudaError_t nyxb_smooth_launch(const DevSetup&, const DevSmoothT<DevStation>&, size_t, cudaStream_t);
 template cudaError_t nyxb_smooth_launch(const DevSetup&, const DevSmoothT<DevPosDevice>&, size_t, cudaStream_t);
+template cudaError_t nyxb_smooth_launch(const DevSetup&, const DevSmoothT<DevAerStation>&, size_t, cudaStream_t);

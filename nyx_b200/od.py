@@ -38,12 +38,17 @@ from .frames import IAU_EARTH_FRAME, NS_PER_S, Almanac, Frame
 class MeasurementType(enum.IntEnum):
     Range = abi.MSR_RANGE
     Doppler = abi.MSR_DOPPLER
+    Azimuth = abi.MSR_AZIMUTH      # degrees, ground stations (GroundStation.with_msr_type)
+    Elevation = abi.MSR_ELEVATION
     X = abi.MSR_X          # position fixes (PositionDevice), km in the integration frame
     Y = abi.MSR_Y
     Z = abi.MSR_Z
 
 
 _POSITION_TYPES = (MeasurementType.X, MeasurementType.Y, MeasurementType.Z)
+# the observation slots of an arc for ground stations that measure angles (nyxb_od_aer_batch): slot = type
+AER_TYPES = (MeasurementType.Range, MeasurementType.Doppler, MeasurementType.Azimuth, MeasurementType.Elevation)
+_ANGLE_TYPES = (MeasurementType.Azimuth, MeasurementType.Elevation)
 
 
 class KalmanVariant(enum.IntEnum):
@@ -110,6 +115,26 @@ class GroundStation:
         return cls("Goldstone", 35.247_164, 243.205, 1.071_149_04, IAU_EARTH_FRAME, elevation_mask_deg,
                    stochastic_noises={MeasurementType.Range: range_noise_km, MeasurementType.Doppler: doppler_noise_km_s})
 
+    def with_msr_type(self, msr_type: MeasurementType, noise: StochasticNoise) -> "GroundStation":
+        """`GroundStation::with_msr_type` (ground_station/mod.rs:137-150): sets the type's noise and appends the type to the list
+        unless it is there already."""
+        msr_type = MeasurementType(msr_type)
+        self.stochastic_noises = {**self.stochastic_noises, msr_type: noise}
+        if msr_type not in self.measurement_types:
+            self.measurement_types = [*self.measurement_types, msr_type]
+        return self
+
+    @property
+    def has_angles(self) -> bool:
+        return any(t in _ANGLE_TYPES for t in self.measurement_types)
+
+    def north_east_fixed(self):
+        """Unit geodetic north and east in the body-fixed frame (the S and E axes of the SEZ frame, Vallado's RAZEL)."""
+        lat, lon = math.radians(self.latitude_deg), math.radians(self.longitude_deg)
+        north = np.array([-math.sin(lat) * math.cos(lon), -math.sin(lat) * math.sin(lon), math.cos(lat)])
+        east = np.array([-math.sin(lon), math.cos(lon), 0.0])
+        return north, east
+
     def body_fixed(self):
         """Geodetic (lat, long, height) -> body-fixed Cartesian position and local zenith on the frame's ellipsoid
         (anise `Orbit::try_latlongalt`; sphere when the frame has no polar radius)."""
@@ -130,7 +155,23 @@ class GroundStation:
         types = list(self.measurement_types)
         if not 1 <= len(types) <= 2 or len(set(types)) != len(types):
             raise ODError("a ground station carries one or two of {Range, Doppler}")
-        g = abi.GroundStationC()
+        return self._fill_c(abi.GroundStationC(), types, integration_frame, almanac)
+
+    def to_aer_c(self, integration_frame: Frame, almanac: Optional[Almanac]) -> abi.AerStationC:
+        """The station for nyxb_od_aer_batch: one to four distinct types of Range, Doppler, Azimuth and Elevation."""
+        if self.integration_time is not None or self.light_time_correction:
+            raise ODError("only instantaneous measurements without light-time correction are supported on the GPU path")
+        types = list(self.measurement_types)
+        if not 1 <= len(types) <= 4 or len(set(types)) != len(types) or any(t not in AER_TYPES for t in types):
+            raise ODError("a ground station carries one to four distinct types of {Range, Doppler, Azimuth, Elevation}")
+        g = self._fill_c(abi.AerStationC(), types, integration_frame, almanac)
+        north, east = self.north_east_fixed()
+        for i in range(3):
+            g.north_fixed[i] = north[i]
+            g.east_fixed[i] = east[i]
+        return g
+
+    def _fill_c(self, g, types, integration_frame: Frame, almanac: Optional[Almanac]):
         pos, up = self.body_fixed()
         for i in range(3):
             g.pos_fixed_km[i] = pos[i]
@@ -189,8 +230,9 @@ class PositionDevice:
 @dataclass
 class TrackingDataArc:
     """One tracking schedule (epochs + tracker names) with `n` observation sets: obs[k][type][i], NaN = type not in
-    the measurement's data (both NaN: measurement k absent from arc i).  `types` names the observation slots: (Range, Doppler), or
-    (X, Y, Z) for position fixes, whose obs is [m][3][n] (all three NaN: absent)."""
+    the measurement's data (both NaN: measurement k absent from arc i).  `types` names the observation slots: (Range, Doppler),
+    (X, Y, Z) for position fixes, whose obs is [m][3][n] (all three NaN: absent), or AER_TYPES (Range, Doppler, Azimuth, Elevation)
+    for ground stations with angles, whose obs is [m][4][n]."""
 
     epoch_ns: np.ndarray            # [m] int64 ascending
     tracker: List[str]              # [m]
@@ -201,6 +243,10 @@ class TrackingDataArc:
     def is_position(self) -> bool:
         return tuple(self.types) == _POSITION_TYPES
 
+    @property
+    def is_aer(self) -> bool:
+        return tuple(self.types) == AER_TYPES
+
     def __post_init__(self):
         self.epoch_ns = np.ascontiguousarray(self.epoch_ns, dtype=np.int64)
         self.obs = np.ascontiguousarray(self.obs, dtype=np.float64)
@@ -208,9 +254,12 @@ class TrackingDataArc:
         m = self.epoch_ns.shape[0]
         if self.obs.ndim == 2:
             self.obs = np.ascontiguousarray(self.obs[:, :, None])
-        if self.types not in ((MeasurementType.Range, MeasurementType.Doppler), _POSITION_TYPES):
-            raise ODError("types must be (Range, Doppler) or (X, Y, Z)")
-        if self.is_position:
+        if self.types not in ((MeasurementType.Range, MeasurementType.Doppler), _POSITION_TYPES, AER_TYPES):
+            raise ODError("types must be (Range, Doppler), (X, Y, Z) or (Range, Doppler, Azimuth, Elevation)")
+        if self.is_aer:
+            if len(self.tracker) != m or self.obs.shape[0] != m or self.obs.shape[1] != 4:
+                raise ODError("expected epoch_ns[m], tracker[m], obs[m][4][n]")
+        elif self.is_position:
             if len(self.tracker) != m or self.obs.shape[0] != m or self.obs.shape[1] != 3:
                 raise ODError("expected epoch_ns[m], tracker[m], obs[m][3][n]")
         elif len(self.tracker) != m or self.obs.shape[0] != m or self.obs.shape[1] != 2:
@@ -228,6 +277,7 @@ class TrackingDataArc:
     # ---- parquet I/O in the reference's layout (od/msr/trackingdata/io_parquet.rs:43-354): one arc per file
     _COLUMNS = ("Range (km)", "Doppler (km/s)")   # MeasurementType::to_field names (od/msr/types.rs)
     _POS_COLUMNS = ("X (km)", "Y (km)", "Z (km)")
+    _AER_COLUMNS = ("Range (km)", "Doppler (km/s)", "Azimuth (deg)", "Elevation (deg)")
 
     def to_parquet(self, path, index: int = 0, metadata: Optional[dict] = None):
         """`TrackingDataArc::to_parquet` for the observation set `index`: "Epoch (UTC)", "Tracking device" and one nullable
@@ -244,7 +294,7 @@ class TrackingDataArc:
         cols = [pa.array(epochs_to_utc_iso(self.epoch_ns[present]), type=pa.string()),
                 pa.array([t for t, p in zip(self.tracker, present) if p], type=pa.string())]
         fields = [pa.field("Epoch (UTC)", pa.string(), nullable=False), pa.field("Tracking device", pa.string(), nullable=False)]
-        for c, name in enumerate(self._POS_COLUMNS if self.is_position else self._COLUMNS):
+        for c, name in enumerate(self._POS_COLUMNS if self.is_position else self._AER_COLUMNS if self.is_aer else self._COLUMNS):
             v = o[present, c]
             if np.isnan(v).all():
                 continue   # unique_types(): a type no measurement carries has no column
@@ -256,25 +306,38 @@ class TrackingDataArc:
         return path
 
     @classmethod
-    def from_parquet(cls, path) -> "TrackingDataArc":
+    def from_parquet(cls, path, types=None) -> "TrackingDataArc":
         """`TrackingDataArc::from_parquet` (io_parquet.rs:43-213): needs "Epoch (UTC)", "Tracking device" and at least one of
         the measurement columns this path knows: range / Doppler, or X / Y / Z (an arc of types (X, Y, Z)), not both kinds; rows are
-        sorted by epoch."""
+        sorted by epoch.  `types=AER_TYPES` reads range, Doppler, "Azimuth (deg)" and "Elevation (deg)" into an arc of those four
+        types instead."""
         import pyarrow.parquet as pq
-
-        from .cosmic import utc_iso_to_epochs
 
         tab = pq.read_table(str(path))
         names = set(tab.column_names)
         for need in ("Epoch (UTC)", "Tracking device"):
             if need not in names:
                 raise ODError(f"MissingData: {need}")
+        if types is not None:
+            if tuple(MeasurementType(t) for t in types) != AER_TYPES:
+                raise ODError("from_parquet reads types=None or types=AER_TYPES")
+            if names & set(cls._POS_COLUMNS):
+                raise ODError("X / Y / Z columns in an arc of ground-station types")
+            if not names & set(cls._AER_COLUMNS):
+                raise ODError("MissingData: `Range (km)`, `Doppler (km/s)`, `Azimuth (deg)` or `Elevation (deg)`")
+            return cls._read_columns(tab, names, cls._AER_COLUMNS, AER_TYPES)
         ground, pos = bool(names & set(cls._COLUMNS)), bool(names & set(cls._POS_COLUMNS))
         if ground and pos:
             raise ODError("range / Doppler and X / Y / Z columns in one arc: one tracker kind per arc")
         if not ground and not pos:
             raise ODError("MissingData: `Range (km)`, `Doppler (km/s)` or `X (km)`, `Y (km)`, `Z (km)`")
-        columns = cls._POS_COLUMNS if pos else cls._COLUMNS
+        types = _POSITION_TYPES if pos else (MeasurementType.Range, MeasurementType.Doppler)
+        return cls._read_columns(tab, names, cls._POS_COLUMNS if pos else cls._COLUMNS, types)
+
+    @classmethod
+    def _read_columns(cls, tab, names, columns, types) -> "TrackingDataArc":
+        from .cosmic import utc_iso_to_epochs
+
         ep = utc_iso_to_epochs(tab["Epoch (UTC)"].to_pylist())
         obs = np.full((len(ep), len(columns)), np.nan)
         for c, name in enumerate(columns):
@@ -282,7 +345,6 @@ class TrackingDataArc:
                 obs[:, c] = [np.nan if v is None else v for v in tab[name].to_pylist()]
         order = np.argsort(ep, kind="stable")
         trk = tab["Tracking device"].to_pylist()
-        types = _POSITION_TYPES if pos else (MeasurementType.Range, MeasurementType.Doppler)
         return cls(ep[order], [trk[i] for i in order], obs[order][:, :, None], types)
 
     def filter_by_offset(self, start_ns: Optional[int] = None, end_ns: Optional[int] = None) -> "TrackingDataArc":
@@ -592,16 +654,25 @@ class ODSolution:
     def _is_position(self) -> bool:
         return self.arc is not None and self.arc.is_position
 
+    def _is_aer(self) -> bool:
+        return self.arc is not None and self.arc.is_aer
+
     def _tag_fields(self, tag):
-        """(measurement, window, rejected, msr_size) of a record tag, in the layout of the run's tracker kind (NYXB_OD_TAG or
-        NYXB_OD_POS_TAG)."""
-        return abi.od_pos_tag_fields(tag) if self._is_position() else abi.od_tag_fields(tag)
+        """(measurement, window, rejected, msr_size) of a record tag, in the layout of the run's tracker kind (NYXB_OD_TAG, or
+        NYXB_OD_POS_TAG for position fixes and stations with angles)."""
+        return abi.od_pos_tag_fields(tag) if self._is_position() or self._is_aer() else abi.od_tag_fields(tag)
+
+    def _ratio_slot(self, w: int, M: int) -> int:
+        """The slot of window w's residual ratio: w for stations with angles, else w at msr_size 1 and 0 otherwise."""
+        return w if (M == 1 or self._is_aer()) else 0
 
     def _residual_types(self):
-        """(type, unit) of the residual columns: Range / Doppler, or X / Y / Z for position fixes."""
+        """(type, unit) of the residual columns: Range / Doppler (and Azimuth / Elevation for stations with angles), or X / Y / Z for
+        position fixes."""
         if self._is_position():
             return [(t, "km") for t in _POSITION_TYPES]
-        return [(MeasurementType.Range, "km"), (MeasurementType.Doppler, "km/s")]
+        rd = [(MeasurementType.Range, "km"), (MeasurementType.Doppler, "km/s")]
+        return rd + [(MeasurementType.Azimuth, "deg"), (MeasurementType.Elevation, "deg")] if self._is_aer() else rd
 
     def _need_records(self):
         if self.records is None:
@@ -665,7 +736,7 @@ class ODSolution:
                     continue
             else:
                 post = filt_post[mk, slots, i]
-            out.append((self.prefit[mk, slots, i].copy(), np.array(post), float(self.resid_ratio[mk, w if M == 1 else 0, i]), bool(rej)))
+            out.append((self.prefit[mk, slots, i].copy(), np.array(post), float(self.resid_ratio[mk, self._ratio_slot(w, M), i]), bool(rej)))
         return out
 
     def _rms(self, i, f):
@@ -711,6 +782,10 @@ class ODSolution:
             names, dev_c = odp.position_devices_c()
             tracker = np.array([names.index(t) if t in names else -1 for t in self.arc.tracker], dtype=np.int32)
             sm = eng.od_position_smooth_batch(odp.config_c(), len(names), dev_c, tracker, self.arc.obs, rec, self.status)
+        elif self.arc.is_aer:
+            names, st_c = odp.aer_stations_c(frame)
+            tracker = np.array([names.index(t) if t in names else -1 for t in self.arc.tracker], dtype=np.int32)
+            sm = eng.od_aer_smooth_batch(odp.config_c(), len(names), st_c, tracker, self.arc.obs, rec, self.status)
         else:
             names, st_c = odp.stations_c(frame)
             tracker = np.array([names.index(t) if t in names else -1 for t in self.arc.tracker], dtype=np.int32)
@@ -936,12 +1011,20 @@ class KalmanODProcess:
             arr[i] = self.devices[nme].to_c(frame, self.almanac)
         return names, arr
 
+    def aer_stations_c(self, frame: Frame):
+        names = list(self.devices)
+        arr = (abi.AerStationC * max(len(names), 1))()
+        for i, nme in enumerate(names):
+            arr[i] = self.devices[nme].to_aer_c(frame, self.almanac)
+        return names, arr
+
     def process_arcs(self, initial_estimates: Sequence[KfEstimate], arc: TrackingDataArc, record_estimates: bool = False,
                      estimates_capacity: Optional[int] = None) -> ODSolution:
         """n independent `process_arc(initial_estimate_i, arc_i)` runs (od/process/mod.rs:128-497) in one launch.  With
         `estimates_capacity` K, the first K entries of each filter's ODSolution.estimates are recorded (1 456 bytes each), which
         `ODSolution.smooth()`, `residuals`, the RMS statistics and the per-estimate parquet export need; the filter's results do not
-        change."""
+        change.  Ground stations run through nyxb_od_aer_batch exactly when the arc's types are AER_TYPES (range, Doppler, azimuth,
+        elevation); stations that measure angles need such an arc."""
         n = len(initial_estimates)
         if arc.n != n:
             raise ODError(f"arc carries {arc.n} observation sets for {n} filters")
@@ -967,11 +1050,19 @@ class KalmanODProcess:
                 raise ODError("msr_size 3 needs position devices")
             if arc.is_position:
                 raise ODError("ground stations need a tracking arc of types (Range, Doppler)")
-            names, st_c = self.stations_c(frame)
-            tracker = np.array([names.index(t) if t in names else -1 for t in arc.tracker], dtype=np.int32)
-            rec_kw = {} if estimates_capacity is None else {"estimates_capacity": estimates_capacity}
-            res = eng.od_ekf_batch(self.config_c(), len(names), st_c, arc.epoch_ns, tracker, arc.obs, st, cs, ep, cov0,
-                                   record_estimates=record_estimates, **rec_kw)
+            if arc.is_aer:
+                names, st_c = self.aer_stations_c(frame)
+                tracker = np.array([names.index(t) if t in names else -1 for t in arc.tracker], dtype=np.int32)
+                res = eng.od_aer_batch(self.config_c(), len(names), st_c, arc.epoch_ns, tracker, arc.obs, st, cs, ep, cov0,
+                                       record_estimates=record_estimates, estimates_capacity=estimates_capacity)
+            else:
+                if any(d.has_angles for d in self.devices.values()):
+                    raise ODError("stations that measure azimuth or elevation need a tracking arc of types AER_TYPES")
+                names, st_c = self.stations_c(frame)
+                tracker = np.array([names.index(t) if t in names else -1 for t in arc.tracker], dtype=np.int32)
+                rec_kw = {} if estimates_capacity is None else {"estimates_capacity": estimates_capacity}
+                res = eng.od_ekf_batch(self.config_c(), len(names), st_c, arc.epoch_ns, tracker, arc.obs, st, cs, ep, cov0,
+                                       record_estimates=record_estimates, **rec_kw)
         res.templates = [e.nominal_state for e in initial_estimates]
         res.arc = arc
         res.devices = self.devices
@@ -1112,6 +1203,8 @@ class BatchLeastSquares:
                  lm_lambda_min: float = 1e-12, lm_lambda_max: float = 1e12, lm_use_diag_scaling: bool = True):
         if any(isinstance(d, PositionDevice) for d in devices.values()):
             raise ODError("batch least squares takes ground stations only")
+        if any(d.has_angles for d in devices.values()):
+            raise ODError("batch least squares takes range and Doppler only, not azimuth or elevation")
         self.prop = prop
         self.devices = dict(devices)
         self.almanac = almanac
@@ -1147,6 +1240,8 @@ class BatchLeastSquares:
             raise ODError("no initial guess")
         if arc.n != n:
             raise ODError(f"arc carries {arc.n} observation sets for {n} problems")
+        if arc.is_aer:
+            raise ODError("batch least squares takes arcs of types (Range, Doppler), not AER_TYPES")
         frame = guesses[0].orbit.frame
         st, cs, ep = pack_spacecraft(guesses)
         eng = self.prop.engine(frame, self.almanac)
@@ -1218,10 +1313,13 @@ def station_state(gs: GroundStation, t_ns: int, integration_frame: Frame, almana
 def simulate_tracking(truth_epochs_ns, truth_states, devices: Dict[str, GroundStation], schedule: Sequence[str], frame: Frame,
                       almanac: Optional[Almanac], rng: Optional[np.random.Generator] = None) -> TrackingDataArc:
     """Synthetic range / Doppler observations of `truth_states[k]` ([m][6][n]) at `truth_epochs_ns[k]` from tracker
-    `schedule[k]`; white noise of each station's sigma when `rng` is given.  Invisible passes are NaN (absent)."""
+    `schedule[k]`; white noise of each station's sigma when `rng` is given.  Invisible passes are NaN (absent).  When a station
+    carries azimuth or elevation the arc has types AER_TYPES (obs [m][4][n]) and the angles, in degrees, are those of
+    nyxb_aer_station (azimuth in [0, 360) before noise)."""
     truth_states = np.asarray(truth_states, dtype=np.float64)
     m, _, n = truth_states.shape
-    obs = np.full((m, 2, n), np.nan)
+    aer = any(gs.has_angles for gs in devices.values())
+    obs = np.full((m, 4 if aer else 2, n), np.nan)
     for k in range(m):
         gs = devices[schedule[k]]
         r_tx, v_tx, up_in = station_state(gs, int(truth_epochs_ns[k]), frame, almanac)
@@ -1230,6 +1328,10 @@ def simulate_tracking(truth_epochs_ns, truth_states, devices: Dict[str, GroundSt
         rng_km = np.linalg.norm(rho, axis=0)
         rr = (rho * dv).sum(0) / rng_km
         elev = np.degrees(np.arcsin((rho * up_in[:, None]).sum(0) / rng_km))
+        if aer:
+            R = _rotation_matrix(gs.frame.rotation, int(truth_epochs_ns[k]))
+            north, east = (R.T @ u for u in gs.north_east_fixed())
+            az = np.mod(np.degrees(np.arctan2((rho * east[:, None]).sum(0), (rho * north[:, None]).sum(0))), 360.0)
         vis = elev >= gs.elevation_mask_deg
         if gs.frame.ephemeris_id != frame.ephemeris_id:
             # line of sight blocked by the body the spacecraft orbits (Vallado's SIGHT)
@@ -1239,10 +1341,13 @@ def simulate_tracking(truth_epochs_ns, truth_states, devices: Dict[str, GroundSt
             blocked = (tau >= 0.0) & (tau <= 1.0) & ((1.0 - tau) * r1sq + r12 * tau <= frame.mean_equatorial_radius_km() ** 2)
             vis &= ~blocked
         for t in gs.measurement_types:
-            val = rng_km if t == MeasurementType.Range else rr
+            val = {MeasurementType.Range: rng_km, MeasurementType.Doppler: rr}.get(t)
+            if val is None:
+                val = az if t == MeasurementType.Azimuth else elev
             noise = rng.normal(0.0, gs.stochastic_noises[t].sigma, n) if rng is not None else 0.0
             obs[k, int(t), :] = np.where(vis, val + noise, np.nan)
-    return TrackingDataArc(np.asarray(truth_epochs_ns, dtype=np.int64), list(schedule), obs)
+    return TrackingDataArc(np.asarray(truth_epochs_ns, dtype=np.int64), list(schedule), obs,
+                           AER_TYPES if aer else (MeasurementType.Range, MeasurementType.Doppler))
 
 
 def simulate_position_fixes(truth_epochs_ns, truth_states, devices: Dict[str, PositionDevice], schedule: Sequence[str],

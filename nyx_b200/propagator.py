@@ -418,6 +418,18 @@ class Engine:
         in ONE launch; per-measurement outputs [m][3][n].  `record_estimates`: the estimated state and covariance diagonal after each
         measurement, as od_ekf_batch.  With `estimates_capacity` K the first K estimates of each filter are recorded (tags
         NYXB_OD_POS_TAG); the filter's results are the same bits."""
+        return self._od_slots_batch("nyxb_od_position_batch", abi.PositionArcC, 3, cfg_c, n_devices, devices_c, msr_epoch_ns, msr_tracker,
+                                    obs, state_soa, consts_soa, epoch0_ns, covar0_soa, record_estimates, estimates_capacity)
+
+    def od_aer_batch(self, cfg_c, n_stations, stations_c, msr_epoch_ns, msr_tracker, obs, state_soa, consts_soa, epoch0_ns,
+                     covar0_soa, record_estimates: bool = False, estimates_capacity: Optional[int] = None):
+        """`nyxb_od_aer_batch`: od_position_batch's contract for ground stations with angles (nyxb_aer_station): obs [m][4][n], slot =
+        type (Range, Doppler, Azimuth, Elevation); per-measurement outputs [m][4][n], the ratio of window w in slot w."""
+        return self._od_slots_batch("nyxb_od_aer_batch", abi.TrackingArcC, 4, cfg_c, n_stations, stations_c, msr_epoch_ns, msr_tracker,
+                                    obs, state_soa, consts_soa, epoch0_ns, covar0_soa, record_estimates, estimates_capacity)
+
+    def _od_slots_batch(self, fn, arc_cls, ns, cfg_c, n_devices, devices_c, msr_epoch_ns, msr_tracker, obs, state_soa, consts_soa,
+                        epoch0_ns, covar0_soa, record_estimates, estimates_capacity):
         from .od import ODSolution
 
         state_soa = np.ascontiguousarray(state_soa, dtype=np.float64)
@@ -431,11 +443,11 @@ class Engine:
         m = msr_epoch_ns.shape[0]
         if state_soa.shape != (9, n) or consts_soa.shape != (4, n) or epoch0_ns.shape != (n,) or covar0_soa.shape != (81, n):
             raise ValueError("expected state[9][n], consts[4][n], epoch0[n], covar0[81][n]")
-        if obs.shape != (m, 3, n) or msr_tracker.shape != (m,):
-            raise ValueError("expected obs[m][3][n], tracker[m]")
-        arc = abi.PositionArcC(m, msr_epoch_ns.ctypes.data, msr_tracker.ctypes.data, obs.ctypes.data)
+        if obs.shape != (m, ns, n) or msr_tracker.shape != (m,):
+            raise ValueError(f"expected obs[m][{ns}][n], tracker[m]")
+        arc = arc_cls(m, msr_epoch_ns.ctypes.data, msr_tracker.ctypes.data, obs.ctypes.data)
         out_state = np.empty((9, n)); out_epoch = np.empty(n, dtype=np.int64); out_cov = np.empty((81, n)); out_dev = np.empty((9, n))
-        ratio = np.full((m, 3, n), np.nan); prefit = np.full((m, 3, n), np.nan); postfit = np.full((m, 3, n), np.nan)
+        ratio = np.full((m, ns, n), np.nan); prefit = np.full((m, ns, n), np.nan); postfit = np.full((m, ns, n), np.nan)
         flags = np.zeros((m, n), dtype=np.int32)
         est_state = np.full((m, 9, n), np.nan) if record_estimates else None
         est_cov = np.full((m, 9, n), np.nan) if record_estimates else None
@@ -449,36 +461,44 @@ class Engine:
         if estimates_capacity is not None:
             records, rec_c = _od_records(int(estimates_capacity), n)
             rec_p = C.byref(rec_c)
-        rc = self._lib.nyxb_od_position_batch(self._h, C.byref(cfg_c), int(n_devices), devices_c, C.byref(arc), n,
-                                              state_soa.ctypes.data, consts_soa.ctypes.data, epoch0_ns.ctypes.data,
-                                              covar0_soa.ctypes.data, C.byref(out), rec_p)
+        rc = getattr(self._lib, fn)(self._h, C.byref(cfg_c), int(n_devices), devices_c, C.byref(arc), n, state_soa.ctypes.data,
+                                    consts_soa.ctypes.data, epoch0_ns.ctypes.data, covar0_soa.ctypes.data, C.byref(out), rec_p)
         if rc != 0:
-            raise PropagationError(f"nyxb_od_position_batch rc={rc}: {abi.last_error()}")
+            raise PropagationError(f"{fn} rc={rc}: {abi.last_error()}")
         covar = np.ascontiguousarray(out_cov.T.reshape(n, 9, 9).transpose(0, 2, 1))
         return ODSolution(out_state, out_epoch, covar, out_dev, ratio, prefit, postfit, flags, est_state, est_cov, details, status,
                           records=records)
 
     def od_position_smooth_batch(self, cfg_c, n_devices, devices_c, msr_tracker, obs, records: dict, filter_status, outputs=None):
         """`nyxb_od_position_smooth_batch`: od_smooth_batch for the records of od_position_batch; postfit is [K][3][n]."""
+        return self._od_slots_smooth("nyxb_od_position_smooth_batch", abi.PositionArcC, 3, cfg_c, n_devices, devices_c, msr_tracker, obs,
+                                     records, filter_status, outputs)
+
+    def od_aer_smooth_batch(self, cfg_c, n_stations, stations_c, msr_tracker, obs, records: dict, filter_status, outputs=None):
+        """`nyxb_od_aer_smooth_batch`: od_smooth_batch for the records of od_aer_batch; obs [m][4][n], postfit [K][4][n]."""
+        return self._od_slots_smooth("nyxb_od_aer_smooth_batch", abi.TrackingArcC, 4, cfg_c, n_stations, stations_c, msr_tracker, obs,
+                                     records, filter_status, outputs)
+
+    def _od_slots_smooth(self, fn, arc_cls, ns, cfg_c, n_devices, devices_c, msr_tracker, obs, records, filter_status, outputs):
         msr_tracker = np.ascontiguousarray(msr_tracker, dtype=np.int32)
         obs = np.ascontiguousarray(obs, dtype=np.float64)
         filter_status = np.ascontiguousarray(filter_status, dtype=np.int32)
         cap, n = records["epoch"].shape
         m = msr_tracker.shape[0]
-        if obs.shape != (m, 3, n) or filter_status.shape != (n,):
-            raise ValueError("expected obs[m][3][n], filter_status[n]")
+        if obs.shape != (m, ns, n) or filter_status.shape != (n,):
+            raise ValueError(f"expected obs[m][{ns}][n], filter_status[n]")
         rec_c = abi.OdRecordsC(cap, *(np.ascontiguousarray(records[k]).ctypes.data for k in _REC_KEYS))
-        shapes = {"state": 9, "deviation": 9, "covar": 81, "fs_ratio": 9, "postfit": 3}
+        shapes = {"state": 9, "deviation": 9, "covar": 81, "fs_ratio": 9, "postfit": ns}
         want = shapes if outputs is None else {k: shapes[k] for k in outputs}
         r = {k: np.empty((cap, rows, n)) for k, rows in want.items()}
         r["status"] = np.zeros(n, dtype=np.int32)
         out = abi.SmoothOutputsC(*(r[k].ctypes.data if k in r else None for k in ("state", "deviation", "covar", "fs_ratio", "postfit")),
                                  r["status"].ctypes.data)
-        arc = abi.PositionArcC(m, None, msr_tracker.ctypes.data, obs.ctypes.data)
-        rc = self._lib.nyxb_od_position_smooth_batch(self._h, C.byref(cfg_c), int(n_devices), devices_c, C.byref(arc), n, C.byref(rec_c),
-                                                     filter_status.ctypes.data, C.byref(out))
+        arc = arc_cls(m, None, msr_tracker.ctypes.data, obs.ctypes.data)
+        rc = getattr(self._lib, fn)(self._h, C.byref(cfg_c), int(n_devices), devices_c, C.byref(arc), n, C.byref(rec_c),
+                                    filter_status.ctypes.data, C.byref(out))
         if rc != 0:
-            raise PropagationError(f"nyxb_od_position_smooth_batch rc={rc}: {abi.last_error()}")
+            raise PropagationError(f"{fn} rc={rc}: {abi.last_error()}")
         return r
 
     def _bls_args(self, msr_epoch_ns, msr_tracker, obs, state_soa, consts_soa, epoch0_ns):
