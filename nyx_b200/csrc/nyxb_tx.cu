@@ -12,9 +12,12 @@
 //     13 FP64 instructions per entry.
 //   * Everything that is serial per right-hand side — reduction of the partial sums, acceleration assembly, RK stage algebra,
 //     body-fixed DCM, 1/r, the (cos, sin)(m lambda) cos^m(phi) and rho^m tables, and per step the error norm, the step-size controller,
-//     recording and the stop condition — runs on three HELPER warps per set (helper j owns state components j and j+3), concurrently
-//     with the walkers, which meanwhile walk the OTHER set of the CTA: two sets alternate through the walkers (named barriers
-//     READY[set] / DONE[set]), so the FP64 pipe sees the walk of one set while the latency-bound chain of the other is hidden.
+//     recording and the stop condition — runs on two HELPER warps per set, concurrently with the walkers, which meanwhile walk the
+//     OTHER set of the CTA: two sets alternate through the walkers (named barriers READY[set] / DONE[set]), so the FP64 pipe sees
+//     the walk of one set while the latency-bound chain of the other is hidden.  Helper 0 (the lead) owns the position side (the
+//     candidate and error sums of the positions, the stage DCMs, the controller, the set queue), helper 1 the acceleration side
+//     (reduction of the partial sums, acceleration, V_{i+1}, P_{i+2}, the velocity sums).  8 walkers + 2 x 2 helpers = 12 warps:
+//     every scheduler hosts two walkers and one helper, and the register cap is 168 per thread.
 //     The first version of this kernel ran these phases on the walker warps themselves, between CTA-wide barriers, and spent much
 //     of the warp-time in barrier stalls with the FP64 pipe half idle.
 //   * Persistent CTAs, one per SM; every set context pulls (set, time-slice) tickets from a global counter: with fewer contexts than
@@ -38,7 +41,7 @@
 
 namespace {
 constexpr int NL = 32;   // trajectories per set, one per lane: stride of every per-trajectory shared-memory array
-constexpr int HW = 3;    // helper warps per set context
+constexpr int HW = 2;    // helper warps per set context: 0 = lead (position side), 1 = acceleration side
 constexpr unsigned FULL = 0xffffffffu;
 
 // ---- per-trajectory controller state kept in shared memory ([field][lane])
@@ -51,10 +54,10 @@ enum { F_FIXED = 1, F_PREVFIXED = 2, F_RETRY = 4, F_LAST = 8, F_DONE = 16, F_BAC
 //   wk   [2][WK][32]     walker inputs of a stage: ub, r2, and the powers of z = (cos, sin)(lambda) cos(phi) and rho it starts its
 //                        columns from — P = 8, 10: every z^e, e = 0..2P, and rho^e, e = 1..2P (WK = 6P + 4; the walkers only load);
 //                        P = 16: z^(2^k), rho^(2^k), k = 0..5 (WK = 20; the walkers multiply them together)   (helpers -> walkers)
-//   rn   [2][9][32]      DCM of the stage being prepared (lead helper -> all helpers)
+//   rn   [2][9][32]      DCM of the stage being prepared (lead helper -> both helpers)
 //   part [2][P][4][32]   partial sums of a stage                                                   (walkers -> helpers)
 //   as   [2][18][32]     what the helpers need to assemble that stage's acceleration later (DCM, unit vector, K0, K1, two-body factor, position)
-//   ysp  [2][3][32]      position components of a coming stage, exchanged between the three helpers
+//   ysp  [2][3][32]      position of a coming stage (acceleration helper -> both helpers)
 //   helper-private: kst [16][6][32] (k_i = (V_i, A_i)), nxt / er / ycur [6][32], controller fields
 struct TxLayout {
     unsigned blob, ctx0, ctx_stride;                                  // bytes
@@ -439,8 +442,8 @@ __device__ __noinline__ void tx_park_ctl(const DevSink& sink, const DevTxQueue& 
     if (step_io) step_io[tr] = step_ns;
 }
 
-// ---- prologue of stage q for the 32 trajectories of a set, run by the lead helper: body-fixed position, 1/r, the recursion
-// scalars the walkers need, and everything the three helpers need to assemble the acceleration of that stage later
+// ---- prologue of stage q for the 32 trajectories of a set, run by both helpers of the set: body-fixed position, 1/r, the recursion
+// scalars the walkers need, and everything the helpers need to assemble the acceleration of that stage later
 enum { AS_R = 0, AS_S = 9, AS_T, AS_U, AS_K0, AS_K1, AS_FAC, AS_P0, AS_P1, AS_P2, AS_COUNT };
 // walker inputs.  P = 8, 10 (E = 2P): WK_POW + e = Re z^e, WK_POW + E + 1 + e = Im z^e (e = 0..E), WK_POW + 2E + 1 + e = rho^e (e = 1..E);
 // P = 16: WK_POW + 3k = Re z^(2^k), + 1 = Im, + 2 = rho^(2^k)
@@ -452,17 +455,17 @@ template <int P> struct TxWk {
     static constexpr int ZR = WK_POW, ZI = WK_POW + E + 1, RH = WK_POW + 2 * E + 1;   // RH + e = rho^e
 };
 
-// Stage prologue, run by the three helpers of the context once the position of the stage (ysp) and its DCM (rn) are in shared
-// memory: each helper derives (s, t, u, rho) itself, then helper 0 publishes the scalars of the acceleration assembly (as) and
-// ub, r2; helpers 1 and 2 publish the powers the walkers start their columns from.
-template <int P>
+// Stage prologue, run by the two helpers of the context once the position of the stage (ysp) and its DCM (rn) are in shared
+// memory: each helper derives (s, t, u, rho) itself, then helper 0 publishes the scalars of the acceleration assembly (as), ub, r2
+// and the powers of rho; helper 1 publishes the powers of z the walkers start their columns from (P = 16: the z^(2^k), rho^(2^k)).
+template <int P, bool COLD>
 __device__ __forceinline__ void tx_prologue(const DevSetup& S, const TxSm& sm, int lane, int par, int j, const double* ysp, long long t_ns) {
     const DevGrav& gv = S.grav;
     const double* rn = sm.rn + par * 9 * NL + lane;
     const double p0 = ysp[lane], p1 = ysp[NL + lane], p2 = ysp[2 * NL + lane];
     double y0 = p0, y1 = p1, y2 = p2;
     double ir_c = 0.0;   // 1/|r| about the integration centre (two-body term)
-    if (S.grav_body >= 0) {   // field of another body: the state is translated to it first (gravity_field.rs:149-154)
+    if (COLD && S.grav_body >= 0) {   // field of another body: the state is translated to it first (gravity_field.rs:149-154)
         ir_c = rsqrt(fma(y2, y2, fma(y1, y1, y0 * y0)));
         field_offset(S, t_ns, y0, y1, y2);
     }
@@ -485,36 +488,8 @@ __device__ __forceinline__ void tx_prologue(const DevSetup& S, const TxSm& sm, i
         as[AS_K0 * NL] = K0; as[AS_K1 * NL] = K0 * rho;
         as[AS_FAC * NL] = -S.mu_central * ir_c * ir_c * ir_c;   // two-body (orbital.rs:86-92), from the same 1/r when the field is the centre's
         as[AS_P0 * NL] = p0; as[AS_P1 * NL] = p1; as[AS_P2 * NL] = p2;
-        if constexpr (!TxWk<P>::ALL) {   // z^(2^k), rho^(2^k): the walkers assemble z^e, rho^(e+1) of their columns from these
-            double zr = s_, zi = t_, rp = rho;
-#pragma unroll
-            for (int k = 0; k < 6; ++k) {
-                wk[(WK_POW + 3 * k) * NL] = zr; wk[(WK_POW + 3 * k + 1) * NL] = zi; wk[(WK_POW + 3 * k + 2) * NL] = rp;
-                const double nr = fma(zr, zr, -(zi * zi));
-                zi = 2.0 * zr * zi; zr = nr; rp *= rp;
-            }
-        }
-    } else if constexpr (TxWk<P>::ALL) {
-        // z^1..z^8 by doubling (z^2; z^3, z^4; z^5..z^8); helper 2 goes on to z^(8+k) = z^8 z^k, z^(16+k) = z^16 z^k; helper 1 adds
-        // the powers of rho the same way
-        constexpr int E = TxWk<P>::E;
-        static_assert(E > 8 && E <= 24, "published powers");
-        double* wr = wk + TxWk<P>::ZR * NL;
-        double* wi = wk + TxWk<P>::ZI * NL;
-        double zr[9], zi[9];
-        zr[1] = s_; zi[1] = t_;
-#pragma unroll
-        for (int lo = 1; lo < 8; lo *= 2) {
-#pragma unroll
-            for (int k = 1; k <= lo; ++k) {
-                zr[lo + k] = fma(zr[lo], zr[k], -(zi[lo] * zi[k]));
-                zi[lo + k] = fma(zr[lo], zi[k], zi[lo] * zr[k]);
-            }
-        }
-        if (j == 1) {
-            wr[0] = 1.0; wi[0] = 0.0;
-#pragma unroll
-            for (int k = 1; k <= 8; ++k) { wr[k * NL] = zr[k]; wi[k * NL] = zi[k]; }
+        if constexpr (TxWk<P>::ALL) {   // rho^1..rho^8 by doubling, then rho^(8+k) = rho^8 rho^k, rho^(16+k) = rho^16 rho^k
+            constexpr int E = TxWk<P>::E;
             double rp[9];
             rp[1] = rho;
 #pragma unroll
@@ -530,19 +505,45 @@ __device__ __forceinline__ void tx_prologue(const DevSetup& S, const TxSm& sm, i
                 if (8 + k <= E) wp[(8 + k) * NL] = (k == 8) ? r16 : rp[8] * rp[k];
                 if (16 + k <= E) wp[(16 + k) * NL] = r16 * rp[k];
             }
-        } else {
-            const double z16r = fma(zr[8], zr[8], -(zi[8] * zi[8])), z16i = 2.0 * zr[8] * zi[8];
+        }
+    } else if constexpr (TxWk<P>::ALL) {
+        // z^1..z^8 by doubling (z^2; z^3, z^4; z^5..z^8), then z^(8+k) = z^8 z^k, z^(16+k) = z^16 z^k
+        constexpr int E = TxWk<P>::E;
+        static_assert(E > 8 && E <= 24, "published powers");
+        double* wr = wk + TxWk<P>::ZR * NL;
+        double* wi = wk + TxWk<P>::ZI * NL;
+        double zr[9], zi[9];
+        zr[1] = s_; zi[1] = t_;
 #pragma unroll
-            for (int k = 1; k <= 8; ++k) {
-                if (8 + k <= E) {
-                    wr[(8 + k) * NL] = (k == 8) ? z16r : fma(zr[8], zr[k], -(zi[8] * zi[k]));
-                    wi[(8 + k) * NL] = (k == 8) ? z16i : fma(zr[8], zi[k], zi[8] * zr[k]);
-                }
-                if (16 + k <= E) {
-                    wr[(16 + k) * NL] = fma(z16r, zr[k], -(z16i * zi[k]));
-                    wi[(16 + k) * NL] = fma(z16r, zi[k], z16i * zr[k]);
-                }
+        for (int lo = 1; lo < 8; lo *= 2) {
+#pragma unroll
+            for (int k = 1; k <= lo; ++k) {
+                zr[lo + k] = fma(zr[lo], zr[k], -(zi[lo] * zi[k]));
+                zi[lo + k] = fma(zr[lo], zi[k], zi[lo] * zr[k]);
             }
+        }
+        wr[0] = 1.0; wi[0] = 0.0;
+#pragma unroll
+        for (int k = 1; k <= 8; ++k) { wr[k * NL] = zr[k]; wi[k * NL] = zi[k]; }
+        const double z16r = fma(zr[8], zr[8], -(zi[8] * zi[8])), z16i = 2.0 * zr[8] * zi[8];
+#pragma unroll
+        for (int k = 1; k <= 8; ++k) {
+            if (8 + k <= E) {
+                wr[(8 + k) * NL] = (k == 8) ? z16r : fma(zr[8], zr[k], -(zi[8] * zi[k]));
+                wi[(8 + k) * NL] = (k == 8) ? z16i : fma(zr[8], zi[k], zi[8] * zr[k]);
+            }
+            if (16 + k <= E) {
+                wr[(16 + k) * NL] = fma(z16r, zr[k], -(z16i * zi[k]));
+                wi[(16 + k) * NL] = fma(z16r, zi[k], z16i * zr[k]);
+            }
+        }
+    } else {   // z^(2^k), rho^(2^k): the walkers assemble z^e, rho^(e+1) of their columns from these
+        double zr = s_, zi = t_, rp = rho;
+#pragma unroll
+        for (int k = 0; k < 6; ++k) {
+            wk[(WK_POW + 3 * k) * NL] = zr; wk[(WK_POW + 3 * k + 1) * NL] = zi; wk[(WK_POW + 3 * k + 2) * NL] = rp;
+            const double nr = fma(zr, zr, -(zi * zi));
+            zi = 2.0 * zr * zi; zr = nr; rp *= rp;
         }
     }
 }
@@ -591,6 +592,9 @@ __device__ __forceinline__ void tx_rot_store(double* rot, int lane, const TxRotB
     rot[5 * NL + lane] = b.cw;
 }
 
+// the right-hand side has terms beyond the harmonic field (accel_cold)
+__host__ __device__ inline bool tx_cold(const DevSetup& S) { return S.n_bodies > 0 || S.has_srp || S.has_drag || S.n_xgrav > 0; }
+
 // z^W, rho^(W+1) (sequence a) and z^(2^NB - 1 - W), rho^(2^NB - W) (sequence b) from the published z^(2^k), rho^(2^k): W and its
 // complement split the NB powers between them; the first factor of each product is a copy
 template <int W, int NB>
@@ -613,7 +617,9 @@ __device__ __forceinline__ void tx_start_powers(const double* wk, double& zar, d
     }
 }
 
-template <int P, int NCTX>
+// COLD: the setup has third bodies, SRP, drag, further fields or a field about another body (accel_cold / field_offset).  Without
+// it the helpers' stage loop has no call in it: the values live across those calls were what spilled to local memory.
+template <int P, int NCTX, bool COLD>
 __global__ void __launch_bounds__((P + HW * NCTX) * 32, 1)
 nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, const __grid_constant__ DevTxQueue q, size_t n,
           const double* __restrict__ state, const double* __restrict__ consts, const long long* __restrict__ epoch0,
@@ -622,8 +628,8 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
     static_assert(P <= NYXB_TX_MAXP && NCTX >= 1 && NCTX <= 2, "walker positions / set contexts");
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ __align__(8) unsigned long long tma_bar;
-    // READY[context][parity]: "the walker inputs of the next stage with this parity are published" — an mbarrier (96 arrivals: the
-    // three helpers of the context) rather than a named barrier, because the walkers POLL it: a walker warp takes whichever
+    // READY[context][parity]: "the walker inputs of the next stage with this parity are published" — an mbarrier (64 arrivals: the
+    // two helpers of the context) rather than a named barrier, because the walkers POLL it: a walker warp takes whichever
     // context has a stage ready, so the serial stretch between two step attempts of one set (error norm, controller, commit,
     // first prologue) is covered by the other set's stages instead of stalling the walkers.
     __shared__ __align__(8) unsigned long long ready_bar[NCTX][2];
@@ -635,8 +641,8 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
 #endif
     constexpr int NPOW = 6;   // P = 16: z^(2^k), k < NPOW: bits of the exponents below 2P, and the common ratio z^(2P)
     static_assert(P == 8 || P == 10 || P == 16, "walker positions");
-    constexpr int NT_RW = (P + HW) * 32;
-    constexpr int NT_HB = HW * 32;   // threads on the helpers' own barrier   // threads on a READY / DONE barrier: the walkers + the three helpers of the context
+    constexpr int NT_RW = (P + HW) * 32;   // threads on a DONE barrier: the walkers + the helpers of the context
+    constexpr int NT_HB = HW * 32;         // threads on the helpers' own barrier and arrivals on READY
     // named barriers of context c: HB (helpers among themselves), READY[parity], DONE[parity]
     constexpr int BAR_PER_CTX = 5;
     const int N = S.grav.N;
@@ -673,11 +679,10 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
         // parity-(i & 1) buffers.  The harmonic sum of stage i+1 needs only the POSITION of that stage, which depends on the
         // accelerations up to stage i-1 (second-order system): the helpers publish it one walk ahead, so the walkers never wait for
         // the stage they have just finished — only, once per step, for the controller.
-        // column position of this warp.  A warp's scheduler is warp id mod 4, and the six helper warps land 2-2-1-1 on the four
-        // schedulers (P = 8: warps 8 and 12, 9 and 13, 10, 11); the zigzag gives the low positions a third column and a few more
-        // padded entries (N = 21: 34 32 32 30 30 30 28 28).  The lightest pairs go to the schedulers that also host two helpers
-        // (measured before: walks of 3 380 clocks on those against 2 590 on the others, and a stage ends with its slowest walk).
-        const int pos = (P == 8) ? ((0x23571046u >> (4 * w)) & 0xfu) : w;   // warp 0..7 -> 6 4 0 1 7 5 3 2
+        // column position of this warp.  A warp's scheduler is warp id mod 4; with P = 8 every scheduler hosts walkers w and w + 4
+        // and one helper (warps 8..11).  The zigzag gives the low positions a third column and a few more padded entries
+        // (N = 21: 34 32 32 30 30 30 28 28), so position k shares its scheduler with position 7 - k: 34+28, 32+28, 32+30, 30+30.
+        const int pos = (P == 8 && w >= 4) ? 11 - w : w;   // warp 0..7 -> 0 1 2 3 7 6 5 4
         const int* my = sched + pos * (2 + 2 * Tx.kmax);
         const int rec_off = my[0], ncol = my[1];
         unsigned active = (1u << NCTX) - 1u;
@@ -782,20 +787,26 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
     }
 
     // =================================================================================================== HELPER
-    // set context; helper role j: owns state components j (position) and j + 3 (velocity) of trajectory `lane` of the set
+    // set context; two helpers per set, lane = trajectory of the set:
+    //   helper 0 (lead): candidate state and error estimate of the positions, the DCMs of stage 0 and of every stage i+2, the
+    //                    controller, the set queue, loading and parking the controller state;
+    //   helper 1:        the state vector (load, stage-0 and stage-1 inputs, commit, park), reduction of the partial sums, the acceleration (with accel_cold) of all three components, V_{i+1} and
+    //                    P_{i+2} (both need the acceleration just assembled, so they stay on the warp that has it), candidate state
+    //                    and error estimate of the velocities, the DCM of stage 1 and the orientation angles of the next step.
+    // Both derive the stage prologue (tx_prologue) and split what it publishes.
     const int c = (w - P) / HW, j = (w - P) % HW;
     const TxSm sm = tx_views(smem, L, c, N);
     const int BAR_HB = 1 + c * BAR_PER_CTX, BAR_DONE = BAR_HB + 3;
     const DevGrav& gv = S.grav;
-    const bool has_extra = S.n_bodies > 0 || S.has_srp || S.has_drag || S.n_xgrav > 0;
-    const bool lead = (j == 0);   // helper 0 also runs the DCM, the controller and the set queue
+    const bool has_extra = COLD && tx_cold(S);
+    const bool lead = (j == 0);
     const double* ta = S.tb.a;    // a_{q,m} (stage q >= 1, m < q) = ta[(q - 1) * NYXB_MAX_STAGES + m]
 
     // The two sets of a CTA must not reach the serial stretch between two attempts (error norm, controller, commit, first
     // prologues: ~11 000 clocks without work for the walkers) at the same time, and nothing pulls them apart once they run in
     // phase (measured: both contexts started together stayed within 1 % of an attempt of each other, and the walkers idled through
     // every such stretch).  Context 1 therefore starts when context 0 is half-way through its first attempt.
-    bool kick_pending = (NCTX > 1 && c == 0);
+    bool kick_pending = (NCTX > 1 && c == 0 && lead);
     if (NCTX > 1 && c == 1) {
         if (lead && lane == 0) mbar_wait(&kick_bar, 0);
         nb_sync(BAR_HB, NT_HB);
@@ -825,7 +836,7 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
             s_exit[c] = set < 0;   // nothing fresh, nothing parked: every unfinished set is in progress in another context
         }
         nb_sync(BAR_HB, NT_HB);
-        if (s_exit[c] && kick_pending && lead && lane == 0) tx_mbar_arrive(&kick_bar);
+        if (s_exit[c] && kick_pending && lane == 0) tx_mbar_arrive(&kick_bar);
         if (s_exit[c]) {
             tx_mbar_arrive(&ready_bar[c][0]);   // releases the walkers (they expect stage 0), which read s_exit and drop this context
             return;
@@ -837,14 +848,14 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
         const size_t tr = valid ? traj_raw : (size_t)set * NL;   // an absent lane shadows the set's first trajectory, never committed
 
         // ---------------------------------------------------------------- load the set
+        if (!lead) {
 #pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-            const int cc = j + 3 * hh;
-            const double yc = (round == 0) ? state[(size_t)cc * n + tr] : __ldcg(out_state + (size_t)cc * n + tr);
-            sm.ycur[cc * NL + lane] = yc;
-            if (round == 0 && valid && sink.cap > 0) sink.state[((size_t)cc * sink.cap) * n + tr] = yc;
-        }
-        if (lead) {
+            for (int cc = 0; cc < 6; ++cc) {
+                const double yc = (round == 0) ? state[(size_t)cc * n + tr] : __ldcg(out_state + (size_t)cc * n + tr);
+                sm.ycur[cc * NL + lane] = yc;
+                if (round == 0 && valid && sink.cap > 0) sink.state[((size_t)cc * sink.cap) * n + tr] = yc;
+            }
+        } else {
             tx_load_ctl(S, sink, q, sm, lane, n, tr, valid, round, state, consts, epoch0, end_epoch, step_io, out_state, out_epoch);
             tx_pick_step(sm, lane, end_epoch);
             const bool done = sm.i32[TXW_FLAGS * NL + lane] & F_DONE;
@@ -859,155 +870,206 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
             TX_TRACE(TR_TOP, c, 0);
             const double h = sm.f64[TXF_H * NL + lane];
             const long long epoch = sm.i64[TXI_EPOCH * NL + lane];
-            const double r_own = sm.ycur[j * NL + lane], v_own = sm.ycur[(3 + j) * NL + lane];
-            // orientation angles at the step epoch (the lead evaluates every DCM of the attempt).  They are NOT evaluated here, on the
-            // serial path between two attempts: helper 1 evaluates them for the epoch this attempt leads to while the walkers are
-            // busy, and commits them to sm.rot when the controller accepts the step (a rejected step keeps its epoch).
+            // orientation angles at the step epoch (the lead evaluates every DCM of the attempt but that of stage 1).  They are NOT
+            // evaluated here, on the serial path between two attempts: helper 1 evaluates them for the epoch this attempt leads to
+            // while the walkers are busy, and commits them to sm.rot when the controller accepts the step (a rejected step keeps its
+            // epoch).
             TxRotBase rb_;
             rb_.sa = 0.0; rb_.ca = 1.0; rb_.sd = 1.0; rb_.cd = 0.0; rb_.sw = 0.0; rb_.cw = 1.0;
-            TxRotBase rb_next = rb_;
             const bool fixed = sm.i32[TXW_FLAGS * NL + lane] & F_FIXED;
-            // candidate state and error estimate (instance.rs:402-414), accumulated stage by stage in the reference's order
-            double nx_r = r_own, nx_v = v_own, er_r = 0.0, er_v = 0.0;
-            int rc_acc = 0;
             double Rn[9];
             // ---- prime the pipeline: stage 0 (the state itself) and stage 1 (needs only V_0 = v): instance.rs:369-394
-            sm.kst[(0 * 6 + j) * NL + lane] = v_own;                 // k_0[j] = V_0
-            sm.ysp[(0 * 3 + j) * NL + lane] = r_own;                 // P_0
             const long long off1 = (stages > 1) ? dur_from_seconds(S.tb.c[0] * h) : 0;
-            if (stages > 1) sm.ysp[(1 * 3 + j) * NL + lane] = fma(h, ta[0] * v_own, r_own);   // P_1 = r + h a_10 V_0
+            if (!lead) {
+#pragma unroll
+                for (int k = 0; k < 3; ++k) {
+                    const double r_k = sm.ycur[k * NL + lane], v_k = sm.ycur[(3 + k) * NL + lane];
+                    sm.kst[(0 * 6 + k) * NL + lane] = v_k;                                            // k_0[k] = V_0
+                    sm.ysp[(0 * 3 + k) * NL + lane] = r_k;                                            // P_0
+                    if (stages > 1) sm.ysp[(1 * 3 + k) * NL + lane] = fma(h, ta[0] * v_k, r_k);      // P_1 = r + h a_10 V_0
+                }
+            }
             nb_sync(BAR_HB, NT_HB);
             TX_TRACE(TR_PRIMED, c, 0);
+            if (gv.rot.kind != 0) {   // committed by helper 1 before the barrier above
+                rb_.sa = sm.rot[lane]; rb_.ca = sm.rot[NL + lane]; rb_.sd = sm.rot[2 * NL + lane]; rb_.cd = sm.rot[3 * NL + lane];
+                rb_.sw = sm.rot[4 * NL + lane]; rb_.cw = sm.rot[5 * NL + lane];
+            }
+            TxRotBase rb_next = rb_;
             if (lead) {
-                if (gv.rot.kind != 0) {
-                    rb_.sa = sm.rot[lane]; rb_.ca = sm.rot[NL + lane]; rb_.sd = sm.rot[2 * NL + lane]; rb_.cd = sm.rot[3 * NL + lane];
-                    rb_.sw = sm.rot[4 * NL + lane]; rb_.cw = sm.rot[5 * NL + lane];
-                }
                 tx_dcm(gv.rot, rb_, 0, Rn);
 #pragma unroll
                 for (int k = 0; k < 9; ++k) sm.rn[k * NL + lane] = Rn[k];
-            } else if (j == 1 && stages > 1) {   // the DCM of stage 1 in parallel with the lead's (both sat on the serial path between attempts)
-                TxRotBase rb1 = rb_;
-                if (gv.rot.kind != 0) {
-                    rb1.sa = sm.rot[lane]; rb1.ca = sm.rot[NL + lane]; rb1.sd = sm.rot[2 * NL + lane]; rb1.cd = sm.rot[3 * NL + lane];
-                    rb1.sw = sm.rot[4 * NL + lane]; rb1.cw = sm.rot[5 * NL + lane];
-                }
-                tx_dcm(gv.rot, rb1, off1, Rn);
+            } else if (stages > 1) {   // the DCM of stage 1 in parallel with the lead's (both sat on the serial path between attempts)
+                tx_dcm(gv.rot, rb_, off1, Rn);
 #pragma unroll
                 for (int k = 0; k < 9; ++k) sm.rn[(9 + k) * NL + lane] = Rn[k];
             }
             nb_sync(BAR_HB, NT_HB);
             TX_TRACE(TR_DCM01, c, 0);
-            tx_prologue<P>(S, sm, lane, 0, j, sm.ysp, epoch);
+            tx_prologue<P, COLD>(S, sm, lane, 0, j, sm.ysp, epoch);
             tx_mbar_arrive(&ready_bar[c][0]);
             TX_TRACE(TR_READY, c, 0);
             if (stages > 1) {
-                tx_prologue<P>(S, sm, lane, 1, j, sm.ysp + 3 * NL, epoch + off1);
+                tx_prologue<P, COLD>(S, sm, lane, 1, j, sm.ysp + 3 * NL, epoch + off1);
                 tx_mbar_arrive(&ready_bar[c][1]);
                 TX_TRACE(TR_READY, c, 1);
             }
-            nb_sync(BAR_HB, NT_HB);   // the lead overwrites rn[0] (DCM of stage 2) in the first slack below: every helper has read it by now
-            // ---- derive(): the stages of one attempt for the 32 trajectories (instance.rs:358-493), one walk ahead of the walkers
-            for (int i = 0; i < stages; ++i) {
-                const int par = i & 1;
-                // -- slack: everything that does not need the acceleration of stage i
-                double preV = 0.0, preP = 0.0;
-                long long off2 = 0;
-                {
-                    const double vi = sm.kst[(i * 6 + j) * NL + lane];   // V_i
-                    if (!fixed) er_r = fma(h * S.tb.e[i], vi, er_r);
-                    nx_r = fma(h * S.tb.b[i], vi, nx_r);
-                }
-                if (j == 1 && i == 0 && gv.rot.kind != 0)
-                    rb_next = tx_rot_base(gv.rot, epoch + (fixed ? sm.i64[TXI_STEP * NL + lane] : dur_from_seconds(h)));
-                if (i + 1 < stages) {   // V_{i+1} = v + h sum_{l<=i} a_{i+1,l} A_l: all terms but the last
-                    const double* arow = ta + i * NYXB_MAX_STAGES;
-                    const double* kc = sm.kst + (3 + j) * NL + lane;
-                    double w0 = 0.0, w1 = 0.0;
-                    int l = 0;
-                    for (; l + 1 < i; l += 2) { w0 = fma(arow[l], kc[l * 6 * NL], w0); w1 = fma(arow[l + 1], kc[(l + 1) * 6 * NL], w1); }
-                    if (l < i) w0 = fma(arow[l], kc[l * 6 * NL], w0);
-                    preV = w0 + w1;
-                }
-                if (i + 2 < stages) {   // P_{i+2} = r + h sum_{m<=i+1} a_{i+2,m} V_m: all terms but the last (V_i is known)
-                    const double* arow = ta + (i + 1) * NYXB_MAX_STAGES;
-                    const double* kc = sm.kst + j * NL + lane;
-                    double w0 = 0.0, w1 = 0.0;
-                    int m = 0;
-                    for (; m + 1 <= i; m += 2) { w0 = fma(arow[m], kc[m * 6 * NL], w0); w1 = fma(arow[m + 1], kc[(m + 1) * 6 * NL], w1); }
-                    if (m <= i) w0 = fma(arow[m], kc[m * 6 * NL], w0);
-                    preP = w0 + w1;
-                    off2 = dur_from_seconds(S.tb.c[i + 1] * h);
-                    TX_TRACE(TR_PRE_DONE, c, i);
-                    if (lead) {   // DCM of stage i+2 (its parity buffer was last read in the prologue of stage i, two barriers ago)
+            nb_sync(BAR_HB, NT_HB);   // the lead overwrites rn[0] (DCM of stage 2) in the first slack below: both helpers have read it by now
+            // ---- derive(): the stages of one attempt for the 32 trajectories (instance.rs:358-493), one walk ahead of the walkers.
+            // Candidate state and error estimate (instance.rs:402-414) accumulate stage by stage in the reference's order.  Per stage
+            // both helpers pass DONE[par] and, before the last stage, HB and the prologue of stage i+2, in the same order.
+            if (lead) {
+                double nx_r[3], er_r[3];
+#pragma unroll
+                for (int k = 0; k < 3; ++k) { nx_r[k] = sm.ycur[k * NL + lane]; er_r[k] = 0.0; }
+                for (int i = 0; i < stages; ++i) {
+                    const int par = i & 1;
+                    // -- slack: position side of the sums (V_i is known), DCM of stage i+2
+                    long long off2 = 0;
+#pragma unroll
+                    for (int k = 0; k < 3; ++k) {
+                        const double vi = sm.kst[(i * 6 + k) * NL + lane];   // V_i
+                        if (!fixed) er_r[k] = fma(h * S.tb.e[i], vi, er_r[k]);
+                        nx_r[k] = fma(h * S.tb.b[i], vi, nx_r[k]);
+                    }
+                    if (i + 2 < stages) {   // DCM of stage i+2 (its parity buffer was last read in the prologue of stage i, two barriers ago)
+                        off2 = dur_from_seconds(S.tb.c[i + 1] * h);
+                        TX_TRACE(TR_PRE_DONE, c, i);
                         tx_dcm(gv.rot, rb_, off2, Rn);
 #pragma unroll
                         for (int k = 0; k < 9; ++k) sm.rn[(par * 9 + k) * NL + lane] = Rn[k];
                     }
+                    TX_TRACE(TR_DCM_DONE, c, i);
+                    if (kick_pending && i == stages / 2) {
+                        if (lane == 0) tx_mbar_arrive(&kick_bar);
+                        kick_pending = false;
+                    }
+                    TX_TRACE(TR_DONE_WAIT, c, i);
+                    nb_sync(BAR_DONE + par, NT_RW);   // the walkers' partial sums of stage i are back
+                    TX_TRACE(TR_DONE_SEEN, c, i);
+                    if (i + 1 < stages) {
+                        nb_sync(BAR_HB, NT_HB);   // V_{i+1} and the position of stage i+2 are in shared memory
+                        TX_TRACE(TR_HB_PASSED, c, i);
+                        if (i + 2 < stages) {
+                            tx_prologue<P, COLD>(S, sm, lane, par, 0, sm.ysp + par * 3 * NL, epoch + off2);
+                            tx_mbar_arrive(&ready_bar[c][par]);   // walker inputs of stage i+2 are published
+                            TX_TRACE(TR_READY, c, i + 2);
+                        }
+                    }
                 }
-                TX_TRACE(TR_DCM_DONE, c, i);
-                if (kick_pending && i == stages / 2) {
-                    if (lead && lane == 0) tx_mbar_arrive(&kick_bar);
-                    kick_pending = false;
+#pragma unroll
+                for (int k = 0; k < 3; ++k) { sm.nxt[k * NL + lane] = nx_r[k]; sm.er[k * NL + lane] = er_r[k]; }
+            } else {
+                double r_own[3], v_own[3], nx_v[3], er_v[3];
+#pragma unroll
+                for (int k = 0; k < 3; ++k) {
+                    r_own[k] = sm.ycur[k * NL + lane]; v_own[k] = sm.ycur[(3 + k) * NL + lane];
+                    nx_v[k] = v_own[k]; er_v[k] = 0.0;
                 }
-                TX_TRACE(TR_DONE_WAIT, c, i);
-                nb_sync(BAR_DONE + par, NT_RW);   // the walkers' partial sums of stage i are back
-                TX_TRACE(TR_DONE_SEEN, c, i);
+                int rc_acc = 0;
+                for (int i = 0; i < stages; ++i) {
+                    const int par = i & 1;
+                    // -- slack: everything that does not need the acceleration of stage i
+                    double preV[3] = {0.0, 0.0, 0.0}, preP[3] = {0.0, 0.0, 0.0};
+                    long long off2 = 0;
+                    if (i == 0 && gv.rot.kind != 0)
+                        rb_next = tx_rot_base(gv.rot, epoch + (fixed ? sm.i64[TXI_STEP * NL + lane] : dur_from_seconds(h)));
+                    if (i + 1 < stages) {   // V_{i+1} = v + h sum_{l<=i} a_{i+1,l} A_l: all terms but the last
+                        const double* arow = ta + i * NYXB_MAX_STAGES;
+#pragma unroll
+                        for (int k = 0; k < 3; ++k) {
+                            const double* kc = sm.kst + (3 + k) * NL + lane;
+                            double w0 = 0.0, w1 = 0.0;
+                            int l = 0;
+                            for (; l + 1 < i; l += 2) { w0 = fma(arow[l], kc[l * 6 * NL], w0); w1 = fma(arow[l + 1], kc[(l + 1) * 6 * NL], w1); }
+                            if (l < i) w0 = fma(arow[l], kc[l * 6 * NL], w0);
+                            preV[k] = w0 + w1;
+                        }
+                    }
+                    if (i + 2 < stages) {   // P_{i+2} = r + h sum_{m<=i+1} a_{i+2,m} V_m: all terms but the last (V_i is known)
+                        const double* arow = ta + (i + 1) * NYXB_MAX_STAGES;
+#pragma unroll
+                        for (int k = 0; k < 3; ++k) {
+                            const double* kc = sm.kst + k * NL + lane;
+                            double w0 = 0.0, w1 = 0.0;
+                            int m = 0;
+                            for (; m + 1 <= i; m += 2) { w0 = fma(arow[m], kc[m * 6 * NL], w0); w1 = fma(arow[m + 1], kc[(m + 1) * 6 * NL], w1); }
+                            if (m <= i) w0 = fma(arow[m], kc[m * 6 * NL], w0);
+                            preP[k] = w0 + w1;
+                        }
+                        off2 = dur_from_seconds(S.tb.c[i + 1] * h);
+                        TX_TRACE(TR_PRE_DONE, c, i);
+                    }
+                    TX_TRACE(TR_DONE_WAIT, c, i);
+                    nb_sync(BAR_DONE + par, NT_RW);   // the walkers' partial sums of stage i are back
+                    TX_TRACE(TR_DONE_SEEN, c, i);
 
-                // -- reduce the partial sums, assemble the acceleration component j of stage i (spacecraft.rs:216-247)
-                double X, Y, Z, Wt;
-                {
-                    double ax[4] = {0.0, 0.0, 0.0, 0.0}, ay[4] = {0.0, 0.0, 0.0, 0.0}, az[4] = {0.0, 0.0, 0.0, 0.0}, aw4[4] = {0.0, 0.0, 0.0, 0.0};
+                    // -- reduce the partial sums, assemble the acceleration of stage i (spacecraft.rs:216-247)
+                    double X, Y, Z, Wt;
+                    {
+                        double ax[4] = {0.0, 0.0, 0.0, 0.0}, ay[4] = {0.0, 0.0, 0.0, 0.0}, az[4] = {0.0, 0.0, 0.0, 0.0}, aw4[4] = {0.0, 0.0, 0.0, 0.0};
 #pragma unroll
-                    for (int p = 0; p < P; ++p) {
-                        const double* pt = sm.part + ((par * P + p) * 4) * NL + lane;
-                        ax[p & 3] += pt[0]; ay[p & 3] += pt[NL]; az[p & 3] += pt[2 * NL]; aw4[p & 3] += pt[3 * NL];
+                        for (int p = 0; p < P; ++p) {
+                            const double* pt = sm.part + ((par * P + p) * 4) * NL + lane;
+                            ax[p & 3] += pt[0]; ay[p & 3] += pt[NL]; az[p & 3] += pt[2 * NL]; aw4[p & 3] += pt[3 * NL];
+                        }
+                        X = (ax[0] + ax[1]) + (ax[2] + ax[3]); Y = (ay[0] + ay[1]) + (ay[2] + ay[3]);
+                        Z = (az[0] + az[1]) + (az[2] + az[3]); Wt = (aw4[0] + aw4[1]) + (aw4[2] + aw4[3]);
                     }
-                    X = (ax[0] + ax[1]) + (ax[2] + ax[3]); Y = (ay[0] + ay[1]) + (ay[2] + ay[3]);
-                    Z = (az[0] + az[1]) + (az[2] + az[3]); Wt = (aw4[0] + aw4[1]) + (aw4[2] + aw4[3]);
-                }
-                TX_TRACE(TR_REDUCED, c, i);
-                const double* as = sm.as + par * AS_COUNT * NL + lane;
-                const double K0 = as[AS_K0 * NL], K1 = as[AS_K1 * NL];
-                const double aw = -K0 * Wt;
-                const double ab0 = fma(aw, as[AS_S * NL], K1 * X), ab1 = fma(aw, as[AS_T * NL], K1 * Y), ab2 = fma(aw, as[AS_U * NL], K1 * Z);
-                double acc = fma(as[AS_FAC * NL], as[(AS_P0 + j) * NL],
-                                 fma(as[(AS_R + 6 + j) * NL], ab2, fma(as[(AS_R + 3 + j) * NL], ab1, as[(AS_R + j) * NL] * ab0)));
-                if (has_extra) {
-                    double yy[9], aa[3] = {0.0, 0.0, 0.0};
-                    const double hz = (i > 0) ? h * 0.0 : 0.0;
-                    yy[0] = as[AS_P0 * NL]; yy[1] = as[AS_P1 * NL]; yy[2] = as[AS_P2 * NL];
+                    TX_TRACE(TR_REDUCED, c, i);
+                    const double* as = sm.as + par * AS_COUNT * NL + lane;
+                    const double K0 = as[AS_K0 * NL], K1 = as[AS_K1 * NL];
+                    const double aw = -K0 * Wt;
+                    const double ab0 = fma(aw, as[AS_S * NL], K1 * X), ab1 = fma(aw, as[AS_T * NL], K1 * Y), ab2 = fma(aw, as[AS_U * NL], K1 * Z);
+                    double acc[3];
 #pragma unroll
-                    for (int e = 0; e < 3; ++e) yy[3 + e] = sm.kst[(i * 6 + e) * NL + lane];   // V_i
-                    yy[6] = sm.f64[TXF_CR * NL + lane] + hz; yy[7] = sm.f64[TXF_CD * NL + lane] + hz; yy[8] = sm.f64[TXF_PM * NL + lane] + hz;
-                    const long long offi = (i > 0) ? dur_from_seconds(S.tb.c[i - 1] * h) : 0;
-                    const int rcx = accel_cold<true>(S, sm.f64[TXF_DRY * NL + lane], sm.f64[TXF_EXTRA * NL + lane], sm.f64[TXF_SRPA * NL + lane],
-                                                     sm.f64[TXF_DRAGA * NL + lane], epoch + offi, yy, aa);
-                    acc += (j == 0) ? aa[0] : (j == 1 ? aa[1] : aa[2]);
-                    if (rcx && !rc_acc) rc_acc = rcx | ((i + 1) << 8);
-                }
-                sm.kst[(i * 6 + 3 + j) * NL + lane] = acc;     // k_i[3+j] = A_i
-                if (!fixed) er_v = fma(h * S.tb.e[i], acc, er_v);
-                nx_v = fma(h * S.tb.b[i], acc, nx_v);
-                if (i + 1 < stages) {
-                    const double vn = fma(h, fma(ta[i * NYXB_MAX_STAGES + i], acc, preV), v_own);   // V_{i+1}
-                    sm.kst[((i + 1) * 6 + j) * NL + lane] = vn;                                    // k_{i+1}[j]
-                    if (i + 2 < stages)
-                        sm.ysp[(par * 3 + j) * NL + lane] = fma(h, fma(ta[(i + 1) * NYXB_MAX_STAGES + i + 1], vn, preP), r_own);   // P_{i+2}
-                    TX_TRACE(TR_ACC_DONE, c, i);
-                    nb_sync(BAR_HB, NT_HB);   // V_{i+1} and the position components of stage i+2 of all three helpers are in shared memory
-                    TX_TRACE(TR_HB_PASSED, c, i);
-                    if (i + 2 < stages) {
-                        tx_prologue<P>(S, sm, lane, par, j, sm.ysp + par * 3 * NL, epoch + off2);
-                        tx_mbar_arrive(&ready_bar[c][par]);   // walker inputs of stage i+2 are published
-                        TX_TRACE(TR_READY, c, i + 2);
+                    for (int k = 0; k < 3; ++k)
+                        acc[k] = fma(as[AS_FAC * NL], as[(AS_P0 + k) * NL],
+                                     fma(as[(AS_R + 6 + k) * NL], ab2, fma(as[(AS_R + 3 + k) * NL], ab1, as[(AS_R + k) * NL] * ab0)));
+                    if (has_extra) {
+                        double yy[9], aa[3] = {0.0, 0.0, 0.0};
+                        const double hz = (i > 0) ? h * 0.0 : 0.0;
+                        yy[0] = as[AS_P0 * NL]; yy[1] = as[AS_P1 * NL]; yy[2] = as[AS_P2 * NL];
+#pragma unroll
+                        for (int e = 0; e < 3; ++e) yy[3 + e] = sm.kst[(i * 6 + e) * NL + lane];   // V_i
+                        yy[6] = sm.f64[TXF_CR * NL + lane] + hz; yy[7] = sm.f64[TXF_CD * NL + lane] + hz; yy[8] = sm.f64[TXF_PM * NL + lane] + hz;
+                        const long long offi = (i > 0) ? dur_from_seconds(S.tb.c[i - 1] * h) : 0;
+                        const int rcx = accel_cold<true>(S, sm.f64[TXF_DRY * NL + lane], sm.f64[TXF_EXTRA * NL + lane], sm.f64[TXF_SRPA * NL + lane],
+                                                         sm.f64[TXF_DRAGA * NL + lane], epoch + offi, yy, aa);
+#pragma unroll
+                        for (int k = 0; k < 3; ++k) acc[k] += aa[k];
+                        if (rcx && !rc_acc) rc_acc = rcx | ((i + 1) << 8);
+                    }
+#pragma unroll
+                    for (int k = 0; k < 3; ++k) {
+                        sm.kst[(i * 6 + 3 + k) * NL + lane] = acc[k];     // k_i[3+k] = A_i
+                        if (!fixed) er_v[k] = fma(h * S.tb.e[i], acc[k], er_v[k]);
+                        nx_v[k] = fma(h * S.tb.b[i], acc[k], nx_v[k]);
+                    }
+                    if (i + 1 < stages) {
+#pragma unroll
+                        for (int k = 0; k < 3; ++k) {
+                            const double vn = fma(h, fma(ta[i * NYXB_MAX_STAGES + i], acc[k], preV[k]), v_own[k]);   // V_{i+1}
+                            sm.kst[((i + 1) * 6 + k) * NL + lane] = vn;                                            // k_{i+1}[k]
+                            if (i + 2 < stages)
+                                sm.ysp[(par * 3 + k) * NL + lane] = fma(h, fma(ta[(i + 1) * NYXB_MAX_STAGES + i + 1], vn, preP[k]), r_own[k]);   // P_{i+2}
+                        }
+                        TX_TRACE(TR_ACC_DONE, c, i);
+                        nb_sync(BAR_HB, NT_HB);   // V_{i+1} and the position of stage i+2 are in shared memory
+                        TX_TRACE(TR_HB_PASSED, c, i);
+                        if (i + 2 < stages) {
+                            tx_prologue<P, COLD>(S, sm, lane, par, 1, sm.ysp + par * 3 * NL, epoch + off2);
+                            tx_mbar_arrive(&ready_bar[c][par]);   // walker inputs of stage i+2 are published
+                            TX_TRACE(TR_READY, c, i + 2);
+                        }
                     }
                 }
+#pragma unroll
+                for (int k = 0; k < 3; ++k) { sm.nxt[(3 + k) * NL + lane] = nx_v[k]; sm.er[(3 + k) * NL + lane] = er_v[k]; }
+                sm.i32[TXW_RCST * NL + lane] = rc_acc;
             }
             TX_TRACE(TR_STAGES_END, c, 0);
-            sm.nxt[j * NL + lane] = nx_r; sm.nxt[(3 + j) * NL + lane] = nx_v;
-            sm.er[j * NL + lane] = er_r; sm.er[(3 + j) * NL + lane] = er_v;
-            if (lead) sm.i32[TXW_RCST * NL + lane] = rc_acc;
             nb_sync(BAR_HB, NT_HB);
             TX_TRACE(TR_CTRL_IN, c, 0);
             if (lead) {
@@ -1022,12 +1084,11 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
             }
             nb_sync(BAR_HB, NT_HB);
             TX_TRACE(TR_CTRL_END, c, 0);
-            if (sm.i32[TXW_ACC * NL + lane]) {
-                if (j == 1 && gv.rot.kind != 0) tx_rot_store(sm.rot, lane, rb_next);   // read by the lead after the next HB barrier
+            if (!lead && sm.i32[TXW_ACC * NL + lane]) {
+                if (gv.rot.kind != 0) tx_rot_store(sm.rot, lane, rb_next);   // read by both helpers after the next HB barrier
                 const long long ns = sm.i64[TXI_NSTEPS * NL + lane];
 #pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {
-                    const int cc = j + 3 * hh;
+                for (int cc = 0; cc < 6; ++cc) {
                     const double nx = sm.nxt[cc * NL + lane];
                     sm.ycur[cc * NL + lane] = nx;
                     // the channel send of instance.rs:186-193 / 255-259: lanes are consecutive trajectories, one 256-byte store per warp
@@ -1039,13 +1100,13 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
         }
 
         if (kick_pending) {
-            if (lead && lane == 0) tx_mbar_arrive(&kick_bar);
+            if (lane == 0) tx_mbar_arrive(&kick_bar);
             kick_pending = false;
         }
         // ---------------------------------------------------------------- park the set (== final outputs when it is done)
-        if (valid) {
-            out_state[(size_t)j * n + tr] = sm.ycur[j * NL + lane];
-            out_state[(size_t)(j + 3) * n + tr] = sm.ycur[(j + 3) * NL + lane];
+        if (!lead && valid) {
+#pragma unroll
+            for (int cc = 0; cc < 6; ++cc) out_state[(size_t)cc * n + tr] = sm.ycur[cc * NL + lane];
         }
         if (lead) tx_park_ctl(sink, q, sm, lane, n, tr, step_io, out_state, out_epoch, out_status);
         __threadfence();
@@ -1065,14 +1126,14 @@ nyxb_k_tx(const __grid_constant__ DevSetup S, const __grid_constant__ DevTx Tx, 
 }
 
 // walker positions and set contexts for a field of degree N: two sets in flight while both fit in shared memory
-template <int P, int NCTX>
+template <int P, int NCTX, bool COLD>
 cudaError_t tx_launch_p(const DevSetup* S, const DevTx* Tx, const DevTxQueue* q, size_t n, const double* state, const double* consts,
                         const long long* epoch0, long long end_epoch, long long* step_io, double* out_state, long long* out_epoch,
                         int* out_status, const DevSink* sink, int grid, size_t smem, unsigned blob_bytes, unsigned off_recK,
                         unsigned off_seed, unsigned off_sched, cudaStream_t stream) {
-    cudaError_t e = cudaFuncSetAttribute(nyxb_k_tx<P, NCTX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(nyxb_k_tx<P, NCTX, COLD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    nyxb_k_tx<P, NCTX><<<grid, (P + HW * NCTX) * 32, smem, stream>>>(*S, *Tx, *q, n, state, consts, epoch0, end_epoch, step_io, out_state,
+    nyxb_k_tx<P, NCTX, COLD><<<grid, (P + HW * NCTX) * 32, smem, stream>>>(*S, *Tx, *q, n, state, consts, epoch0, end_epoch, step_io, out_state,
                                                                   out_epoch, out_status, *sink, blob_bytes, off_recK, off_seed, off_sched);
     return cudaGetLastError();
 }
@@ -1201,7 +1262,9 @@ extern "C" cudaError_t nyxb_launch_tx(const DevSetup* S, const DevTx* Tx, const 
     size_t smem = 0;
     const int nctx = tx_contexts(S, Tx, &smem);
     if (nctx < 1 || grid < 1) return cudaErrorInvalidConfiguration;
-#define NYXB_TX_GO(PP, CC) tx_launch_p<PP, CC>(S, Tx, q, n, state, consts, epoch0, end_epoch, step_io, out_state, out_epoch, out_status, sink, grid, smem, b.bytes, b.off_recK, b.off_seed, b.off_sched, stream)
+    const bool cold = tx_cold(*S) || S->grav_body >= 0;
+#define NYXB_TX_GO(PP, CC) (cold ? tx_launch_p<PP, CC, true>(S, Tx, q, n, state, consts, epoch0, end_epoch, step_io, out_state, out_epoch, out_status, sink, grid, smem, b.bytes, b.off_recK, b.off_seed, b.off_sched, stream) \
+                             : tx_launch_p<PP, CC, false>(S, Tx, q, n, state, consts, epoch0, end_epoch, step_io, out_state, out_epoch, out_status, sink, grid, smem, b.bytes, b.off_recK, b.off_seed, b.off_sched, stream))
     if (Tx->P == 8) return nctx == 2 ? NYXB_TX_GO(8, 2) : NYXB_TX_GO(8, 1);
     if (Tx->P == 10) return nctx == 2 ? NYXB_TX_GO(10, 2) : NYXB_TX_GO(10, 1);
     if (Tx->P == 16) return NYXB_TX_GO(16, 1);

@@ -1,7 +1,8 @@
 """Timeline of CTA 0 of the transposed kernel (diagnostic build: make -C nyx_b200/csrc EXTRA=-DNYXB_TX_TRACE, run with
-NYXB_TX_TRACE_FILE=out.bin): python scripts/tx_trace.py out.bin [walkers=8]
-Prints, in SM clocks: walk duration, walker wait per walk, helper latency DONE -> READY (post), READY -> next DONE wait (slack),
-the serial stretch between two attempts, and how long a published stage waits for the walkers."""
+NYXB_TX_TRACE_FILE=out.bin): python scripts/tx_trace.py out.bin [walkers=8] [helpers per set=2]
+Prints, in SM clocks: walk duration (all walkers and per scheduler), walker wait per walk, helper latency DONE -> READY (post),
+READY -> next DONE wait (slack), the serial stretch between two attempts, and how long a published stage waits for the walkers.
+Helper 0 of a set is the lead (position side, DCMs, controller); helper 1 reduces the partial sums and assembles the accelerations."""
 import sys
 import numpy as np
 
@@ -9,6 +10,7 @@ CAP = 8192
 NAMES = {1: "POLL", 2: "WALK", 3: "WALK_END", 4: "DONE_WAIT", 5: "DONE_SEEN", 6: "READY", 7: "STAGES_END", 8: "CTRL_END", 9: "TOP", 10: "PRE_DONE", 11: "DCM_DONE", 12: "REDUCED", 13: "ACC_DONE", 14: "HB_PASSED"}
 raw = np.fromfile(sys.argv[1], dtype=np.uint64).reshape(32, CAP)
 P = int(sys.argv[2]) if len(sys.argv) > 2 else 8
+HW = int(sys.argv[3]) if len(sys.argv) > 3 else 2
 
 
 def decode(strip):
@@ -29,6 +31,7 @@ walk_end = {}    # (ctx, walk ordinal of that ctx) -> latest WALK_END over the w
 walk_start = {}
 print("walkers:")
 allw, allp = [], []
+per_sched = {}
 for w in range(P):
     t, code, ctx, stg = decode(raw[w])
     ordn = {0: 0, 1: 0}
@@ -37,19 +40,22 @@ for w in range(P):
         if code[i] == 1 and code[i + 1] == 2 and code[i + 2] == 3:
             c = ctx[i + 1]
             allp.append(t[i + 1] - t[i]); allw.append(t[i + 2] - t[i + 1])
+            per_sched.setdefault(w % 4, []).append(t[i + 2] - t[i + 1])
             k = (c, ordn[c]); ordn[c] += 1
             walk_end[k] = max(walk_end.get(k, 0), t[i + 2]); walk_start[k] = min(walk_start.get(k, 1 << 62), t[i + 1])
             i += 3
         else:
             i += 1
 stats("walk (READY seen -> DONE arrive)", allw)
+for sc in sorted(per_sched):
+    stats(f"walk on scheduler {sc} (walkers {', '.join(str(w) for w in range(P) if w % 4 == sc)})", per_sched[sc])
 stats("wait before a walk (poll)", allp)
 print(f"  walkers busy {100 * sum(allw) / (sum(allw) + sum(allp)):.1f} % of their time")
 print("helpers (lead = first helper of a context):")
-for h in range(P, P + 6):
+for h in range(P, P + 2 * HW):
     t, code, ctx, stg = decode(raw[h])
     if len(t) == 0: continue
-    c = (h - P) // 3
+    c = (h - P) // HW
     post, slack, dwait, ready_at = [], [], [], {}
     last_ready = None
     ordn = 0
@@ -63,7 +69,7 @@ for h in range(P, P + 6):
             if j < len(t) and code[j] == 6: post.append(t[j] - t[i])
         if code[i] == 6: last_ready = t[i]
     bound = [t[j] - t[i] for i in range(len(t)) if code[i] == 7 for j in range(i + 1, min(i + 6, len(t))) if code[j] == 6 and stg[j] == 0][:10000]
-    print(f" helper warp {h} (context {c}, helper {(h - P) % 3}):")
+    print(f" helper warp {h} (context {c}, helper {(h - P) % HW}, scheduler {h % 4}):")
     seg = {}
     for i in range(len(t) - 1):
         if code[i] in (6, 10, 11, 5, 12, 13, 14) and code[i + 1] in (10, 11, 4, 12, 13, 14, 6) and stg[i] == stg[i + 1] or (code[i] == 6 and code[i + 1] == 10):
@@ -74,7 +80,7 @@ for h in range(P, P + 6):
     stats("between attempts: last stage done -> READY(0)", bound)
 # how long does a published stage wait for the walkers? lead's READY(c, stage) vs first walker start of that walk
 for c in range(2):
-    t, code, ctx, stg = decode(raw[P + 3 * c])
+    t, code, ctx, stg = decode(raw[P + HW * c])
     ready = [t[i] for i in range(len(t)) if code[i] == 6]
     lat = [walk_start[(c, k)] - ready[k] for k in range(min(len(ready), sum(1 for kk in walk_start if kk[0] == c))) if (c, k) in walk_start]
     stats(f"context {c}: READY published -> first walker starts", lat)
