@@ -371,7 +371,11 @@ int32_t nyxb_traj_resample_dev(nyxb_engine* eng, size_t n, const nyxb_traj_sink*
  *  run_status         [n] or NULL: out_status of the propagation — runs with an error code are skipped;
  *  out_event_epoch_ns [n], out_event_state [6][n] (NaN where not located),
  *  out_status         [n]: NYXB_TRAJ_OK; NYXB_TRAJ_NO_DATA (skipped run, fewer than two records);
- *                     NYXB_EVENT_NOT_BRACKETED (the scalar has the same sign at both ends of the last step). */
+ *                     NYXB_EVENT_NOT_BRACKETED (the scalar has the same sign at both ends of the last step).
+ * The search cannot see a truncated recording: it takes the last two records the sink holds.  When the run took more steps
+ * than the sink's capacity (count == capacity), those are not the bracketing step and the located event is wrong or
+ * NOT_BRACKETED.  Give the propagation a sink with room for every step (PropInstance.until_nth_event refuses a capacity
+ * that is too small; MonteCarlo.run_until_nth_event grows its sink and propagates again). */
 enum { NYXB_EVENT_NOT_BRACKETED = 2 };
 int32_t nyxb_event_locate(nyxb_engine* eng, size_t n, const nyxb_traj_sink* sink, int32_t kind, double value,
                           int64_t epoch_precision_ns, const int32_t* run_status,

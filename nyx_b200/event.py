@@ -118,12 +118,14 @@ def brent(f: Callable[[float], float], a: float, b: float, xtol: float, max_iter
     return b
 
 
-def locate_event(traj: Traj, event: Event):
+def locate_event(traj: Traj, event: Event, bracket=None):
     """event.rs:166-211: bracket = the last two recorded states (the device stopped at the end of the crossing step);
-    Brent on `event(traj.at(epoch))`, then the interpolated state at the event epoch."""
+    Brent on `event(traj.at(epoch))`, then the interpolated state at the event epoch.  `bracket` = (t_a, t_b), t_a < t_b, the
+    step to search instead: a backward run's last step is the earliest one of its (ascending) trajectory, which is where
+    `nyxb_event_locate` searches."""
     if len(traj) < 2:
         raise ValueError("trajectory too short to hold an event bracket")
-    t_a, t_b = int(traj.epochs_ns[-2]), int(traj.epochs_ns[-1])
+    t_a, t_b = (int(traj.epochs_ns[-2]), int(traj.epochs_ns[-1])) if bracket is None else (int(bracket[0]), int(bracket[1]))
     t0 = t_a
 
     def f(dt_s: float) -> float:

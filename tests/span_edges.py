@@ -437,14 +437,15 @@ def oracle_stm_chain(name):
 
 # ---- 40-digit universal-variable Kepler solution (Curtis, Orbital Mechanics for Engineering Students, algorithm 3.3 / 3.4)
 def kepler(r0, v0, dt_ns, mu=TWOBODY_MU, dps=40):
-    """position (km) and velocity (km/s) after dt_ns on the two-body orbit through (r0, v0)"""
+    """position (km) and velocity (km/s) after dt_ns on the two-body orbit through (r0, v0); dt_ns may be an mpmath number
+    (a fraction of a nanosecond, for root searches)"""
     import mpmath as mp
 
     with mp.workdps(dps):
         mu = mp.mpf(mu)
         r0 = [mp.mpf(float(x)) for x in r0]
         v0 = [mp.mpf(float(x)) for x in v0]
-        dt = mp.mpf(int(dt_ns)) / 10**9
+        dt = (dt_ns if isinstance(dt_ns, mp.mpf) else mp.mpf(int(dt_ns))) / 10**9
         if dt == 0:
             return np.array([float(x) for x in r0]), np.array([float(x) for x in v0])
         rn = mp.sqrt(sum(x * x for x in r0))
