@@ -39,8 +39,9 @@ extern "C" {
                               and nyxb_predict_outputs, then nyxb_od_bls_batch, nyxb_od_bls_evaluate_batch, nyxb_bls_config, nyxb_bls_outputs and
                               the status codes 6-8, then nyxb_od_records, nyxb_od_ekf_record_batch, nyxb_smooth_outputs, nyxb_od_smooth_batch,
                               then NYXB_MSR_X/Y/Z, nyxb_position_device, nyxb_position_arc, nyxb_od_position_batch, nyxb_od_position_smooth_batch,
-                              then NYXB_MSR_AZIMUTH/ELEVATION, nyxb_aer_station, nyxb_od_aer_batch, nyxb_od_aer_smooth_batch
-                              and the status codes 9-10 were added later without a bump (a pure addition: no existing type or entry point changed).  Earlier: 2: nyxb_srp gained `estimate`; STM, filter and dispersion entry points.  3: nyxb_traj_resample[_dev], nyxb_event_locate[_dev] */
+                              then NYXB_MSR_AZIMUTH/ELEVATION, nyxb_aer_station, nyxb_od_aer_batch, nyxb_od_aer_smooth_batch,
+                              then nyxb_interlink_tx, nyxb_od_interlink_batch, nyxb_od_interlink_smooth_batch
+                              and the status codes 9-12 were added later without a bump (a pure addition: no existing type or entry point changed).  Earlier: 2: nyxb_srp gained `estimate`; STM, filter and dispersion entry points.  3: nyxb_traj_resample[_dev], nyxb_event_locate[_dev] */
 
 /* ---- IntegratorMethod — propagators/rk_methods/mod.rs:65-79 (same order) ---- */
 enum nyxb_method {
@@ -209,6 +210,10 @@ enum nyxb_status {
     NYXB_ERR_INVALID_MEASUREMENT = 8,  /* ODError::InvalidMeasurement: an observation that is not finite (blse/mod.rs:266-272) */
     NYXB_ERR_SINGULAR_STM = 9,         /* ODError::SingularStateTransitionMatrix (solution/smooth.rs:149-154) */
     NYXB_ERR_RECORDS_TRUNCATED = 10,   /* the estimate records of a filter exceed their capacity: nothing to smooth from */
+    NYXB_ERR_TX_NO_DATA = 11,          /* ODError::ODTrajError: the interlink transmitter's recording does not cover the epoch
+                                          (interlink/trk_device.rs:180-183, sensitivity.rs:93-101) */
+    NYXB_ERR_NO_RANGE = 12,            /* ODError::MeasurementSimError: an interlink Doppler row without an observed range in the same
+                                          measurement (interlink/sensitivity.rs:105-110) */
     NYXB_WARN_MAX_ATTEMPTS = 0x100 /* OR-ed flag: instance.rs:440-445 (warn only) */
 };
 
@@ -284,7 +289,9 @@ int32_t nyxb_propagate_batch_multi(nyxb_engine* const* engines, int32_t n_engine
  * the state after every accepted step, final partial step included.  Record s of trajectory i lives at
  *   epoch_ns[s*n + i],  state[(c*capacity + s)*n + i]  (c = x,y,z,vx,vy,vz)
  * i.e. step-major SoA: trajectories that advance together write coalesced 56-byte-per-step streams.
- * count[i] = min(n_steps + 1, capacity); records beyond `capacity` are dropped (the final state is still returned). */
+ * count[i] = min(n_steps + 1, capacity); records beyond `capacity` are dropped (the final state is still returned).
+ * As the transmitters of nyxb_od_interlink_batch / _smooth_batch (HOST pointers, n = n_tx): every column must be complete, with
+ * 1 <= count[j] <= capacity (a propagation that dropped records has count > capacity and is refused), epochs in step order. */
 typedef struct {
     int64_t capacity;
     int64_t* epoch_ns;   /* [capacity][n] */
@@ -658,6 +665,50 @@ int32_t nyxb_od_aer_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n
 int32_t nyxb_od_aer_smooth_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_stations, const nyxb_aer_station* stations,
                                  const nyxb_tracking_arc* arc, size_t n, const nyxb_od_records* rec, const int32_t* filter_status,
                                  nyxb_smooth_outputs* out);
+
+/* ---- Spacecraft-to-spacecraft tracking (od/interlink: InterlinkTxSpacecraft): a transmitter spacecraft, known by its recorded
+ * trajectory, measures the range and Doppler of the filtered spacecraft.  The filter of nyxb_od_ekf_batch with nyxb_interlink_tx in
+ * place of nyxb_ground_station; obs, prefit, postfit and resid_ratio are [n_msr][2][n] with the ground station's slots and record tags
+ * (NYXB_OD_TAG).  The transmitter's state is Traj::at of its recording (nyxb_traj_resample's arithmetic), evaluated at every use.
+ * As coded in the reference (interlink/trk_device.rs:180-232, interlink/sensitivity.rs:50-172, process/mod.rs:300-330):
+ *   - h_tilde runs BEFORE measure, with the transmitter at the nominal state's epoch (the measurement epoch): rho_tx = r_rx - r_tx and
+ *     v_rx - v_tx, the range row [dr / rho_obs, 0 ...], the Doppler row [dv / rho_obs - rho_dot_obs dr / rho_obs^2, dr / rho_obs, 0 0 0]
+ *     from the OBSERVED range and Doppler.  Identity rows for types absent from the measurement.  A Doppler row needs an observed range
+ *     in the same measurement: without one the filter ends with NYXB_ERR_NO_RANGE;
+ *   - the computed observation (measure_instantaneous at the propagator's epoch): the transmitter interpolated at that epoch, the line
+ *     of sight tested against the body at the centre of the integration frame (Vallado's SIGHT, receiver first as for ground stations), range |rho| and
+ *     range rate rho . v_rx / |rho| with v_rx the receiver's velocity in the integration frame: the transmitter's velocity is NOT
+ *     subtracted (the reference's comment says otherwise), then minus the bias;
+ *   - an epoch outside the transmitter's recording ends the filter with NYXB_ERR_TX_NO_DATA (not "not visible"), also when the line of
+ *     sight would be blocked: h_tilde comes first.
+ * No integration time, no aberration correction; the recording must be in the integration frame of the estimates.  Batch least squares
+ * does not take interlink devices. */
+typedef struct {
+    int32_t tx;                  /* column of the transmitter's recording in the sink (0 .. n_tx - 1) */
+    int32_t n_types;             /* 1 or 2 */
+    int32_t types[2];            /* NYXB_MSR_RANGE / _DOPPLER, distinct, in the device's list order */
+    double noise_var[2];         /* km^2, km^2/s^2 per list position */
+    double bias[2];              /* per list position */
+    double body_radius_km;       /* radius of the body at the centre of the integration frame, which can obstruct the link; <= 0: no test */
+} nyxb_interlink_tx;
+
+/* n filters over one schedule.  cfg as nyxb_od_ekf_batch with msr_size 1 or 2; n_types need not be a multiple of msr_size (a short last
+ * window, as nyxb_od_aer_batch).  tx_sink: the n_tx transmitter recordings as nyxb_traj_sink lays them out for n = n_tx, HOST pointers:
+ * record s of column j at epoch_ns[s*n_tx + j], state[(c*capacity + s)*n_tx + j], count[j] records (1 <= count <= capacity; ascending
+ * or descending epochs as a propagation writes them).  rec: NULL, or the estimate records (NYXB_OD_TAG); `out` is bit-identical either
+ * way.  NYXB_RC_BAD_ARG before any launch: a type other than Range / Doppler, a duplicate type, n_types outside 1..2, a column outside
+ * the sink, a recording with count > capacity or count < 1, msr_size outside 1..2, a NULL required pointer; NYXB_RC_UNSUPPORTED: the
+ * setups nyxb_propagate_batch_stm rejects.  Per-filter failures are statuses.  Kernel family as nyxb_od_ekf_batch. */
+int32_t nyxb_od_interlink_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_devices, const nyxb_interlink_tx* devices,
+                                size_t n_tx, const nyxb_traj_sink* tx_sink, const nyxb_tracking_arc* arc, size_t n,
+                                const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns, const double* covar0_soa,
+                                const nyxb_od_outputs* out, const nyxb_od_records* rec);
+
+/* ODSolution::smooth of interlink filters: the contract of nyxb_od_smooth_batch with the records of nyxb_od_interlink_batch, the
+ * residual recomputed with the transmitter at record k's epoch; a record epoch outside the recording gives NYXB_ERR_TX_NO_DATA. */
+int32_t nyxb_od_interlink_smooth_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_devices, const nyxb_interlink_tx* devices,
+                                       size_t n_tx, const nyxb_traj_sink* tx_sink, const nyxb_tracking_arc* arc, size_t n,
+                                       const nyxb_od_records* rec, const int32_t* filter_status, nyxb_smooth_outputs* out);
 
 /* ---- Covariance mapping over an ensemble: n independent `KalmanODProcess::predict_until` runs (od/process/mod.rs:440-486) in ONE
  * kernel launch.  Record 0 is the initial estimate; then chunks of cfg->max_step_ns (`for_duration(max_step)`: adaptive steps, the

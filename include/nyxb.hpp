@@ -558,8 +558,50 @@ struct PositionDevice {
     }
 };
 
+// Traj (md/trajectory/traj.rs) reduced to what the interlink needs: ascending epochs and (x, y, z, vx, vy, vz) per record in `frame`
+struct Traj {
+    std::optional<std::string> name;
+    Frame frame = EARTH_J2000();
+    std::vector<int64_t> epoch_ns;   // [k] ascending
+    std::vector<double> state;       // [k][6]
+    size_t size() const { return epoch_ns.size(); }
+};
+
+// InterlinkTxSpacecraft (od/interlink/trk_device.rs:37-260): a transmitter known by its recorded trajectory, measuring the range and
+// Doppler of the filtered spacecraft (nyxb_interlink_tx in nyxb.h, with the reference's as-coded quirks).  Instantaneous measurements
+// without aberration correction only, with the trajectory in the integration frame; `key` names the device in TrackingDataArc.tracker.
+struct InterlinkTxSpacecraft {
+    std::string key;
+    Traj traj;
+    std::vector<MeasurementType> measurement_types;
+    std::vector<StochasticNoise> noises;   // per list position
+    std::optional<int64_t> integration_time;
+    std::optional<std::string> ab_corr;
+    std::string name() const { return traj.name ? *traj.name : "unnamed"; }   // trk_device.rs:93-95
+    nyxb_interlink_tx to_c(int32_t column, const Frame& integration_frame) const {
+        if (integration_time) throw std::runtime_error("interlink: integrated (two-way) measurements are not supported");
+        if (ab_corr) throw std::runtime_error("interlink: aberration correction is not supported (ab_corr must be None)");
+        if (traj.frame.ephemeris_id != integration_frame.ephemeris_id || traj.frame.rotation.kind != integration_frame.rotation.kind)
+            throw std::runtime_error("interlink: the transmitter's trajectory is not in the integration frame");
+        if (traj.size() == 0) throw std::runtime_error("interlink: the transmitter's trajectory is empty");
+        if (measurement_types.empty() || measurement_types.size() > 2 || noises.size() != measurement_types.size())
+            throw std::runtime_error("an interlink carries one or two of {Range, Doppler}, each with its noise");
+        nyxb_interlink_tx d{};
+        d.tx = column; d.n_types = (int32_t)measurement_types.size();
+        for (int q = 0; q < d.n_types; ++q) {
+            const MeasurementType t = measurement_types[q];
+            if (t != MeasurementType::Range && t != MeasurementType::Doppler) throw std::runtime_error("an interlink carries Range and Doppler only");
+            if (q == 1 && t == measurement_types[0]) throw std::runtime_error("an interlink carries distinct types");
+            d.types[q] = (int32_t)t; d.noise_var[q] = noises[q].covariance(); d.bias[q] = noises[q].bias_constant;
+        }
+        d.body_radius_km = integration_frame.mean_equatorial_radius_km;
+        return d;
+    }
+};
+
 class KalmanODProcess;
 class PositionKalmanODProcess;
+class InterlinkKalmanODProcess;
 
 struct ODSolution {
     size_t n = 0, m = 0, ns = 2;   // ns: observation slots, 2 (ground stations), 4 (ground stations with angles) or 3 (position fixes)
@@ -584,6 +626,8 @@ struct ODSolution {
     inline ODSolution smooth(const KalmanODProcess& odp, const TrackingDataArc& arc) const;
     // the same for position fixes (nyxb_od_position_smooth_batch; sm_postfit [cap][3][n])
     inline ODSolution smooth(const PositionKalmanODProcess& odp, const TrackingDataArc& arc) const;
+    // the same for interlink transmitters (nyxb_od_interlink_smooth_batch; sm_postfit [cap][2][n])
+    inline ODSolution smooth(const InterlinkKalmanODProcess& odp, const TrackingDataArc& arc) const;
 };
 
 // Covariance mapping of one estimate (KalmanODProcess::predict_until): record k at epoch0 + k * max_step, k < count
@@ -825,6 +869,98 @@ inline ODSolution ODSolution::smooth(const PositionKalmanODProcess& odp, const T
     nyxb_smooth_outputs out{s.sm_state.data(), s.sm_deviation.data(), s.sm_covar.data(), s.sm_fs_ratio.data(), s.sm_postfit.data(), s.sm_status.data()};
     if (nyxb_od_position_smooth_batch(eng.get(), &cfg, (int32_t)dev.size(), dev.data(), &carc, n, &rec, status.data(), &out) != NYXB_RC_OK)
         throw std::runtime_error(std::string("nyxb_od_position_smooth_batch: ") + nyxb_last_error());
+    return s;
+}
+
+// KalmanODProcess<.., InterlinkTxSpacecraft> (od/process/mod.rs:128-497 with od/interlink): the filter over interlink transmitters,
+// msr_size 1 or 2, on a two-slot arc (slot = Range / Doppler).  Each device's trajectory is one column of the recordings handed to
+// nyxb_od_interlink_batch; record tags NYXB_OD_TAG.
+class InterlinkKalmanODProcess {
+  public:
+    Propagator prop; KalmanVariant variant; std::optional<SigmaRejection> sigma_reject; std::vector<InterlinkTxSpacecraft> devices;
+    const Almanac* almanac = nullptr; std::optional<ProcessNoise3D> process_noise;
+    int64_t max_step = 60 * NS_PER_S, epoch_precision = 1000; int32_t msr_size = 2;
+    InterlinkKalmanODProcess(Propagator p, KalmanVariant v, std::optional<SigmaRejection> rej, std::vector<InterlinkTxSpacecraft> dev,
+                             const Almanac* alm = nullptr, int32_t msr = 2)
+        : prop(std::move(p)), variant(v), sigma_reject(rej), devices(std::move(dev)), almanac(alm), msr_size(msr) {}
+    InterlinkKalmanODProcess& with_process_noise(ProcessNoise3D snc) { process_noise = snc; return *this; }
+    nyxb_od_config config() const { return detail::od_config(variant, sigma_reject, process_noise, max_step, epoch_precision, msr_size); }
+    std::vector<int32_t> tracker_index(const TrackingDataArc& arc) const {
+        std::vector<int32_t> trk(arc.epoch_ns.size());
+        for (size_t k = 0; k < trk.size(); ++k) { trk[k] = -1; for (size_t j = 0; j < devices.size(); ++j) if (devices[j].key == arc.tracker[k]) trk[k] = (int32_t)j; }
+        return trk;
+    }
+    // the devices (device j reads column j) and their recordings as a host-pointer nyxb_traj_sink over the struct's own arrays
+    struct Links {
+        std::vector<nyxb_interlink_tx> dev; std::vector<int64_t> epoch, count; std::vector<double> state; nyxb_traj_sink sink{};
+    };
+    Links links(const Frame& frame) const {
+        Links l;
+        const size_t ntx = devices.size();
+        size_t cap = 0;
+        for (auto& d : devices) cap = std::max(cap, d.traj.size());
+        l.epoch.assign(cap * ntx, 0); l.state.assign(6 * cap * ntx, 0.0); l.count.assign(ntx, 0);
+        for (size_t j = 0; j < ntx; ++j) {
+            const Traj& t = devices[j].traj;
+            l.dev.push_back(devices[j].to_c((int32_t)j, frame));
+            l.count[j] = (int64_t)t.size();
+            for (size_t s = 0; s < t.size(); ++s) {
+                l.epoch[s * ntx + j] = t.epoch_ns[s];
+                for (int c = 0; c < 6; ++c) l.state[((size_t)c * cap + s) * ntx + j] = t.state[s * 6 + c];
+            }
+        }
+        l.sink = nyxb_traj_sink{(int64_t)cap, l.epoch.data(), l.state.data(), l.count.data()};
+        return l;
+    }
+
+    // arc.ns must be 2; estimates_capacity >= 0 also records the estimates (tags NYXB_OD_TAG), with the same filter outputs
+    ODSolution process_arcs(const std::vector<KfEstimate>& initial, const TrackingDataArc& arc, int64_t estimates_capacity = -1) const {
+        const size_t n = initial.size(), m = arc.epoch_ns.size();
+        if (arc.ns != 2 || arc.n != n || arc.obs.size() != m * 2 * n || arc.tracker.size() != m)
+            throw std::runtime_error("interlink devices need a two-slot arc (Range, Doppler) matching the filters");
+        std::vector<Spacecraft> noms; for (auto& e : initial) noms.push_back(e.nominal_state);
+        const Frame& frame = noms.at(0).frame;
+        const Links l = links(frame);
+        auto eng = detail::make_engine(prop.dynamics, frame, almanac, prop.method, prop.opts, prop.mode, prop.device);
+        detail::Soa soa(noms);
+        std::vector<double> cov0(81 * n);
+        for (size_t i = 0; i < n; ++i) for (int r = 0; r < 9; ++r) for (int c = 0; c < 9; ++c) cov0[(size_t)(c * 9 + r) * n + i] = initial[i].covar[r * 9 + c];
+        std::vector<int32_t> trk = tracker_index(arc);
+        const nyxb_od_config cfg = config();
+        nyxb_tracking_arc carc{(int64_t)m, arc.epoch_ns.data(), trk.data(), arc.obs.data()};
+        ODSolution s; s.n = n; s.m = m; s.ns = 2; s.frame = frame;
+        s.state.resize(9 * n); s.epoch.resize(n); s.covar.resize(81 * n); s.state_dev.resize(9 * n); s.resid_ratio.resize(m * 2 * n); s.prefit.resize(m * 2 * n);
+        s.postfit.resize(m * 2 * n); s.msr_flags.resize(m * n); s.details.resize(n); s.status.resize(n);
+        nyxb_od_outputs out{s.state.data(), s.epoch.data(), s.covar.data(), s.state_dev.data(), s.resid_ratio.data(), s.prefit.data(), s.postfit.data(),
+                            s.msr_flags.data(), nullptr, nullptr, s.details.data(), s.status.data()};
+        nyxb_od_records rec = detail::alloc_records(s, estimates_capacity);
+        if (nyxb_od_interlink_batch(eng.get(), &cfg, (int32_t)l.dev.size(), l.dev.data(), l.dev.size(), &l.sink, &carc, n, soa.state.data(),
+                                    soa.consts.data(), soa.epoch.data(), cov0.data(), &out, estimates_capacity >= 0 ? &rec : nullptr) != NYXB_RC_OK)
+            throw std::runtime_error(std::string("nyxb_od_interlink_batch: ") + nyxb_last_error());
+        return s;
+    }
+};
+
+inline ODSolution ODSolution::smooth(const InterlinkKalmanODProcess& odp, const TrackingDataArc& arc) const {
+    if (rec_count.empty()) throw std::runtime_error("no estimate records: run process_arcs(.., estimates_capacity)");
+    if (smoother_run) throw std::runtime_error("already smoothed");
+    auto eng = detail::make_engine(odp.prop.dynamics, frame, odp.almanac, odp.prop.method, odp.prop.opts, odp.prop.mode, odp.prop.device);
+    const InterlinkKalmanODProcess::Links l = odp.links(frame);
+    std::vector<int32_t> trk = odp.tracker_index(arc);
+    const nyxb_od_config cfg = odp.config();
+    nyxb_tracking_arc carc{(int64_t)m, arc.epoch_ns.data(), trk.data(), arc.obs.data()};
+    nyxb_od_records rec{rec_capacity, const_cast<int64_t*>(rec_epoch.data()), const_cast<int64_t*>(rec_tag.data()), const_cast<double*>(rec_nominal.data()),
+                        const_cast<double*>(rec_deviation.data()), const_cast<double*>(rec_covar.data()), const_cast<double*>(rec_stm.data()),
+                        const_cast<int64_t*>(rec_count.data())};
+    ODSolution s = *this;
+    const size_t cap = (size_t)rec_capacity;
+    s.smoother_run = true;
+    s.sm_state.resize(cap * 9 * n); s.sm_deviation.resize(cap * 9 * n); s.sm_covar.resize(cap * 81 * n); s.sm_fs_ratio.resize(cap * 9 * n);
+    s.sm_postfit.resize(cap * 2 * n); s.sm_status.resize(n);
+    nyxb_smooth_outputs out{s.sm_state.data(), s.sm_deviation.data(), s.sm_covar.data(), s.sm_fs_ratio.data(), s.sm_postfit.data(), s.sm_status.data()};
+    if (nyxb_od_interlink_smooth_batch(eng.get(), &cfg, (int32_t)l.dev.size(), l.dev.data(), l.dev.size(), &l.sink, &carc, n, &rec, status.data(),
+                                       &out) != NYXB_RC_OK)
+        throw std::runtime_error(std::string("nyxb_od_interlink_smooth_batch: ") + nyxb_last_error());
     return s;
 }
 

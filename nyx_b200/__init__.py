@@ -22,7 +22,7 @@ from .event import Event, brent, locate_event
 from .od import (BatchLeastSquares, BLSEnsembleSolution, BLSSolution, BLSSolver, GroundStation, KalmanODProcess, KalmanVariant, KfEstimate, LocalFrame, MeasurementType, ODError, ODSolution,
                  PredictionSolution, ProcessNoise3D, SigmaRejection, SpacecraftKalmanOD, SpacecraftKalmanScalarOD, SpacecraftUncertainty,
                  StochasticNoise, TrackingDataArc, simulate_tracking, station_state)
-from .od import AER_TYPES, PositionDevice, simulate_position_fixes
+from .od import AER_TYPES, InterlinkTxSpacecraft, PositionDevice, simulate_interlink, simulate_position_fixes
 from .propagator import (Engine, ErrorControl, IntegrationDetails, IntegratorMethod, IntegratorOptions, PropagationError,
                          PropInstance, Propagator)
 

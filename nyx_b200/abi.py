@@ -169,6 +169,7 @@ MSRF_PROCESSED, MSRF_REJECTED, MSRF_NOT_VISIBLE, MSRF_ABSENT = 1, 2, 4, 8
 BLS_NORMAL_EQUATIONS, BLS_LEVENBERG_MARQUARDT = 0, 1
 ERR_TOO_FEW_MEASUREMENTS, ERR_SINGULAR_INFORMATION, ERR_INVALID_MEASUREMENT = 6, 7, 8
 ERR_SINGULAR_STM, ERR_RECORDS_TRUNCATED = 9, 10
+ERR_TX_NO_DATA, ERR_NO_RANGE = 11, 12   # interlink: the transmitter's recording misses the epoch; a Doppler row without a range
 OD_TAG_TIME_UPDATE = -1   # estimate-record tags: NYXB_OD_TAG(k, w, rejected, msr_size) = ((k*2 + w)*2 + rejected)*2 + msr_size - 1
 
 
@@ -219,6 +220,17 @@ class AerStationC(C.Structure):
         ("types", C.c_int32 * 4),
         ("noise_var", C.c_double * 4),
         ("bias", C.c_double * 4),
+        ("body_radius_km", C.c_double),
+    ]
+
+
+class InterlinkTxC(C.Structure):
+    _fields_ = [
+        ("tx", C.c_int32),
+        ("n_types", C.c_int32),
+        ("types", C.c_int32 * 2),
+        ("noise_var", C.c_double * 2),
+        ("bias", C.c_double * 2),
         ("body_radius_km", C.c_double),
     ]
 
@@ -434,6 +446,13 @@ def _declare(lib):
     lib.nyxb_od_aer_smooth_batch.restype = C.c_int32
     lib.nyxb_od_aer_smooth_batch.argtypes = [vp, C.POINTER(OdConfigC), C.c_int32, C.POINTER(AerStationC), C.POINTER(TrackingArcC),
                                              C.c_size_t, C.POINTER(OdRecordsC), vp, C.POINTER(SmoothOutputsC)]
+    lib.nyxb_od_interlink_batch.restype = C.c_int32
+    lib.nyxb_od_interlink_batch.argtypes = [vp, C.POINTER(OdConfigC), C.c_int32, C.POINTER(InterlinkTxC), C.c_size_t, C.POINTER(TrajSink),
+                                            C.POINTER(TrackingArcC), C.c_size_t, vp, vp, vp, vp, C.POINTER(OdOutputsC), C.POINTER(OdRecordsC)]
+    lib.nyxb_od_interlink_smooth_batch.restype = C.c_int32
+    lib.nyxb_od_interlink_smooth_batch.argtypes = [vp, C.POINTER(OdConfigC), C.c_int32, C.POINTER(InterlinkTxC), C.c_size_t,
+                                                   C.POINTER(TrajSink), C.POINTER(TrackingArcC), C.c_size_t, C.POINTER(OdRecordsC), vp,
+                                                   C.POINTER(SmoothOutputsC)]
     lib.nyxb_od_position_batch.restype = C.c_int32
     lib.nyxb_od_position_batch.argtypes = [vp, C.POINTER(OdConfigC), C.c_int32, C.POINTER(PositionDeviceC), C.POINTER(PositionArcC),
                                            C.c_size_t, vp, vp, vp, vp, C.POINTER(OdOutputsC), C.POINTER(OdRecordsC)]
@@ -529,6 +548,8 @@ EXPORTED_SYMBOLS = [
     "nyxb_engine_set_tx_positions",
     "nyxb_abi_version",
     "nyxb_last_error",
+    "nyxb_od_interlink_batch",
+    "nyxb_od_interlink_smooth_batch",
 ]
 
 

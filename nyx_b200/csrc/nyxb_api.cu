@@ -39,6 +39,7 @@ static_assert(sizeof(nyxb_ground_station) == 176 && sizeof(nyxb_od_config) == 72
 static_assert(sizeof(nyxb_bls_config) == 80 && sizeof(nyxb_bls_outputs) == 72, "ABI layout");
 static_assert(sizeof(nyxb_od_records) == 64 && sizeof(nyxb_smooth_outputs) == 48, "ABI layout");
 static_assert(sizeof(nyxb_position_device) == 64 && sizeof(nyxb_position_arc) == 32 && sizeof(nyxb_aer_station) == 256, "ABI layout");
+static_assert(sizeof(nyxb_interlink_tx) == 56, "ABI layout");
 
 static thread_local std::string g_err;
 static void set_err(const std::string& s) { g_err = s; }
@@ -1154,12 +1155,18 @@ struct PosTags {
     static int64_t msr_size(int64_t tg) { return NYXB_OD_POS_TAG_MSR_SIZE(tg); }
     static bool outside(int w, int M, int n_types) { return w * M >= n_types; }
 };
+// interlink records: the ground station's tags, with a short last window as a station with angles
+struct LinkTags : GroundTags {
+    static bool outside(int w, int M, int n_types) { return PosTags::outside(w, M, n_types); }
+};
 
 // The common part of the two smoothing calls: the per-filter statuses decided on the host, then upload, the smoothing launch and
 // read-back.  The records of the filters left to smooth must belong to this arc and msr_size.  hs: the packed devices.
+// win_err: the status of a window that cannot be formed (the even err_key of nyxb_k_smooth).
 template <class Tags, class Dev>
 int32_t od_smooth_run(nyxb_engine* eng, int M, const std::vector<Dev>& hs, int64_t n_msr, const int32_t* arc_tracker, const double* arc_obs,
-                      size_t n, const nyxb_od_records* rec, const int32_t* filter_status, nyxb_smooth_outputs* out) {
+                      size_t n, const nyxb_od_records* rec, const int32_t* filter_status, nyxb_smooth_outputs* out,
+                      int32_t win_err = NYXB_ERR_EPHEMERIS) {
     constexpr int NS = Dev::NS;
     const size_t m = (size_t)n_msr, cap = (size_t)rec->capacity;
     const int32_t n_stations = (int32_t)hs.size();
@@ -1227,7 +1234,7 @@ int32_t od_smooth_run(nyxb_engine* eng, int M, const std::vector<Dev>& hs, int64
     // the reference's error is the first one met going backwards from the last estimate: the largest k (singular before measure);
     // the outputs of such a filter were set to NaN on the device
     for (size_t i = 0; i < n; ++i)
-        if (key[i] >= 0) out->status[i] = (key[i] & 1) ? NYXB_ERR_SINGULAR_STM : NYXB_ERR_EPHEMERIS;
+        if (key[i] >= 0) out->status[i] = (key[i] & 1) ? NYXB_ERR_SINGULAR_STM : win_err;
     return NYXB_RC_OK;
 }
 }  // namespace
@@ -1304,6 +1311,87 @@ extern "C" int32_t nyxb_od_aer_smooth_batch(nyxb_engine* eng, const nyxb_od_conf
     std::vector<DevAerStation> hs;
     if (int32_t rc = pack_aer_stations(eng, n_stations, stations, hs)) return rc;
     return od_smooth_run<PosTags>(eng, cfg->msr_size, hs, arc->n_msr, arc->tracker, arc->obs, n, rec, filter_status, out);
+}
+
+namespace {
+// The checks and packing of interlink transmitters and of their recordings (nyxb_od_interlink_batch / _smooth_batch): every column of
+// the sink holds 1 to capacity records, every device names a column and one or two distinct types of Range and Doppler.
+int32_t pack_links(int32_t n_devices, const nyxb_interlink_tx* devices, size_t n_tx, const nyxb_traj_sink* sink, std::vector<DevLink>& hs) {
+    if (!sink || sink->capacity < 0 || (n_tx > 0 && (!sink->epoch_ns || !sink->state || !sink->count))) {
+        set_err("null argument: the transmitter recordings");
+        return NYXB_RC_BAD_ARG;
+    }
+    for (size_t j = 0; j < n_tx; ++j)
+        if (sink->count[j] < 1 || sink->count[j] > sink->capacity) {
+            set_err("bad transmitter recording: count must be 1 to capacity (a recording that dropped records is incomplete)");
+            return NYXB_RC_BAD_ARG;
+        }
+    hs.assign((size_t)(n_devices > 0 ? n_devices : 0), DevLink{});
+    for (int32_t s = 0; s < n_devices; ++s) {
+        const nyxb_interlink_tx& g = devices[s];
+        if (g.n_types < 1 || g.n_types > 2) { set_err("bad interlink device: n_types must be 1 or 2"); return NYXB_RC_BAD_ARG; }
+        if (g.tx < 0 || (size_t)g.tx >= n_tx) { set_err("bad interlink device: transmitter column outside the recordings"); return NYXB_RC_BAD_ARG; }
+        for (int q = 0; q < g.n_types; ++q) {
+            if (g.types[q] != NYXB_MSR_RANGE && g.types[q] != NYXB_MSR_DOPPLER) {
+                set_err("bad interlink device: measurement types must be Range or Doppler");
+                return NYXB_RC_BAD_ARG;
+            }
+            if (q == 1 && g.types[0] == g.types[1]) { set_err("bad interlink device: duplicate measurement type"); return NYXB_RC_BAD_ARG; }
+        }
+        DevLink& d = hs[s];
+        d.tx_n = (long long)n_tx;
+        d.col = g.tx; d.n_types = g.n_types;
+        for (int q = 0; q < 2; ++q) { d.types[q] = g.types[q]; d.noise_var[q] = g.noise_var[q]; d.bias[q] = g.bias[q]; }
+        d.body_radius = g.body_radius_km;
+    }
+    return NYXB_RC_OK;
+}
+// uploads the recordings into B and points every device at them
+int32_t put_links(DevBufs& B, size_t n_tx, const nyxb_traj_sink* sink, cudaStream_t st, std::vector<DevLink>& hs) {
+    const size_t cap = (size_t)sink->capacity;
+    const NyxbTrajView tv{(long long)cap, B.put((const long long*)sink->epoch_ns, cap * n_tx, st), B.put(sink->state, 6 * cap * n_tx, st),
+                          B.put((const long long*)sink->count, n_tx, st)};
+    if (int32_t rc = B.check("device allocation / upload failed (transmitter recordings)")) return rc;
+    for (DevLink& d : hs) d.tx = tv;
+    return NYXB_RC_OK;
+}
+}  // namespace
+
+extern "C" int32_t nyxb_od_interlink_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_devices, const nyxb_interlink_tx* devices,
+                                           size_t n_tx, const nyxb_traj_sink* tx_sink, const nyxb_tracking_arc* arc, size_t n,
+                                           const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
+                                           const double* covar0_soa, const nyxb_od_outputs* out, const nyxb_od_records* rec) {
+    if (int32_t rc = filter_args<DevLink>(eng, cfg, n_devices, devices, arc, state_soa, consts_soa, epoch0_ns, covar0_soa, out, rec))
+        return rc;
+    std::vector<DevLink> hs;
+    if (int32_t rc = pack_links(n_devices, devices, n_tx, tx_sink, hs)) return rc;
+    if (n == 0) return NYXB_RC_OK;
+    cudaStream_t st;
+    if (int32_t rc = od_stream(eng, st)) return rc;
+    DevBufs B;
+    if (int32_t rc = put_links(B, n_tx, tx_sink, st, hs)) return rc;
+    return od_filter_run(eng, cfg, hs, arc->n_msr, arc->epoch_ns, arc->tracker, arc->obs, n, state_soa, consts_soa, epoch0_ns, covar0_soa,
+                         out, rec);
+}
+
+extern "C" int32_t nyxb_od_interlink_smooth_batch(nyxb_engine* eng, const nyxb_od_config* cfg, int32_t n_devices,
+                                                  const nyxb_interlink_tx* devices, size_t n_tx, const nyxb_traj_sink* tx_sink,
+                                                  const nyxb_tracking_arc* arc, size_t n, const nyxb_od_records* rec,
+                                                  const int32_t* filter_status, nyxb_smooth_outputs* out) {
+    if (!eng || !cfg || !arc || !rec || !filter_status || !out || !out->status || (n_devices > 0 && !devices) || n_devices < 0) {
+        set_err("null argument");
+        return NYXB_RC_BAD_ARG;
+    }
+    if (cfg->msr_size != 1 && cfg->msr_size != 2) { set_err("msr_size must be 1 or 2"); return NYXB_RC_BAD_ARG; }
+    if (!records_ok(rec)) return NYXB_RC_BAD_ARG;
+    if (arc->n_msr < 0 || (arc->n_msr > 0 && (!arc->tracker || !arc->obs))) { set_err("null tracking arc arrays"); return NYXB_RC_BAD_ARG; }
+    std::vector<DevLink> hs;
+    if (int32_t rc = pack_links(n_devices, devices, n_tx, tx_sink, hs)) return rc;
+    cudaStream_t st;
+    if (int32_t rc = od_stream(eng, st)) return rc;
+    DevBufs B;
+    if (int32_t rc = put_links(B, n_tx, tx_sink, st, hs)) return rc;
+    return od_smooth_run<LinkTags>(eng, cfg->msr_size, hs, arc->n_msr, arc->tracker, arc->obs, n, rec, filter_status, out, NYXB_ERR_TX_NO_DATA);
 }
 
 extern "C" int32_t nyxb_od_predict_batch(nyxb_engine* eng, const nyxb_od_config* cfg, size_t n, const double* state_soa,

@@ -106,6 +106,8 @@ template cudaError_t launch(const DevSetup&, const OdFilterJob<DevPosDevice, fal
 template cudaError_t launch(const DevSetup&, const OdFilterJob<DevPosDevice, true>&, size_t, const OdIo&, cudaStream_t);
 template cudaError_t launch(const DevSetup&, const OdFilterJob<DevAerStation, false>&, size_t, const OdIo&, cudaStream_t);
 template cudaError_t launch(const DevSetup&, const OdFilterJob<DevAerStation, true>&, size_t, const OdIo&, cudaStream_t);
+template cudaError_t launch(const DevSetup&, const OdFilterJob<DevLink, false>&, size_t, const OdIo&, cudaStream_t);
+template cudaError_t launch(const DevSetup&, const OdFilterJob<DevLink, true>&, size_t, const OdIo&, cudaStream_t);
 template cudaError_t launch(const DevSetup&, const OdPredictJob&, size_t, const OdIo&, cudaStream_t);
 template cudaError_t launch(const DevSetup&, const OdBlsJob&, size_t, const OdIo&, cudaStream_t);
 

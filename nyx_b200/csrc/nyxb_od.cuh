@@ -2,12 +2,14 @@
 // nyxb_od.cu (kernels, built STRICT and FAST) and nyxb_api.cu (host packing).
 #pragma once
 #include "nyxb_device.cuh"
+#include "nyxb_hermite.h"
 
 #define ODC_KMAX 4           // columns of the Legendre triangle per lane of a warp kernel (>= the host's deal over 32 lanes: 4 at N = 96)
 
 struct GroundTrk;            // the measurement model of each tracker kind (nyxb_od_device.cuh)
 struct PosTrk;
 struct AerTrk;
+struct LinkTrk;
 
 // NS: the observation slots of one measurement (obs is [m][NS][n])
 struct DevStation {
@@ -45,6 +47,20 @@ struct DevAerStation {
     int types[4];
     double noise_var[4], bias[4];
     double body_radius;
+};
+
+// An interlink transmitter (od/interlink): a spacecraft whose state is Traj::at of column `col` of a recording shared by every device
+// of the call (tx, tx_n columns).  Types Range / Doppler in the device's list order; the observation slot of a type is its value, as
+// for DevStation (obs is [m][2][n]); noise_var / bias per list position.
+struct DevLink {
+    static constexpr int NS = 2;
+    using Trk = LinkTrk;
+    NyxbTrajView tx;
+    long long tx_n;
+    int col, n_types;
+    int types[2];
+    double noise_var[2], bias[2];
+    double body_radius;            // the body at the integration frame's centre; <= 0: no line-of-sight test
 };
 
 // Dev: the tracker kind (DevStation, DevPosDevice for position fixes, whose observations are [m][3][n], or DevAerStation, [m][4][n])

@@ -18,6 +18,7 @@
 // Every scalar below (OdInst, h, the window, the gain inputs) is computed by every lane alike, so all lanes take the same branches.
 #pragma once
 #include <cfloat>
+#include <type_traits>
 #include "nyxb_od_device.cuh"
 
 // PropInstance scalars of one trajectory or filter (instance.rs:87-262)
@@ -284,7 +285,7 @@ __device__ __forceinline__ void od_est_push(const OdEstRecords& er, long long& c
 
 // Loads filter i, runs the whole arc and stores the final covariance, deviation, state, details and status.  REC: also write one
 // estimate record per entry of the reference's ODSolution.estimates into *er (null when REC is false); the filter's arithmetic and
-// outputs are the same either way.  TRK: the tracker kind (GroundTrk, PosTrk, AerTrk in nyxb_od_device.cuh); B::Filt's PHt and K hold
+// outputs are the same either way.  TRK: the tracker kind (GroundTrk, PosTrk, AerTrk, LinkTrk in nyxb_od_device.cuh); B::Filt's PHt and K hold
 // 9 x TRK::NS entries.
 template <class B, bool REC = false, class TRK = GroundTrk>
 __device__ void od_process_arc(const DevOdT<typename TRK::Dev>& od, B& b, size_t i, size_t n, const double* state, const double* consts, const long long* epoch0,
@@ -342,10 +343,14 @@ __device__ void od_process_arc(const DevOdT<typename TRK::Dev>& od, B& b, size_t
             const int windows = gs.n_types / M;
             for (int wno = 0; wno <= windows; ++wno) {                          // :270-398
                 typename TRK::Win w;
-                const int wrc = TRK::setup(S, gs, M, wno, o, t_k, in.y, w);
+                const int wrc = TRK::setup(S, gs, M, wno, o, t_k, epoch, in.y, w);
                 if (wrc == OD_WIN_EMPTY) break;
                 if (wrc == OD_WIN_UNAVAILABLE) continue;
                 if (wrc == OD_WIN_EPHEMERIS) { rc = NYXB_ERR_EPHEMERIS; break; }
+                if constexpr (std::is_same<TRK, LinkTrk>::value) {              // the failures only an interlink window has
+                    if (wrc == OD_WIN_TX_NO_DATA) { rc = NYXB_ERR_TX_NO_DATA; break; }
+                    if (wrc == OD_WIN_NO_RANGE) { rc = NYXB_ERR_NO_RANGE; break; }
+                }
                 if (wrc == OD_WIN_NOT_VISIBLE) { flags |= NYXB_MSRF_NOT_VISIBLE; continue; }
                 const double (&H)[NS][9] = w.H;
                 const double* Rk = w.Rk;

@@ -285,5 +285,7 @@ template cudaError_t nyxb_od_coop_launch(const DevSetup&, const OdFilterJob<DevP
 template cudaError_t nyxb_od_coop_launch(const DevSetup&, const OdFilterJob<DevPosDevice, true>&, const int*, size_t, const OdIo&, cudaStream_t);
 template cudaError_t nyxb_od_coop_launch(const DevSetup&, const OdFilterJob<DevAerStation, false>&, const int*, size_t, const OdIo&, cudaStream_t);
 template cudaError_t nyxb_od_coop_launch(const DevSetup&, const OdFilterJob<DevAerStation, true>&, const int*, size_t, const OdIo&, cudaStream_t);
+template cudaError_t nyxb_od_coop_launch(const DevSetup&, const OdFilterJob<DevLink, false>&, const int*, size_t, const OdIo&, cudaStream_t);
+template cudaError_t nyxb_od_coop_launch(const DevSetup&, const OdFilterJob<DevLink, true>&, const int*, size_t, const OdIo&, cudaStream_t);
 template cudaError_t nyxb_od_coop_launch(const DevSetup&, const OdPredictJob&, const int*, size_t, const OdIo&, cudaStream_t);
 template cudaError_t nyxb_od_coop_launch(const DevSetup&, const OdBlsJob&, const int*, size_t, const OdIo&, cudaStream_t);

@@ -251,7 +251,9 @@ struct OdWindowT {
     double H[NS][9];
 };
 using OdWindow = OdWindowT<2>;
-enum { OD_WIN_OK = 0, OD_WIN_EMPTY = 1, OD_WIN_UNAVAILABLE = 2, OD_WIN_NOT_VISIBLE = 3, OD_WIN_EPHEMERIS = 4 };
+// OD_WIN_TX_NO_DATA and OD_WIN_NO_RANGE: interlink windows only (od_link_window_setup)
+enum { OD_WIN_OK = 0, OD_WIN_EMPTY = 1, OD_WIN_UNAVAILABLE = 2, OD_WIN_NOT_VISIBLE = 3, OD_WIN_EPHEMERIS = 4, OD_WIN_TX_NO_DATA = 5,
+       OD_WIN_NO_RANGE = 6 };
 
 // St: DevStation (range, Doppler) or DevAerStation, which adds azimuth and elevation (trk_device.rs:158-208, msr/types.rs:102-117,
 // sensitivity.rs:188-226).  The observation slot of a type is its value.  The angles, in degrees, come from rho = r_sc - r_station in
@@ -377,7 +379,8 @@ __device__ static bool od_sinv(int M, const double Sk[2][2], double Si[2][2]) {
 //              the window's type in the device's list (the ratio takes slot ratio_slot(M, wno));
 // TRK::Dev     the device struct of DevOdT;
 // absent(o)    no type of the measurement is in this filter's arc;
-// setup(..)    the window (od_window_setup's contract);
+// setup(..)    the window (od_window_setup's contract) at the measurement epoch t_k, which is the nominal state's; the propagator's
+//              epoch before it was set to t_k (within epoch_precision of it) comes next, for the interlink's computed observation;
 // ratio(..)    residual ratio of filtering.rs:152-167, false on SingularNoiseRk;
 // gain_setup / gain_entry   K = P H^T S^-1 (filtering.rs:206-231): gain_setup factors S (false on SingularKalmanGain), gain_entry gives
 //              entry q of row r of K from row r of P H^T;
@@ -389,8 +392,8 @@ struct GroundTrk {
     using Win = OdWindow;
     struct Gain { double Si[2][2]; };
     __device__ __forceinline__ static bool absent(const double o[2]) { return o[0] != o[0] && o[1] != o[1]; }
-    __device__ __forceinline__ static int setup(const DevSetup& S, const Dev& gs, int M, int wno, const double o[2], long long t_k, const double y[9],
-                                Win& w) {
+    __device__ __forceinline__ static int setup(const DevSetup& S, const Dev& gs, int M, int wno, const double o[2], long long t_k, long long,
+                                const double y[9], Win& w) {
         return od_window_setup(S, gs, M, wno, o, t_k, y, w);
     }
     __device__ __forceinline__ static bool ratio(int M, const double Sk[2][2], const double Rk[2], const double pre[2], double& r) {
@@ -471,7 +474,8 @@ struct PosTrk {
     // chol: S = L L^T (M = 3), else Si: S^-1 (M <= 2: od_sinv, M = 3: the closed-form 3x3 inverse after a failed Cholesky)
     struct Gain { bool chol; double L[3][3]; double Si[3][3]; };
     __device__ __forceinline__ static bool absent(const double o[3]) { return o[0] != o[0] && o[1] != o[1] && o[2] != o[2]; }
-    __device__ __forceinline__ static int setup(const DevSetup&, const Dev& d, int M, int wno, const double o[3], long long, const double y[9], Win& w) {
+    __device__ __forceinline__ static int setup(const DevSetup&, const Dev& d, int M, int wno, const double o[3], long long, long long,
+                                const double y[9], Win& w) {
         return od_pos_window_setup(d, M, wno, o, y, w);
     }
     // M <= 2: od_ratio on the leading 2x2 block, the ground station's arithmetic
@@ -550,8 +554,8 @@ struct AerTrk {
     using Win = OdWindowT<4>;
     using Gain = GroundTrk::Gain;
     __device__ __forceinline__ static bool absent(const double o[4]) { return o[0] != o[0] && o[1] != o[1] && o[2] != o[2] && o[3] != o[3]; }
-    __device__ __forceinline__ static int setup(const DevSetup& S, const Dev& gs, int M, int wno, const double o[4], long long t_k, const double y[9],
-                                Win& w) {
+    __device__ __forceinline__ static int setup(const DevSetup& S, const Dev& gs, int M, int wno, const double o[4], long long t_k, long long,
+                                const double y[9], Win& w) {
         return od_window_setup(S, gs, M, wno, o, t_k, y, w);
     }
     __device__ __forceinline__ static bool ratio(int M, const double Sk[4][4], const double Rk[4], const double pre[4], double& r) {
@@ -568,4 +572,85 @@ struct AerTrk {
     __device__ __forceinline__ static long long tag(long long k, int wno, int rej, int M) { return PosTrk::tag(k, wno, rej, M); }
     __device__ __forceinline__ static long long tag_msr(long long tg) { return PosTrk::tag_msr(tg); }
     __device__ __forceinline__ static int tag_window(long long tg) { return PosTrk::tag_window(tg); }
+};
+
+// An interlink transmitter (DevLink; interlink/trk_device.rs:180-232, interlink/sensitivity.rs:50-172, process/mod.rs:300-330), as
+// coded.  h_tilde runs first, with the transmitter at the nominal state's epoch t_nom: dr = r_rx - r_tx, dv = v_rx - v_tx, and the
+// OBSERVED range and Doppler in the rows; identity rows for types absent from the measurement, OD_WIN_NO_RANGE for a Doppler row without
+// an observed range.  Then measure_instantaneous at the propagator's epoch t_prop: the transmitter again, the line of sight against the
+// body at the frame's centre (Vallado's SIGHT, the receiver as r1), range |rho| and range rate rho . v_rx / |rho|: the transmitter's
+// velocity is not subtracted.  A transmitter epoch outside the recording is OD_WIN_TX_NO_DATA, before any obstruction test.
+__device__ static int od_link_window_setup(const DevLink& d, int M, int wno, const double o[2], long long t_nom, long long t_prop,
+                                           const double y[9], OdWindow& w) {
+    w.ncur = 0;
+    for (int q = wno * M; q < (wno + 1) * M && q < d.n_types; ++q) w.cur[w.ncur++] = d.types[q];
+    if (w.ncur == 0) return OD_WIN_EMPTY;
+    bool any = false;
+    w.avail[0] = w.avail[1] = false;
+    for (int q = 0; q < w.ncur; ++q) { w.avail[q] = (o[w.cur[q]] == o[w.cur[q]]); any = any || w.avail[q]; }
+    if (!any) return OD_WIN_UNAVAILABLE;
+    for (int q = 0; q < 2; ++q) {
+        w.real_obs[q] = 0.0; w.Rk[q] = 0.0; w.comp[q] = 0.0;
+        for (int c = 0; c < 9; ++c) w.H[q][c] = (q == c) ? 1.0 : 0.0;
+    }
+    for (int q = 0; q < w.ncur; ++q) if (w.avail[q]) w.real_obs[q] = o[w.cur[q]];
+    double tx[6];
+    if (nyxb_traj_at(d.tx, (size_t)d.tx_n, (size_t)d.col, t_nom, tx)) return OD_WIN_TX_NO_DATA;   // `location(..).unwrap()`
+    const double dr[3] = { y[0] - tx[0], y[1] - tx[1], y[2] - tx[2] };
+    const double dv[3] = { y[3] - tx[3], y[4] - tx[4], y[5] - tx[5] };
+    for (int q = 0; q < w.ncur; ++q) {
+        if (!w.avail[q]) continue;
+        const double rho = o[NYXB_MSR_RANGE];
+        if (w.cur[q] == NYXB_MSR_DOPPLER) {
+            if (rho != rho) return OD_WIN_NO_RANGE;
+            const double rho_dot = o[NYXB_MSR_DOPPLER], rho2 = rho * rho;
+            w.H[q][0] = dv[0] / rho - rho_dot * dr[0] / rho2;
+            w.H[q][1] = dv[1] / rho - rho_dot * dr[1] / rho2;
+            w.H[q][2] = dv[2] / rho - rho_dot * dr[2] / rho2;
+            w.H[q][3] = dr[0] / rho; w.H[q][4] = dr[1] / rho; w.H[q][5] = dr[2] / rho;
+        } else {
+            w.H[q][0] = dr[0] / rho; w.H[q][1] = dr[1] / rho; w.H[q][2] = dr[2] / rho;
+            for (int c = 3; c < 9; ++c) w.H[q][c] = 0.0;
+        }
+        w.H[q][6] = 0.0; w.H[q][7] = 0.0; w.H[q][8] = 0.0;
+    }
+    if (nyxb_traj_at(d.tx, (size_t)d.tx_n, (size_t)d.col, t_prop, tx)) return OD_WIN_TX_NO_DATA;  // `self.traj.at(rx.epoch())?`
+    if (d.body_radius > 0.0) {                 // r1 = the receiver, r2 = the transmitter: od_window_setup's order for the same test
+        const double r1sq = (y[0] * y[0] + y[1] * y[1]) + y[2] * y[2];
+        const double r2sq = (tx[0] * tx[0] + tx[1] * tx[1]) + tx[2] * tx[2];
+        const double r12 = (y[0] * tx[0] + y[1] * tx[1]) + y[2] * tx[2];
+        const double tau = (r1sq - r12) / (r1sq + r2sq - 2.0 * r12);
+        if (tau >= 0.0 && tau <= 1.0 && (1.0 - tau) * r1sq + r12 * tau <= d.body_radius * d.body_radius) return OD_WIN_NOT_VISIBLE;
+    }
+    const double rho[3] = { y[0] - tx[0], y[1] - tx[1], y[2] - tx[2] };
+    const double rng = sqrt((rho[0] * rho[0] + rho[1] * rho[1]) + rho[2] * rho[2]);
+    const double rr = ((rho[0] * y[3] + rho[1] * y[4]) + rho[2] * y[5]) / rng;
+    for (int q = 0; q < w.ncur; ++q) {
+        const int slot = wno * M + q;
+        w.Rk[q] = d.noise_var[slot];
+        w.comp[q] = ((w.cur[q] == NYXB_MSR_RANGE) ? rng : rr) - d.bias[slot];
+    }
+    return OD_WIN_OK;
+}
+
+// The interlink transmitter: od_link_window_setup, and the ground station's slots, ratio, gain and record tags.
+struct LinkTrk {
+    using Dev = DevLink;
+    static constexpr int NS = Dev::NS;
+    using Win = OdWindow;
+    using Gain = GroundTrk::Gain;
+    __device__ __forceinline__ static bool absent(const double o[2]) { return GroundTrk::absent(o); }
+    __device__ __forceinline__ static int setup(const DevSetup&, const Dev& d, int M, int wno, const double o[2], long long t_k, long long t_prop,
+                                const double y[9], Win& w) {
+        return od_link_window_setup(d, M, wno, o, t_k, t_prop, y, w);
+    }
+    __device__ __forceinline__ static bool ratio(int M, const double Sk[2][2], const double Rk[2], const double pre[2], double& r) {
+        return od_ratio(M, Sk, Rk, pre, r);
+    }
+    __device__ __forceinline__ static bool gain_setup(int M, const double Sk[2][2], Gain& g) { return od_sinv(M, Sk, g.Si); }
+    __device__ __forceinline__ static double gain_entry(int M, const Gain& g, const double* pht, int q) { return GroundTrk::gain_entry(M, g, pht, q); }
+    __device__ __forceinline__ static int ratio_slot(int M, int wno) { return GroundTrk::ratio_slot(M, wno); }
+    __device__ __forceinline__ static long long tag(long long k, int wno, int rej, int M) { return GroundTrk::tag(k, wno, rej, M); }
+    __device__ __forceinline__ static long long tag_msr(long long tg) { return GroundTrk::tag_msr(tg); }
+    __device__ __forceinline__ static int tag_window(long long tg) { return GroundTrk::tag_window(tg); }
 };

@@ -9,11 +9,13 @@
 //
 // Built once, STRICT and without FMA contraction, like the host API: the 9x9 part is then bit-identical to its host build.  The same
 // kernel template serves the ground station's records (nyxb_k_smooth<GroundTrk>), those of position fixes (nyxb_k_smooth<PosTrk>) and
-// those of stations with angles (nyxb_k_smooth<AerTrk>).
+// those of stations with angles (nyxb_k_smooth<AerTrk>) and those of interlink transmitters (nyxb_k_smooth<LinkTrk>, whose transmitter is
+// interpolated at estimate k's epoch; a recording that does not cover it is the ephemeris error's key, reported as NYXB_ERR_TX_NO_DATA).
 #include "nyxb_od_device.cuh"
 #include "nyxb_smooth.h"
+#include <type_traits>
 
-// TRK: the tracker kind of the filter that wrote the records (GroundTrk, PosTrk, AerTrk; nyxb_od_device.cuh)
+// TRK: the tracker kind of the filter that wrote the records (GroundTrk, PosTrk, AerTrk, LinkTrk; nyxb_od_device.cuh)
 template <class TRK>
 __device__ __forceinline__ void smooth_one(const DevSetup& S, const DevSmoothT<typename TRK::Dev>& sm, size_t n) {
     constexpr int NS = TRK::NS;
@@ -68,8 +70,9 @@ __device__ __forceinline__ void smooth_one(const DevSetup& S, const DevSmoothT<t
 #pragma unroll
         for (int s = 0; s < NS; ++s) o[s] = sm.obs[((size_t)mk * NS + s) * n + i];
         typename TRK::Win w;
-        const int wrc = TRK::setup(S, gs, sm.msr_size, wno, o, sm.epoch[(size_t)k * n + i], ys, w);
-        if (wrc == OD_WIN_EPHEMERIS) { atomicMax(&sm.err_key[i], 2 * k); return; }
+        const long long ek = sm.epoch[(size_t)k * n + i];
+        const int wrc = TRK::setup(S, gs, sm.msr_size, wno, o, ek, ek, ys, w);
+        if (wrc == OD_WIN_EPHEMERIS || (std::is_same<TRK, LinkTrk>::value && wrc == OD_WIN_TX_NO_DATA)) { atomicMax(&sm.err_key[i], 2 * k); return; }
         if (wrc == OD_WIN_OK)
             for (int q = 0; q < w.ncur; ++q) sm.postfit[((size_t)k * NS + wno * sm.msr_size + q) * n + i] = w.real_obs[q] - w.comp[q];
     }
@@ -127,3 +130,4 @@ cudaError_t nyxb_smooth_launch(const DevSetup& S, const DevSmoothT<Dev>& sm, siz
 template cudaError_t nyxb_smooth_launch(const DevSetup&, const DevSmoothT<DevStation>&, size_t, cudaStream_t);
 template cudaError_t nyxb_smooth_launch(const DevSetup&, const DevSmoothT<DevPosDevice>&, size_t, cudaStream_t);
 template cudaError_t nyxb_smooth_launch(const DevSetup&, const DevSmoothT<DevAerStation>&, size_t, cudaStream_t);
+template cudaError_t nyxb_smooth_launch(const DevSetup&, const DevSmoothT<DevLink>&, size_t, cudaStream_t);

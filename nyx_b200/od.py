@@ -11,6 +11,8 @@
 * ``KalmanODProcess``          od/process/{initializers.rs:60-113, mod.rs:128-497}; `predict_until` / `predict_for` mod.rs:440-496;
                                `SpacecraftKalmanOD` = MsrSize 2,
                                `SpacecraftKalmanScalarOD` = MsrSize 1 (od/mod.rs:77-91)
+* ``InterlinkTxSpacecraft``    od/interlink/{trk_device.rs:37-260, sensitivity.rs:50-172}: spacecraft-to-spacecraft range and Doppler
+                               through ``nyxb_od_interlink_batch``
 * ``BatchLeastSquares``        od/blse/mod.rs:30-541 (``BLSSolver``, ``BLSSolution``; `estimate` / `evaluate` through
                                ``nyxb_od_bls_batch`` / ``nyxb_od_bls_evaluate_batch``, n problems in one launch)
 
@@ -225,6 +227,71 @@ class PositionDevice:
             d.noise_var[i] = self.stochastic_noises[t].covariance()
             d.bias[i] = self.stochastic_noises[t].bias_constant
         return d
+
+
+@dataclass
+class InterlinkTxSpacecraft:
+    """`InterlinkTxSpacecraft` (od/interlink/trk_device.rs:37-260): a transmitter spacecraft known by its recorded trajectory `traj`,
+    measuring the range and Doppler of the filtered spacecraft (the receiver).  The filter runs through nyxb_od_interlink_batch, with
+    the reference's as-coded quirks (include/nyxb.h, nyxb_interlink_tx): the computed Doppler ignores the transmitter's velocity, the
+    sensitivity rows use the observed range and Doppler, and an epoch outside `traj` ends the filter.  Only instantaneous measurements
+    without aberration correction, with `traj` in the integration frame of the estimates."""
+
+    traj: "Traj"
+    measurement_types: Sequence[MeasurementType]
+    stochastic_noises: Dict[MeasurementType, StochasticNoise]
+    integration_time: Optional[int] = None
+    ab_corr: Optional[object] = None
+
+    def name(self) -> str:
+        """trk_device.rs:93-95: the trajectory's name, or "unnamed"."""
+        return self.traj.name if self.traj.name is not None else "unnamed"
+
+    def to_c(self, tx: int, integration_frame: Frame) -> abi.InterlinkTxC:
+        """The device for nyxb_od_interlink_batch, its transmitter in column `tx` of the recordings."""
+        if self.integration_time is not None:
+            raise ODError("interlink: integrated (two-way) measurements are not supported on the GPU path")
+        if self.ab_corr is not None:
+            raise ODError("interlink: aberration correction is not supported on the GPU path (ab_corr must be None)")
+        fr = self.traj.template.orbit.frame
+        if fr.ephemeris_id != integration_frame.ephemeris_id or fr.rotation != integration_frame.rotation:
+            raise ODError(f"interlink: the transmitter's trajectory is in {fr.name}, the estimates in {integration_frame.name}")
+        if len(self.traj) == 0:
+            raise ODError("interlink: the transmitter's trajectory is empty")
+        types = [MeasurementType(t) for t in self.measurement_types]
+        if not 1 <= len(types) <= 2 or len(set(types)) != len(types) or any(t not in (MeasurementType.Range, MeasurementType.Doppler)
+                                                                               for t in types):
+            raise ODError("an interlink carries one or two of {Range, Doppler}")
+        d = abi.InterlinkTxC()
+        d.tx = int(tx)
+        d.n_types = len(types)
+        for i, t in enumerate(types):
+            if t not in self.stochastic_noises:
+                raise ODError(f"NoiseNotConfigured: {t.name}")
+            d.types[i] = int(t)
+            d.noise_var[i] = self.stochastic_noises[t].covariance()
+            d.bias[i] = self.stochastic_noises[t].bias_constant
+        try:
+            d.body_radius_km = integration_frame.mean_equatorial_radius_km()
+        except ValueError as e:
+            raise ODError(f"interlink: the line-of-sight test needs the radius of the integration frame's body ({e})") from None
+        return d
+
+
+def interlink_sink(trajs: Sequence["Traj"]):
+    """The transmitter recordings of nyxb_od_interlink_batch: (TrajSink, n_tx, arrays kept alive), column j = trajs[j], ascending."""
+    n_tx = len(trajs)
+    cap = max((len(t) for t in trajs), default=0)
+    epoch = np.zeros((cap, n_tx), dtype=np.int64)
+    state = np.zeros((6, cap, n_tx))
+    count = np.zeros(n_tx, dtype=np.int64)
+    for j, t in enumerate(trajs):
+        k = len(t)
+        epoch[:k, j] = t.epochs_ns
+        state[:, :k, j] = np.asarray(t.states, dtype=np.float64)[:, :6].T
+        count[j] = k
+    sink = abi.TrajSink(cap, epoch.ctypes.data, state.ctypes.data, count.ctypes.data)
+    return sink, n_tx, (epoch, state, count)
 
 
 @dataclass
@@ -615,8 +682,9 @@ class ODSolution:
             if res[p] is None:
                 continue
             mk, w, _, _ = self._tag_fields(int(rec["tag"][src, index]))
-            tracker[p] = self.arc.tracker[mk] if self.arc is not None else None
-            dev = (self.devices or {}).get(tracker[p])
+            key = self.arc.tracker[mk] if self.arc is not None else None
+            tracker[p] = self._tracker_name(key) if key is not None else None
+            dev = (self.devices or {}).get(key)
             tl = list(dev.measurement_types) if dev is not None else [MeasurementType.Range, MeasurementType.Doppler]
             types[p] = [int(t) for t in tl[w * M:(w + 1) * M]]
         for label, j in (("Prefit residual", 0), ("Postfit residual", 1)):
@@ -674,6 +742,11 @@ class ODSolution:
         rd = [(MeasurementType.Range, "km"), (MeasurementType.Doppler, "km/s")]
         return rd + [(MeasurementType.Azimuth, "deg"), (MeasurementType.Elevation, "deg")] if self._is_aer() else rd
 
+    def _tracker_name(self, key: str) -> str:
+        """The "Tracker" of a residual: the device's name, which for an interlink is its trajectory's name (export.rs)."""
+        dev = (self.devices or {}).get(key)
+        return dev.name() if isinstance(dev, InterlinkTxSpacecraft) else key
+
     def _need_records(self):
         if self.records is None:
             raise ODError("no estimate records: run process_arcs(.., estimates_capacity=K)")
@@ -694,7 +767,9 @@ class ODSolution:
             return None
         names = {abi.ERR_TOO_FEW_MEASUREMENTS: "TooFewMeasurements: fewer than two estimates",
                  abi.ERR_SINGULAR_STM: "SingularStateTransitionMatrix", abi.ERR_RECORDS_TRUNCATED: "estimate records truncated",
-                 abi.ERR_EPHEMERIS: "epoch outside ephemeris coverage"}
+                 abi.ERR_EPHEMERIS: "epoch outside ephemeris coverage",
+                 abi.ERR_TX_NO_DATA: "ODTrajError: the interlink transmitter's trajectory does not cover the epoch",
+                 abi.ERR_NO_RANGE: "MeasurementSimError: Range measurement data is missing"}
         return names.get(st, f"status {st}")
 
     def estimate(self, k: int, i: int) -> KfEstimate:
@@ -782,6 +857,10 @@ class ODSolution:
             names, dev_c = odp.position_devices_c()
             tracker = np.array([names.index(t) if t in names else -1 for t in self.arc.tracker], dtype=np.int32)
             sm = eng.od_position_smooth_batch(odp.config_c(), len(names), dev_c, tracker, self.arc.obs, rec, self.status)
+        elif odp.is_interlink:
+            names, dev_c, sink = odp.interlink_c(frame)
+            tracker = np.array([names.index(t) if t in names else -1 for t in self.arc.tracker], dtype=np.int32)
+            sm = eng.od_interlink_smooth_batch(odp.config_c(), len(names), dev_c, sink, tracker, self.arc.obs, rec, self.status)
         elif self.arc.is_aer:
             names, st_c = odp.aer_stations_c(frame)
             tracker = np.array([names.index(t) if t in names else -1 for t in self.arc.tracker], dtype=np.int32)
@@ -858,7 +937,7 @@ class ODSolution:
         schema.append(pa.field("Residual ratio", pa.float64(), nullable=True))
         cols.append(pa.array((self.msr_flags[rows, index] & abi.MSRF_REJECTED) != 0, type=pa.bool_()))
         schema.append(pa.field("Residual Rejected", pa.bool_(), nullable=True))
-        cols.append(pa.array([self.arc.tracker[r] for r in rows], type=pa.string()))
+        cols.append(pa.array([self._tracker_name(self.arc.tracker[r]) for r in rows], type=pa.string()))
         schema.append(pa.field("Tracker", pa.string(), nullable=True))
         meta = {"Purpose": "Orbit determination results"}
         meta.update(metadata or {})
@@ -989,13 +1068,35 @@ class KalmanODProcess:
             c.snc_disable_time_ns = int(snc.disable_time)
         return c
 
+    def _kinds(self):
+        kinds = {type(d) for d in self.devices.values()}
+        if len(kinds) > 1:
+            raise ODError("mixed tracker kinds: all devices must be GroundStations, all PositionDevices or all InterlinkTxSpacecraft")
+        return kinds
+
     @property
     def is_position(self) -> bool:
         """True for a filter over PositionDevices; the reference's `Trk` is one type, so the kinds are never mixed."""
-        kinds = {type(d) for d in self.devices.values()}
-        if len(kinds) > 1:
-            raise ODError("mixed tracker kinds: all devices must be GroundStations or all PositionDevices")
-        return kinds == {PositionDevice}
+        return self._kinds() == {PositionDevice}
+
+    @property
+    def is_interlink(self) -> bool:
+        """True for a filter over InterlinkTxSpacecraft (never mixed with another kind)."""
+        return self._kinds() == {InterlinkTxSpacecraft}
+
+    def interlink_c(self, frame: Frame):
+        """(names, devices, recordings) for nyxb_od_interlink_batch: one recording column per distinct trajectory."""
+        names = list(self.devices)
+        trajs: List = []
+        arr = (abi.InterlinkTxC * max(len(names), 1))()
+        for i, nme in enumerate(names):
+            t = self.devices[nme].traj
+            col = next((j for j, u in enumerate(trajs) if u is t), None)
+            if col is None:
+                col = len(trajs)
+                trajs.append(t)
+            arr[i] = self.devices[nme].to_c(col, frame)
+        return names, arr, interlink_sink(trajs)
 
     def position_devices_c(self):
         names = list(self.devices)
@@ -1024,7 +1125,8 @@ class KalmanODProcess:
         `estimates_capacity` K, the first K entries of each filter's ODSolution.estimates are recorded (1 456 bytes each), which
         `ODSolution.smooth()`, `residuals`, the RMS statistics and the per-estimate parquet export need; the filter's results do not
         change.  Ground stations run through nyxb_od_aer_batch exactly when the arc's types are AER_TYPES (range, Doppler, azimuth,
-        elevation); stations that measure angles need such an arc."""
+        elevation); stations that measure angles need such an arc.  InterlinkTxSpacecraft devices run through
+        nyxb_od_interlink_batch over a (Range, Doppler) arc."""
         n = len(initial_estimates)
         if arc.n != n:
             raise ODError(f"arc carries {arc.n} observation sets for {n} filters")
@@ -1045,6 +1147,15 @@ class KalmanODProcess:
             tracker = np.array([names.index(t) if t in names else -1 for t in arc.tracker], dtype=np.int32)
             res = eng.od_position_batch(self.config_c(), len(names), dev_c, arc.epoch_ns, tracker, arc.obs, st, cs, ep, cov0,
                                         record_estimates=record_estimates, estimates_capacity=estimates_capacity)
+        elif self.is_interlink:
+            if self.msr_size == 3:
+                raise ODError("msr_size 3 needs position devices")
+            if tuple(arc.types) != (MeasurementType.Range, MeasurementType.Doppler):
+                raise ODError("interlink devices need a tracking arc of types (Range, Doppler)")
+            names, dev_c, sink = self.interlink_c(frame)
+            tracker = np.array([names.index(t) if t in names else -1 for t in arc.tracker], dtype=np.int32)
+            res = eng.od_interlink_batch(self.config_c(), len(names), dev_c, sink, arc.epoch_ns, tracker, arc.obs, st, cs, ep, cov0,
+                                         record_estimates=record_estimates, estimates_capacity=estimates_capacity)
         else:
             if self.msr_size == 3:
                 raise ODError("msr_size 3 needs position devices")
@@ -1203,6 +1314,8 @@ class BatchLeastSquares:
                  lm_lambda_min: float = 1e-12, lm_lambda_max: float = 1e12, lm_use_diag_scaling: bool = True):
         if any(isinstance(d, PositionDevice) for d in devices.values()):
             raise ODError("batch least squares takes ground stations only")
+        if any(isinstance(d, InterlinkTxSpacecraft) for d in devices.values()):
+            raise ODError("batch least squares does not take interlink devices on the GPU path")
         if any(d.has_angles for d in devices.values()):
             raise ODError("batch least squares takes range and Doppler only, not azimuth or elevation")
         self.prop = prop
@@ -1366,3 +1479,41 @@ def simulate_position_fixes(truth_epochs_ns, truth_states, devices: Dict[str, Po
             noise = rng.normal(0.0, nz.sigma, n) if rng is not None else 0.0
             obs[k, int(t) - abi.MSR_X, :] = (truth_states[k, ii, :] + noise) + nz.bias_constant
     return TrackingDataArc(np.asarray(truth_epochs_ns, dtype=np.int64), list(schedule), obs, _POSITION_TYPES)
+
+
+def interlink_geometry(tx_rv, rx_rv):
+    """(range, range rate) of the receiver states rx_rv ([6][n]) seen from the transmitter states tx_rv ([6][n]) as the reference
+    computes them (interlink/trk_device.rs:195-210): rho = r_rx - r_tx and rho . v_rx / |rho|, the transmitter's velocity left out."""
+    rho = rx_rv[:3] - tx_rv[:3]
+    rng_km = np.sqrt((rho[0] * rho[0] + rho[1] * rho[1]) + rho[2] * rho[2])
+    return rng_km, ((rho[0] * rx_rv[3] + rho[1] * rx_rv[4]) + rho[2] * rx_rv[5]) / rng_km
+
+
+def simulate_interlink(truth_epochs_ns, truth_states, devices: Dict[str, InterlinkTxSpacecraft], schedule: Sequence[str], frame: Frame,
+                       rng: Optional[np.random.Generator] = None) -> TrackingDataArc:
+    """Synthetic interlink observations of the receivers `truth_states[k]` ([m][6][n], integration frame) at `truth_epochs_ns[k]`
+    from transmitter `schedule[k]`, with the reference simulator's geometry (measure_instantaneous, interlink/trk_device.rs:180-232):
+    the transmitter is `traj.at(epoch)`, the link is blocked by the body at the frame's centre (Vallado's SIGHT), and the Doppler
+    ignores the transmitter's velocity, so these data agree with the filter's computed observation.  White noise of each type's sigma
+    and the constant bias when `rng` is given.  Blocked links are NaN (absent).  Returns a (Range, Doppler) arc.  Host-side test data,
+    not a GPU simulator."""
+    truth_states = np.asarray(truth_states, dtype=np.float64)
+    m, _, n = truth_states.shape
+    radius = frame.mean_equatorial_radius_km()
+    obs = np.full((m, 2, n), np.nan)
+    for k in range(m):
+        dev = devices[schedule[k]]
+        tx = dev.traj.at(int(truth_epochs_ns[k])).orbit.to_cartesian_pos_vel()
+        r1 = truth_states[k, :3, :]                          # receiver first, as the ground station's test
+        r2 = np.asarray(tx[:3], dtype=np.float64)[:, None] * np.ones((1, n))
+        r1sq, r2sq, r12 = (r1[0] * r1[0] + r1[1] * r1[1]) + r1[2] * r1[2], (r2[0] * r2[0] + r2[1] * r2[1]) + r2[2] * r2[2], \
+            (r1[0] * r2[0] + r1[1] * r2[1]) + r1[2] * r2[2]
+        tau = (r1sq - r12) / (r1sq + r2sq - 2.0 * r12)
+        blocked = (tau >= 0.0) & (tau <= 1.0) & ((1.0 - tau) * r1sq + r12 * tau <= radius * radius)
+        rng_km, rr = interlink_geometry(np.asarray(tx, dtype=np.float64)[:, None] * np.ones((1, n)), truth_states[k, :6, :])
+        for t in dev.measurement_types:
+            t = MeasurementType(t)
+            nz = dev.stochastic_noises[t]
+            noise = rng.normal(0.0, nz.sigma, n) + nz.bias_constant if rng is not None else 0.0
+            obs[k, int(t), :] = np.where(blocked, np.nan, (rng_km if t == MeasurementType.Range else rr) + noise)
+    return TrackingDataArc(np.asarray(truth_epochs_ns, dtype=np.int64), list(schedule), obs)

@@ -428,8 +428,17 @@ class Engine:
         return self._od_slots_batch("nyxb_od_aer_batch", abi.TrackingArcC, 4, cfg_c, n_stations, stations_c, msr_epoch_ns, msr_tracker,
                                     obs, state_soa, consts_soa, epoch0_ns, covar0_soa, record_estimates, estimates_capacity)
 
+    def od_interlink_batch(self, cfg_c, n_devices, devices_c, tx_sink, msr_epoch_ns, msr_tracker, obs, state_soa, consts_soa, epoch0_ns,
+                           covar0_soa, record_estimates: bool = False, estimates_capacity: Optional[int] = None):
+        """`nyxb_od_interlink_batch`: od_ekf_batch's contract for interlink transmitters (nyxb_interlink_tx) whose recordings are
+        `tx_sink` (interlink_sink's (sink, n_tx, arrays)): obs [m][2][n], slot = type; per-measurement outputs [m][2][n]."""
+        sink_c, n_tx, _keep = tx_sink
+        return self._od_slots_batch("nyxb_od_interlink_batch", abi.TrackingArcC, 2, cfg_c, n_devices, devices_c, msr_epoch_ns, msr_tracker,
+                                    obs, state_soa, consts_soa, epoch0_ns, covar0_soa, record_estimates, estimates_capacity,
+                                    extra=(n_tx, C.byref(sink_c)))
+
     def _od_slots_batch(self, fn, arc_cls, ns, cfg_c, n_devices, devices_c, msr_epoch_ns, msr_tracker, obs, state_soa, consts_soa,
-                        epoch0_ns, covar0_soa, record_estimates, estimates_capacity):
+                        epoch0_ns, covar0_soa, record_estimates, estimates_capacity, extra=()):
         from .od import ODSolution
 
         state_soa = np.ascontiguousarray(state_soa, dtype=np.float64)
@@ -461,7 +470,7 @@ class Engine:
         if estimates_capacity is not None:
             records, rec_c = _od_records(int(estimates_capacity), n)
             rec_p = C.byref(rec_c)
-        rc = getattr(self._lib, fn)(self._h, C.byref(cfg_c), int(n_devices), devices_c, C.byref(arc), n, state_soa.ctypes.data,
+        rc = getattr(self._lib, fn)(self._h, C.byref(cfg_c), int(n_devices), devices_c, *extra, C.byref(arc), n, state_soa.ctypes.data,
                                     consts_soa.ctypes.data, epoch0_ns.ctypes.data, covar0_soa.ctypes.data, C.byref(out), rec_p)
         if rc != 0:
             raise PropagationError(f"{fn} rc={rc}: {abi.last_error()}")
@@ -479,7 +488,13 @@ class Engine:
         return self._od_slots_smooth("nyxb_od_aer_smooth_batch", abi.TrackingArcC, 4, cfg_c, n_stations, stations_c, msr_tracker, obs,
                                      records, filter_status, outputs)
 
-    def _od_slots_smooth(self, fn, arc_cls, ns, cfg_c, n_devices, devices_c, msr_tracker, obs, records, filter_status, outputs):
+    def od_interlink_smooth_batch(self, cfg_c, n_devices, devices_c, tx_sink, msr_tracker, obs, records: dict, filter_status, outputs=None):
+        """`nyxb_od_interlink_smooth_batch`: od_smooth_batch for the records of od_interlink_batch, with the same transmitter recordings."""
+        sink_c, n_tx, _keep = tx_sink
+        return self._od_slots_smooth("nyxb_od_interlink_smooth_batch", abi.TrackingArcC, 2, cfg_c, n_devices, devices_c, msr_tracker, obs,
+                                     records, filter_status, outputs, extra=(n_tx, C.byref(sink_c)))
+
+    def _od_slots_smooth(self, fn, arc_cls, ns, cfg_c, n_devices, devices_c, msr_tracker, obs, records, filter_status, outputs, extra=()):
         msr_tracker = np.ascontiguousarray(msr_tracker, dtype=np.int32)
         obs = np.ascontiguousarray(obs, dtype=np.float64)
         filter_status = np.ascontiguousarray(filter_status, dtype=np.int32)
@@ -495,7 +510,7 @@ class Engine:
         out = abi.SmoothOutputsC(*(r[k].ctypes.data if k in r else None for k in ("state", "deviation", "covar", "fs_ratio", "postfit")),
                                  r["status"].ctypes.data)
         arc = arc_cls(m, None, msr_tracker.ctypes.data, obs.ctypes.data)
-        rc = getattr(self._lib, fn)(self._h, C.byref(cfg_c), int(n_devices), devices_c, C.byref(arc), n, C.byref(rec_c),
+        rc = getattr(self._lib, fn)(self._h, C.byref(cfg_c), int(n_devices), devices_c, *extra, C.byref(arc), n, C.byref(rec_c),
                                     filter_status.ctypes.data, C.byref(out))
         if rc != 0:
             raise PropagationError(f"{fn} rc={rc}: {abi.last_error()}")
