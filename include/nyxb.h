@@ -214,6 +214,10 @@ enum nyxb_status {
                                           (interlink/trk_device.rs:180-183, sensitivity.rs:93-101) */
     NYXB_ERR_NO_RANGE = 12,            /* ODError::MeasurementSimError: an interlink Doppler row without an observed range in the same
                                           measurement (interlink/sensitivity.rs:105-110) */
+    NYXB_ERR_TGT_TOO_MANY_ITERATIONS = 13,     /* TargetingError::TooManyIterations (raphson_finite_diff.rs:746) */
+    NYXB_ERR_TGT_CORRECTION_INEFFECTIVE = 14,  /* TargetingError::CorrectionIneffective: | |err| - previous |err| | < 1e-10 */
+    NYXB_ERR_TGT_SINGULAR_JACOBIAN = 15,       /* TargetingError::SingularJacobian: the pseudo-inverse's m x m inverse failed */
+    NYXB_ERR_TGT_NON_FINITE = 16,              /* an objective value or Jacobian entry that is not finite (anise's partial_for fails) */
     NYXB_WARN_MAX_ATTEMPTS = 0x100 /* OR-ed flag: instance.rs:440-445 (warn only) */
 };
 
@@ -825,6 +829,73 @@ int32_t nyxb_mvn_sample_dev(int32_t device, uint64_t seed, uint64_t first_index,
 int32_t nyxb_reference_normals(uint64_t seed_lo, uint64_t seed_hi, uint64_t skip, size_t n, double* out_z);
 int32_t nyxb_pcg64mcg_u64(uint64_t seed_lo, uint64_t seed_hi, size_t n, uint64_t* out);   /* raw generator output (known-answer tests) */
 int32_t nyxb_ziggurat_tables(double* x257, double* f257);                                  /* the layer tables (inspection) */
+
+/* ---- Impulsive differential correction: `Targeter::try_achieve_from` / `try_achieve_fd` (md/opti/raphson_finite_diff.rs:41-747)
+ * restricted to impulsive variables, for n problems that share the correction and achievement epochs. */
+enum nyxb_tgt_vary { NYXB_VARY_POSITION_X = 0, NYXB_VARY_POSITION_Y = 1, NYXB_VARY_POSITION_Z = 2,
+                     NYXB_VARY_VELOCITY_X = 3, NYXB_VARY_VELOCITY_Y = 4, NYXB_VARY_VELOCITY_Z = 5 };
+/* Objective parameters: the orbital elements, evaluated with mu = nyxb_dynamics.mu_central_km3_s2 (angles in degrees) */
+enum nyxb_tgt_param {
+    NYXB_TGT_X = 0, NYXB_TGT_Y, NYXB_TGT_Z, NYXB_TGT_VX, NYXB_TGT_VY, NYXB_TGT_VZ, NYXB_TGT_RMAG, NYXB_TGT_VMAG, NYXB_TGT_SMA,
+    NYXB_TGT_ECC, NYXB_TGT_INC, NYXB_TGT_RAAN, NYXB_TGT_AOP, NYXB_TGT_TA, NYXB_TGT_AOL, NYXB_TGT_TLONG, NYXB_TGT_PERIOD,
+    NYXB_TGT_ENERGY, NYXB_TGT_HMAG, NYXB_TGT_APOAPSIS, NYXB_TGT_PERIAPSIS, NYXB_TGT_C3, NYXB_TGT_DECLINATION,
+    NYXB_TGT_N_PARAMS
+};
+/* Correction frame of the variables: none (inertial, r and v), VNC (columns v^, h^, v^ x h^) or RIC (columns r^, h^ x r^, h^),
+ * each the local-to-inertial DCM of the state the correction is applied to. */
+enum nyxb_tgt_frame { NYXB_TGT_FRAME_NONE = 0, NYXB_TGT_FRAME_VNC = 1, NYXB_TGT_FRAME_RIC = 2 };
+
+typedef struct {                /* `Variable` (md/opti/target_variable.rs) */
+    int32_t component;          /* enum nyxb_tgt_vary */
+    int32_t pad;
+    double perturbation;        /* finite and nonzero */
+    double init_guess;
+    double max_step;            /* >= 0 */
+    double max_value;           /* >= 0 */
+    double min_value;           /* <= max_value */
+} nyxb_tgt_variable;            /* 48 bytes */
+
+typedef struct {                /* `Objective` (md/objective.rs) */
+    int32_t parameter;          /* enum nyxb_tgt_param */
+    int32_t pad;
+    double desired;
+    double tolerance;
+    double multiplicative_factor;
+    double additive_factor;
+} nyxb_tgt_objective;           /* 40 bytes */
+
+typedef struct {
+    int32_t n_vars;             /* 1..6; duplicate components are allowed and add up */
+    int32_t n_objs;             /* 1..6 */
+    int32_t correction_frame;   /* enum nyxb_tgt_frame; a position variable with a frame is NYXB_RC_BAD_ARG (FrameError) */
+    int32_t iterations;         /* >= 0: at most iterations + 1 nominal evaluations */
+    nyxb_tgt_variable vars[6];
+    nyxb_tgt_objective objs[6];
+} nyxb_target_config;           /* 544 bytes */
+
+/* Problem i propagates state i from epoch0_ns[i] to correction_epoch_ns, applies the initial guesses, then iterates: the nominal and
+ * one perturbed state per variable are propagated to achievement_epoch_ns (from opts.init_step), the objectives are evaluated and the
+ * step J^+ err is clipped and applied, as the reference does.  The reference repeats the perturbed propagations once per objective;
+ * they are deterministic, so each runs once per iteration here.
+ *   out_corrected_soa [9][n]: the start state at the correction epoch plus the total correction, applied once with the DCM of that
+ *                             start state (not the iterated state; the two differ with a frame and several iterations)
+ *   out_achieved_soa  [9][n]: the nominal final state of the last iteration, with the start state's mass and coefficients
+ *   out_correction [n_vars][n], out_errors [n_objs][n], out_iterations [n]: the last iteration's values, also on failure
+ *   out_status [n]: 0 converged, NYXB_ERR_TGT_*, or the status of a failed propagation (the reference panics when a perturbed one
+ *                   fails); the warn flag of every propagation of the problem is OR-ed in.  The batch is never aborted.
+ * One kernel family and lane count is picked for the whole call, at the size of the first iteration's launch (n (n_vars + 1)), so a
+ * problem's result does not depend on how many others still iterate.  Launches: 3 before the loop, then 4 per iteration (staging of
+ * the (n_vars + 1) start states, one propagation over every active problem, the update, the stable compaction of the active
+ * problems), then 1 to write the outputs; each iteration reads back 4 bytes (the active count).
+ * NYXB_RC_BAD_ARG before any launch: counts out of range, an unknown component, parameter or frame, a position variable with a frame,
+ * max_step < 0, max_value < 0, min_value > max_value, a zero or non-finite perturbation, iterations < 0, NULL pointers.
+ * NYXB_RC_UNSUPPORTED: an integration frame other than the states' own (opts.state_center != 0).  HOST pointers everywhere. */
+int32_t nyxb_target_batch(nyxb_engine* eng, const nyxb_target_config* cfg, size_t n,
+                          const double* state_soa, const double* consts_soa, const int64_t* epoch0_ns,
+                          int64_t correction_epoch_ns, int64_t achievement_epoch_ns,
+                          double* out_corrected_soa, double* out_achieved_soa,
+                          double* out_correction, double* out_errors,
+                          int32_t* out_iterations, int32_t* out_status);
 
 /* Tuning / introspection. */
 /* Kernel families behind nyxb_propagate_batch*.  AUTO picks by mode, degree and ensemble size:

@@ -1050,4 +1050,143 @@ class BatchLeastSquares {
     }
 };
 
+// ---- Impulsive targeting: Targeter::try_achieve_from (md/opti/targeter.rs, raphson_finite_diff.rs:41-747) over nyxb_target_batch.
+// Only the impulsive components run (PositionX..VelocityZ); objectives are the nyxb_tgt_param elements.
+enum class Vary : int32_t { PositionX = NYXB_VARY_POSITION_X, PositionY = NYXB_VARY_POSITION_Y, PositionZ = NYXB_VARY_POSITION_Z,
+                            VelocityX = NYXB_VARY_VELOCITY_X, VelocityY = NYXB_VARY_VELOCITY_Y, VelocityZ = NYXB_VARY_VELOCITY_Z };
+enum class TargetFrame : int32_t { None = NYXB_TGT_FRAME_NONE, VNC = NYXB_TGT_FRAME_VNC, RIC = NYXB_TGT_FRAME_RIC };
+
+// Variable with the reference's defaults for the impulsive components (target_variable.rs:219-244)
+struct Variable {
+    Vary component = Vary::VelocityX;
+    double perturbation = 0.0001, init_guess = 0.0, max_step = 0.2, max_value = 5.0, min_value = -5.0;
+    static Variable from(Vary v) { Variable x; x.component = v; return x; }
+};
+
+// Objective (md/objective.rs); `parameter` is an enum nyxb_tgt_param
+struct Objective {
+    int32_t parameter = NYXB_TGT_SMA;
+    double desired_value = 0.0, tolerance = 1e-3, multiplicative_factor = 1.0, additive_factor = 0.0;
+    // default_event_precision (md/param.rs:74-89): 0.1 s for the period, 1e-3 otherwise
+    static Objective new_(int32_t p, double desired) { return within_tolerance(p, desired, p == NYXB_TGT_PERIOD ? 0.1 : 1e-3); }
+    static Objective within_tolerance(int32_t p, double desired, double tol) { Objective o; o.parameter = p; o.desired_value = desired; o.tolerance = tol; return o; }
+};
+
+// TargetingError (md/opti/mod.rs): `variant` is the reference's variant name, `status` the nyxb status
+struct TargetingError : std::runtime_error {
+    std::string variant; int32_t status;
+    TargetingError(std::string v, int32_t st, const std::string& msg) : std::runtime_error(v + ": " + msg), variant(std::move(v)), status(st) {}
+};
+
+struct TargeterSolution {  // md/opti/solution.rs:33-50
+    Spacecraft corrected_state, achieved_state;
+    std::vector<double> correction, achieved_errors;
+    int32_t iterations = 0;
+};
+
+// every problem of one nyxb_target_batch call: [9][n], [n_vars][n], [n_objs][n], [n] (the last iteration's values on failure)
+struct TargeterEnsembleSolution {
+    std::vector<Spacecraft> states; int64_t correction_epoch_ns = 0, achievement_epoch_ns = 0; size_t n_vars = 0, n_objs = 0;
+    std::vector<double> corrected, achieved, correction, errors; std::vector<int32_t> iterations, status;
+    size_t size() const { return states.size(); }
+    // nullopt when problem i converged, else the variant try_achieve_from throws
+    std::optional<std::string> error(size_t i) const {
+        switch (status[i] & 0xFF) {
+            case 0: return std::nullopt;
+            case NYXB_ERR_TGT_TOO_MANY_ITERATIONS: return std::string("TooManyIterations");
+            case NYXB_ERR_TGT_CORRECTION_INEFFECTIVE: return std::string("CorrectionIneffective");
+            case NYXB_ERR_TGT_SINGULAR_JACOBIAN: return std::string("SingularJacobian");
+            case NYXB_ERR_TGT_NON_FINITE: return std::string("NonFinite");
+            default: return std::string("PropError");
+        }
+    }
+    TargeterSolution solution(size_t i) const {
+        if (auto e = error(i)) {
+            if ((status[i] & 0xFF) < NYXB_ERR_TGT_TOO_MANY_ITERATIONS) throw PropagationError(status[i]);
+            throw TargetingError(*e, status[i], "problem " + std::to_string(i));
+        }
+        const size_t n = size();
+        TargeterSolution s;
+        s.corrected_state = detail::unpack(states[i], corrected, std::vector<int64_t>(n, correction_epoch_ns), n, i);
+        s.achieved_state = detail::unpack(states[i], achieved, std::vector<int64_t>(n, achievement_epoch_ns), n, i);
+        for (size_t j = 0; j < n_vars; ++j) s.correction.push_back(correction[j * n + i]);
+        for (size_t j = 0; j < n_objs; ++j) s.achieved_errors.push_back(errors[j * n + i]);
+        s.iterations = iterations[i];
+        return s;
+    }
+};
+
+class Targeter {
+  public:
+    Propagator prop; std::vector<Variable> variables; std::vector<Objective> objectives;
+    int32_t iterations = 100; TargetFrame correction_frame = TargetFrame::None; const Almanac* almanac = nullptr;
+
+    static Targeter new_(Propagator p, std::vector<Variable> v, std::vector<Objective> o) { Targeter t; t.prop = std::move(p); t.variables = std::move(v); t.objectives = std::move(o); return t; }
+    static Targeter delta_v(Propagator p, std::vector<Objective> o) { return new_(std::move(p), {Variable::from(Vary::VelocityX), Variable::from(Vary::VelocityY), Variable::from(Vary::VelocityZ)}, std::move(o)); }
+    static Targeter delta_r(Propagator p, std::vector<Objective> o) { return new_(std::move(p), {Variable::from(Vary::PositionX), Variable::from(Vary::PositionY), Variable::from(Vary::PositionZ)}, std::move(o)); }
+    static Targeter vnc(Propagator p, std::vector<Objective> o) { Targeter t = delta_v(std::move(p), std::move(o)); t.correction_frame = TargetFrame::VNC; return t; }
+    static Targeter vnc_with_components(Propagator p, std::vector<Variable> v, std::vector<Objective> o) { Targeter t = new_(std::move(p), std::move(v), std::move(o)); t.correction_frame = TargetFrame::VNC; return t; }
+
+    nyxb_target_config config() const {
+        if (variables.size() > 6 || objectives.size() > 6) throw TargetingError("UnsupportedProblem", 0, "at most 6 variables and 6 objectives");
+        nyxb_target_config c{};
+        c.n_vars = (int32_t)variables.size(); c.n_objs = (int32_t)objectives.size(); c.correction_frame = (int32_t)correction_frame; c.iterations = iterations;
+        for (size_t j = 0; j < variables.size(); ++j) {
+            const Variable& v = variables[j];
+            c.vars[j] = nyxb_tgt_variable{(int32_t)v.component, 0, v.perturbation, v.init_guess, v.max_step, v.max_value, v.min_value};
+        }
+        for (size_t i = 0; i < objectives.size(); ++i) {
+            const Objective& o = objectives[i];
+            c.objs[i] = nyxb_tgt_objective{o.parameter, 0, o.desired_value, o.tolerance, o.multiplicative_factor, o.additive_factor};
+        }
+        return c;
+    }
+
+    // every state's problem in one call; the states share a frame, their epochs may differ
+    TargeterEnsembleSolution try_achieve_from_many(const std::vector<Spacecraft>& v, int64_t correction_epoch_ns, int64_t achievement_epoch_ns) const {
+        return run(config(), v, correction_epoch_ns, achievement_epoch_ns);
+    }
+    TargeterSolution try_achieve_from(const Spacecraft& s, int64_t correction_epoch_ns, int64_t achievement_epoch_ns) const {
+        return try_achieve_from_many({s}, correction_epoch_ns, achievement_epoch_ns).solution(0);
+    }
+
+    // Targeter::apply (targeter.rs:257-351): the corrected state propagated to the achievement epoch, every objective's unscaled error
+    // within its tolerance, else TargetingError "Verification".  The check is a call with no iteration and unit factors from the
+    // corrected state, so the objectives are evaluated by the same code as the targeting.
+    Spacecraft apply(const TargeterSolution& sol) const {
+        nyxb_target_config c = config();
+        c.iterations = 0;
+        for (int j = 0; j < c.n_vars; ++j) c.vars[j].init_guess = 0.0;
+        for (int i = 0; i < c.n_objs; ++i) { c.objs[i].multiplicative_factor = 1.0; c.objs[i].additive_factor = 0.0; }
+        const int64_t t_c = sol.corrected_state.epoch(), t_f = sol.achieved_state.epoch();
+        TargeterEnsembleSolution e = run(c, {sol.corrected_state}, t_c, t_f);
+        const int32_t st = e.status[0] & 0xFF;
+        if (st != 0 && st < NYXB_ERR_TGT_TOO_MANY_ITERATIONS) throw PropagationError(e.status[0]);
+        std::string msg;
+        for (int i = 0; i < c.n_objs; ++i)
+            if (!(std::fabs(e.errors[(size_t)i]) <= c.objs[i].tolerance))
+                msg += "objective " + std::to_string(i) + " error " + std::to_string(e.errors[(size_t)i]) + "; ";
+        if (!msg.empty()) throw TargetingError("Verification", e.status[0], msg);
+        return detail::unpack(sol.corrected_state, e.achieved, std::vector<int64_t>{t_f}, 1, 0);
+    }
+
+  private:
+    TargeterEnsembleSolution run(const nyxb_target_config& c, const std::vector<Spacecraft>& v, int64_t t_c, int64_t t_f) const {
+        if (v.empty()) throw std::runtime_error("no states");
+        auto eng = detail::make_engine(prop.dynamics, v[0].frame, almanac, prop.method, prop.opts, prop.mode, prop.device);
+        if (prop.kernel != NYXB_KERNEL_AUTO && nyxb_engine_set_kernel(eng.get(), prop.kernel) != NYXB_RC_OK)
+            throw std::runtime_error(std::string("nyxb_engine_set_kernel: ") + nyxb_last_error());
+        detail::Soa soa(v);
+        const size_t n = v.size();
+        TargeterEnsembleSolution e;
+        e.states = v; e.correction_epoch_ns = t_c; e.achievement_epoch_ns = t_f; e.n_vars = (size_t)c.n_vars; e.n_objs = (size_t)c.n_objs;
+        e.corrected.resize(9 * n); e.achieved.resize(9 * n); e.correction.resize(e.n_vars * n); e.errors.resize(e.n_objs * n);
+        e.iterations.resize(n); e.status.resize(n);
+        const int32_t rc = nyxb_target_batch(eng.get(), &c, n, soa.state.data(), soa.consts.data(), soa.epoch.data(), t_c, t_f, e.corrected.data(),
+                                             e.achieved.data(), e.correction.data(), e.errors.data(), e.iterations.data(), e.status.data());
+        if (rc != NYXB_RC_OK) throw std::runtime_error(std::string("nyxb_target_batch: ") + nyxb_last_error());
+        return e;
+    }
+};
+
 }  // namespace nyxb

@@ -25,5 +25,6 @@ from .od import (BatchLeastSquares, BLSEnsembleSolution, BLSSolution, BLSSolver,
 from .od import AER_TYPES, InterlinkTxSpacecraft, PositionDevice, simulate_interlink, simulate_position_fixes
 from .propagator import (Engine, ErrorControl, IntegrationDetails, IntegratorMethod, IntegratorOptions, PropagationError,
                          PropInstance, Propagator)
+from .targeter import (Objective, Targeter, TargeterEnsembleSolution, TargeterSolution, TargetingError, Variable, Vary)
 
 __all__ = [n for n in dir() if not n.startswith("_")]

@@ -24,6 +24,9 @@ RK89, DP78, DP45, RK4, CK45, V56 = range(6)
 # enum nyxb_status
 OK, ERR_PROP_MATH, ERR_FUEL_EXHAUSTED, ERR_MASSLESS, ERR_EPHEMERIS, ERR_EVENT_NOT_FOUND = range(6)
 WARN_MAX_ATTEMPTS = 0x100
+ERR_TGT_TOO_MANY_ITERATIONS, ERR_TGT_CORRECTION_INEFFECTIVE, ERR_TGT_SINGULAR_JACOBIAN, ERR_TGT_NON_FINITE = 13, 14, 15, 16
+# enum nyxb_tgt_frame
+TGT_FRAME_NONE, TGT_FRAME_VNC, TGT_FRAME_RIC = 0, 1, 2
 # enum nyxb_mode
 MODE_STRICT, MODE_FAST = 0, 1
 # enum nyxb_event_kind
@@ -363,6 +366,40 @@ class BlsOutputsC(C.Structure):
     ]
 
 
+class TgtVariableC(C.Structure):
+    _fields_ = [
+        ("component", C.c_int32),
+        ("_pad", C.c_int32),
+        ("perturbation", C.c_double),
+        ("init_guess", C.c_double),
+        ("max_step", C.c_double),
+        ("max_value", C.c_double),
+        ("min_value", C.c_double),
+    ]
+
+
+class TgtObjectiveC(C.Structure):
+    _fields_ = [
+        ("parameter", C.c_int32),
+        ("_pad", C.c_int32),
+        ("desired", C.c_double),
+        ("tolerance", C.c_double),
+        ("multiplicative_factor", C.c_double),
+        ("additive_factor", C.c_double),
+    ]
+
+
+class TargetConfigC(C.Structure):
+    _fields_ = [
+        ("n_vars", C.c_int32),
+        ("n_objs", C.c_int32),
+        ("correction_frame", C.c_int32),
+        ("iterations", C.c_int32),
+        ("vars", TgtVariableC * 6),
+        ("objs", TgtObjectiveC * 6),
+    ]
+
+
 DETAILS_DTYPE = np.dtype(
     [
         ("step_ns", "<i8"),
@@ -499,6 +536,8 @@ def _declare(lib):
     lib.nyxb_engine_set_tx_positions.argtypes = [vp, C.c_int32]
     lib.nyxb_engine_set_tx_tuning.restype = C.c_int32
     lib.nyxb_engine_set_tx_tuning.argtypes = [vp, C.c_int32, C.c_int32]
+    lib.nyxb_target_batch.restype = C.c_int32
+    lib.nyxb_target_batch.argtypes = [vp, C.POINTER(TargetConfigC), C.c_size_t, vp, vp, vp, C.c_int64, C.c_int64, vp, vp, vp, vp, vp, vp]
     lib.nyxb_abi_version.restype = C.c_int32
     lib.nyxb_abi_version.argtypes = []
     lib.nyxb_last_error.restype = C.c_char_p
@@ -550,6 +589,7 @@ EXPORTED_SYMBOLS = [
     "nyxb_last_error",
     "nyxb_od_interlink_batch",
     "nyxb_od_interlink_smooth_batch",
+    "nyxb_target_batch",
 ]
 
 

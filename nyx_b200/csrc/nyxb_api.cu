@@ -16,6 +16,7 @@
 #include "nyxb_device.cuh"
 #include "nyxb_od.cuh"
 #include "nyxb_tableaux.h"
+#include "nyxb_target_dev.h"
 
 // kernels (nyxb_kernels.cu built twice, nyxb_coop.cu)
 extern "C" cudaError_t nyxb_launch_thread_strict(const DevSetup*, size_t, const double*, const double*, const long long*,
@@ -40,6 +41,7 @@ static_assert(sizeof(nyxb_bls_config) == 80 && sizeof(nyxb_bls_outputs) == 72, "
 static_assert(sizeof(nyxb_od_records) == 64 && sizeof(nyxb_smooth_outputs) == 48, "ABI layout");
 static_assert(sizeof(nyxb_position_device) == 64 && sizeof(nyxb_position_arc) == 32 && sizeof(nyxb_aer_station) == 256, "ABI layout");
 static_assert(sizeof(nyxb_interlink_tx) == 56, "ABI layout");
+static_assert(sizeof(nyxb_tgt_variable) == 48 && sizeof(nyxb_tgt_objective) == 40 && sizeof(nyxb_target_config) == 544, "ABI layout");
 
 static thread_local std::string g_err;
 static void set_err(const std::string& s) { g_err = s; }
@@ -531,14 +533,22 @@ static int32_t launch(nyxb_engine* e, size_t n, const double* state, const doubl
     return NYXB_RC_OK;
 }
 
+// The family a launch of n trajectories runs: TRANSPOSED, or COOP / THREAD with `lanes` lanes per trajectory (1 for THREAD)
+static int launch_family(const nyxb_engine* e, size_t n, int& lanes) {
+    lanes = 1;
+    if (pick_kernel(e, n) == NYXB_KERNEL_TRANSPOSED) return NYXB_KERNEL_TRANSPOSED;
+    lanes = pick_lanes(e, n);
+    if (e->kernel == NYXB_KERNEL_THREAD) lanes = 1;
+    if (e->kernel == NYXB_KERNEL_COOP && lanes == 1 && e->S.has_grav) lanes = (e->S.grav.N >= 48) ? 32 : ((e->S.grav.N >= 30) ? 16 : 8);
+    return lanes > 1 ? NYXB_KERNEL_COOP : NYXB_KERNEL_THREAD;
+}
+
 static int32_t launch_inner(nyxb_engine* e, size_t n, const double* state, const double* consts, const int64_t* epoch0,
                             int64_t end_epoch, int64_t* step_io, double* out_state, int64_t* out_epoch,
                             nyxb_details* out_details, int32_t* out_status, const DevSink& sink, cudaStream_t stream) {
-    if (pick_kernel(e, n) == NYXB_KERNEL_TRANSPOSED)
+    int lanes;
+    if (launch_family(e, n, lanes) == NYXB_KERNEL_TRANSPOSED)
         return launch_tx(e, n, state, consts, epoch0, end_epoch, step_io, out_state, out_epoch, out_details, out_status, sink, stream);
-    int lanes = pick_lanes(e, n);
-    if (e->kernel == NYXB_KERNEL_THREAD) lanes = 1;
-    if (e->kernel == NYXB_KERNEL_COOP && lanes == 1 && e->S.has_grav) lanes = (e->S.grav.N >= 48) ? 32 : ((e->S.grav.N >= 30) ? 16 : 8);
     e->last_kernel = lanes > 1 ? NYXB_KERNEL_COOP : NYXB_KERNEL_THREAD;
     cudaError_t err;
     if (lanes > 1 && e->mode == NYXB_MODE_STRICT) {
@@ -1536,6 +1546,125 @@ extern "C" int32_t nyxb_od_bls_evaluate_batch(nyxb_engine* eng, const nyxb_bls_c
     bl.evaluate = 1;
     return od_bls_run(eng, cfg, n_stations, stations, arc, n, state_soa, consts_soa, epoch0_ns, bl, nullptr, nullptr, nullptr, nullptr,
                       rms, nullptr, nullptr, nullptr, status);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Impulsive targeting (Targeter::try_achieve_fd, md/opti/raphson_finite_diff.rs:41-747): update kernels in nyxb_target.cu.
+// ---------------------------------------------------------------------------------------------------------------------
+namespace {
+bool target_config_ok(const nyxb_target_config& c) {
+    if (c.n_vars < 1 || c.n_vars > 6 || c.n_objs < 1 || c.n_objs > 6) { set_err("n_vars and n_objs must be 1..6"); return false; }
+    if (c.correction_frame < NYXB_TGT_FRAME_NONE || c.correction_frame > NYXB_TGT_FRAME_RIC) { set_err("unknown correction frame"); return false; }
+    if (c.iterations < 0) { set_err("iterations must not be negative"); return false; }
+    for (int j = 0; j < c.n_vars; ++j) {
+        const nyxb_tgt_variable& v = c.vars[j];
+        if (v.component < NYXB_VARY_POSITION_X || v.component > NYXB_VARY_VELOCITY_Z) { set_err("unknown variable component"); return false; }
+        if (c.correction_frame != NYXB_TGT_FRAME_NONE && v.component < NYXB_VARY_VELOCITY_X) {
+            set_err("FrameError: a position variable cannot be corrected in a local frame");
+            return false;
+        }
+        // Variable::valid (target_variable.rs:143-168)
+        if (v.max_step < 0.0 || v.max_value < 0.0 || v.min_value > v.max_value) { set_err("VariableError: bad max step or bounds"); return false; }
+        if (!(std::isfinite(v.perturbation) && v.perturbation != 0.0)) { set_err("a perturbation must be finite and nonzero"); return false; }
+    }
+    for (int i = 0; i < c.n_objs; ++i)
+        if (c.objs[i].parameter < 0 || c.objs[i].parameter >= NYXB_TGT_N_PARAMS) { set_err("unknown objective parameter"); return false; }
+    return true;
+}
+
+// Fix the kernel family and lane count that launch_inner would pick for n trajectories, so that every launch of a call uses it.
+struct FamilyPin {
+    nyxb_engine* e;
+    int kernel, lanes;
+    FamilyPin(nyxb_engine* eng, size_t n) : e(eng), kernel(eng->kernel), lanes(eng->lanes) {
+        int l;
+        e->kernel = launch_family(e, n, l);
+        if (e->kernel != NYXB_KERNEL_TRANSPOSED) e->lanes = l;
+    }
+    ~FamilyPin() { e->kernel = kernel; e->lanes = lanes; }
+};
+}  // namespace
+
+extern "C" int32_t nyxb_target_batch(nyxb_engine* eng, const nyxb_target_config* cfg, size_t n, const double* state_soa,
+                                     const double* consts_soa, const int64_t* epoch0_ns, int64_t correction_epoch_ns,
+                                     int64_t achievement_epoch_ns, double* out_corrected_soa, double* out_achieved_soa,
+                                     double* out_correction, double* out_errors, int32_t* out_iterations, int32_t* out_status) {
+    if (!eng || !cfg || !state_soa || !consts_soa || !epoch0_ns || !out_corrected_soa || !out_achieved_soa || !out_correction ||
+        !out_errors || !out_iterations || !out_status) {
+        set_err("null argument");
+        return NYXB_RC_BAD_ARG;
+    }
+    if (!target_config_ok(*cfg)) return NYXB_RC_BAD_ARG;
+    // problem and slab indices are int on the device: n (n_vars + 1) must fit
+    if (n > (size_t)INT32_MAX / 7) { set_err("too many problems"); return NYXB_RC_BAD_ARG; }
+    if (eng->S.state_center >= 0) { set_err("targeting takes states in the integration frame"); return NYXB_RC_UNSUPPORTED; }
+    if (n == 0) return NYXB_RC_OK;
+    cudaStream_t st;
+    if (int32_t rc = od_stream(eng, st)) return rc;
+    const nyxb_target_config& c = *cfg;
+    const size_t V = (size_t)c.n_vars, O = (size_t)c.n_objs, W = V + 1, M = n * W;
+    const double mu = eng->S.mu_central;
+    DevBufs B;
+    TgtDev t{};
+    t.n = n;
+    const double* d_state = B.put(state_soa, 9 * n, st);
+    t.consts = B.put(consts_soa, 4 * n, st);
+    const long long* d_epoch0 = B.put((const long long*)epoch0_ns, n, st);
+    t.start = B.alloc<double>(9 * n); t.epoch_c = B.alloc<long long>(n); t.xi = B.alloc<double>(6 * n); t.total = B.alloc<double>(V * n);
+    t.err = B.alloc<double>(O * n); t.prev_norm = B.alloc<double>(n); t.achieved = B.alloc<double>(9 * n); t.corrected = B.alloc<double>(9 * n);
+    t.iters = B.alloc<int>(n); t.status = B.alloc<int>(n); t.flag = B.alloc<int>(n);
+    int* idx[2] = {B.alloc<int>(n), B.alloc<int>(n)};
+    int* d_count = B.alloc<int>(1);
+    t.idx = idx[0];
+    t.l_state = B.alloc<double>(9 * M); t.l_consts = B.alloc<double>(4 * M); t.l_epoch = B.alloc<long long>(M);
+    t.o_state = B.alloc<double>(9 * M); t.o_status = B.alloc<int>(M);
+    long long* o_epoch = B.alloc<long long>(M);
+    nyxb_details* o_det = B.alloc<nyxb_details>(M);
+    size_t temp_bytes = 0;
+    CUDA_TRY(nyxb_tgt_compact(nullptr, &temp_bytes, idx[0], t.flag, idx[1], d_count, (int)n, st));
+    void* temp = B.alloc<unsigned char>(temp_bytes);
+    if (int32_t rc = B.check()) return rc;
+
+    FamilyPin pin(eng, M);
+    int cur = 0;
+    int A = 0;
+    auto compact = [&](int count) -> int32_t {
+        CUDA_TRY(nyxb_tgt_compact(temp, &temp_bytes, idx[cur], t.flag, idx[cur ^ 1], d_count, count, st));
+        CUDA_TRY(cudaMemcpyAsync(&A, d_count, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        cur ^= 1;
+        eng->launches += 1;
+        return NYXB_RC_OK;
+    };
+    CUDA_TRY(cudaEventRecord(eng->ev0, st));
+    // xi_start: the states at the correction epoch, from opts.init_step (the slab's first n slots serve as the outputs)
+    if (int32_t rc = launch(eng, n, d_state, t.consts, (const int64_t*)d_epoch0, correction_epoch_ns, nullptr, t.o_state,
+                            (int64_t*)o_epoch, o_det, t.o_status, DevSink{}, st))
+        return rc;
+    CUDA_TRY(nyxb_tgt_launch_init(t, c, t.o_state, o_epoch, t.o_status, st));
+    eng->launches += 1;
+    if (int32_t rc = compact((int)n)) return rc;
+    while (A > 0) {
+        const size_t m = (size_t)A * W;
+        CUDA_TRY(nyxb_tgt_launch_stage(t, c, A, idx[cur], st));
+        eng->launches += 1;
+        if (int32_t rc = launch(eng, m, t.l_state, t.l_consts, (const int64_t*)t.l_epoch, achievement_epoch_ns, nullptr, t.o_state,
+                                (int64_t*)o_epoch, o_det, t.o_status, DevSink{}, st))
+            return rc;
+        CUDA_TRY(nyxb_tgt_launch_update(t, c, mu, A, idx[cur], st));
+        eng->launches += 1;
+        if (int32_t rc = compact(A)) return rc;
+    }
+    CUDA_TRY(nyxb_tgt_launch_finish(t, c, st));
+    eng->launches += 1;
+    CUDA_TRY(cudaEventRecord(eng->ev1, st));
+    CUDA_TRY(get(out_corrected_soa, t.corrected, 9 * n, st));
+    CUDA_TRY(get(out_achieved_soa, t.achieved, 9 * n, st));
+    CUDA_TRY(get(out_correction, t.total, V * n, st));
+    CUDA_TRY(get(out_errors, t.err, O * n, st));
+    CUDA_TRY(get(out_iterations, t.iters, n, st));
+    CUDA_TRY(get(out_status, t.status, n, st));
+    return od_finish(eng);
 }
 
 extern "C" int32_t nyxb_mvn_sample_dev(int32_t device, uint64_t seed, uint64_t first_index, size_t n, const double* template_state,

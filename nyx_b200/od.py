@@ -61,6 +61,7 @@ class KalmanVariant(enum.IntEnum):
 class LocalFrame(enum.IntEnum):
     Inertial = 0
     RIC = 1
+    VNC = 2
 
 
 class ODError(RuntimeError):
@@ -456,6 +457,11 @@ class ProcessNoise3D:
     disable_time: int
     local_frame: Optional[LocalFrame] = None
 
+    def __post_init__(self):
+        # the SNC packing (config_c) knows RIC and inertial only; it would treat any other frame as inertial
+        if self.local_frame is not None and self.local_frame not in (LocalFrame.Inertial, LocalFrame.RIC):
+            raise ODError(f"process noise in the {LocalFrame(self.local_frame).name} frame is not supported (RIC or inertial)")
+
     @classmethod
     def from_diagonal(cls, values, disable_time: int, local_frame: Optional[LocalFrame] = None):
         v = np.asarray(values, dtype=np.float64)
@@ -476,6 +482,16 @@ def dcm_ric_to_inertial(orbit: Orbit) -> np.ndarray:
     ch = h / np.linalg.norm(h)
     ih = np.cross(ch, rh)
     return np.column_stack([rh, ih, ch])
+
+
+def dcm_vnc_to_inertial(orbit: Orbit) -> np.ndarray:
+    """Columns V, N, C (anise `Orbit::dcm_to_inertial(LocalFrame::VNC)`): V = v/|v|, N = h/|h|, C = V x N; the convention of the
+    targeter's correction frame (nyx_b200/csrc/nyxb_target.h)."""
+    r, v = orbit.radius_km, orbit.velocity_km_s
+    vh = v / np.linalg.norm(v)
+    h = np.cross(r, v)
+    nh = h / np.linalg.norm(h)
+    return np.column_stack([vh, nh, np.cross(vh, nh)])
 
 
 @dataclass
@@ -509,7 +525,7 @@ class KfEstimate:
 @dataclass
 class SpacecraftUncertainty:
     """sc_uncertainty.rs:36-138 (defaults included).  As coded the covariance is rotated as D^T C D with D = the
-    local->inertial state DCM; the rotation-rate block of the RIC state DCM is taken as zero here (anise's
+    local->inertial state DCM (RIC or VNC); the rotation-rate block of the local state DCM is taken as zero here (anise's
     `rot_mat_dt` is not in the tree)."""
 
     nominal: Spacecraft
@@ -529,7 +545,12 @@ class SpacecraftUncertainty:
                 self.coeff_drag, self.mass_kg]
         if any(v < 0.0 for v in vals):
             raise ODError("uncertainties must be positive")
-        d3 = dcm_ric_to_inertial(self.nominal.orbit) if self.frame == LocalFrame.RIC else np.eye(3)
+        if self.frame == LocalFrame.RIC:
+            d3 = dcm_ric_to_inertial(self.nominal.orbit)
+        elif self.frame == LocalFrame.VNC:
+            d3 = dcm_vnc_to_inertial(self.nominal.orbit)
+        else:
+            d3 = np.eye(3)
         d6 = np.zeros((6, 6))
         d6[:3, :3] = d3
         d6[3:, 3:] = d3

@@ -41,6 +41,8 @@ class StateParameter(enum.Enum):
     Hmag = "Hmag (km^2/s)"
     ApoapsisRadius = "ApoapsisRadius (km)"
     PeriapsisRadius = "PeriapsisRadius (km)"
+    C3 = "C3 (km^2/s^2)"
+    Declination = "Declination (deg)"
     # md/param.rs:172-196 Display names
     Cd = "cd"
     Cr = "cr"
@@ -119,12 +121,16 @@ def evaluate(param: StateParameter, rv: np.ndarray, mu_km3_s2: float, template=N
         return rmag
     if param is StateParameter.Vmag:
         return vmag
+    if param is StateParameter.Declination:
+        return np.degrees(np.arcsin(r[2] / rmag))
     energy = 0.5 * vmag * vmag - mu_km3_s2 / rmag
     if param is StateParameter.Energy:
         return energy
     sma = -mu_km3_s2 / (2.0 * energy)
     if param is StateParameter.SemiMajorAxis:
         return sma
+    if param is StateParameter.C3:
+        return -mu_km3_s2 / sma
     if param is StateParameter.Period:
         return 2.0 * np.pi * np.sqrt(sma * sma * sma / mu_km3_s2)
     h = np.cross(r, v, axis=0)

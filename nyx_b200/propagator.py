@@ -258,6 +258,25 @@ class Engine:
             ret = ret + (crossings,)
         return ret
 
+    def target_batch(self, cfg_c: abi.TargetConfigC, state_soa, consts_soa, epoch0_ns, correction_epoch_ns: int, achievement_epoch_ns: int):
+        """`nyxb_target_batch`: `Targeter::try_achieve_fd` for n problems sharing the two epochs.  Returns a dict of corrected[9][n],
+        achieved[9][n], correction[n_vars][n], errors[n_objs][n], iterations[n], status[n]."""
+        state_soa = np.ascontiguousarray(state_soa, dtype=np.float64)
+        consts_soa = np.ascontiguousarray(consts_soa, dtype=np.float64)
+        epoch0_ns = np.ascontiguousarray(epoch0_ns, dtype=np.int64)
+        n = state_soa.shape[1]
+        if state_soa.shape != (9, n) or consts_soa.shape != (4, n) or epoch0_ns.shape != (n,):
+            raise ValueError("expected state[9][n], consts[4][n], epoch0[n]")
+        out = {"corrected": np.empty((9, n)), "achieved": np.empty((9, n)), "correction": np.empty((max(cfg_c.n_vars, 0), n)),
+               "errors": np.empty((max(cfg_c.n_objs, 0), n)), "iterations": np.zeros(n, dtype=np.int32), "status": np.zeros(n, dtype=np.int32)}
+        rc = self._lib.nyxb_target_batch(self._h, C.byref(cfg_c), n, state_soa.ctypes.data, consts_soa.ctypes.data, epoch0_ns.ctypes.data,
+                                         int(correction_epoch_ns), int(achievement_epoch_ns), out["corrected"].ctypes.data,
+                                         out["achieved"].ctypes.data, out["correction"].ctypes.data, out["errors"].ctypes.data,
+                                         out["iterations"].ctypes.data, out["status"].ctypes.data)
+        if rc != 0:
+            raise PropagationError(f"nyxb_target_batch rc={rc}: {abi.last_error()}")
+        return out
+
     def resample(self, query_epochs_ns, recording=None, n: Optional[int] = None):
         """`nyxb_traj_resample`: `Traj::at` (traj.rs:83-126) for every trajectory of a recording at every query epoch, one launch.
         `recording` = the (epochs[cap][n], states[6][cap][n], count[n]) tuple `propagate_batch(traj_capacity=...)` returned, or
